@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — crops/s through the VSM+VQA forward of the V* guided visual-search hot path (BASELINE.json metric) on N B200s.
+"""bench.py — crops/s through the VSM+VQA forward of the V* guided visual-search hot path (BASELINE.json metric) on N H100s.
 
     python bench.py --gpus 1 --steps 5 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
@@ -37,7 +37,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-FLOPS_PER_CROP = 5.00e12      # BASELINE.md §3 (T=320, g=6, KV-cached); roofline 289 crops/s/GPU at 1443 TF/s
+FLOPS_PER_CROP = 5.00e12      # BASELINE.md §3 (T=320, g=6, KV-cached)
 METRIC = "crops/s through the VSM+VQA forward (guided visual search hot path)"
 
 
@@ -62,6 +62,8 @@ def parse():
     ap.add_argument("--gemm-l2-hints", type=int, default=-1, help="A/B switch for vsb_gemm_set_l2_hints (-1 = library default)")
     ap.add_argument("--fuse-rope", type=int, default=-1, help="A/B switch for vsb_llama_set_fuse_rope (-1 = library default)")
     ap.add_argument("--depth", type=int, default=2, help="frontier batches in flight (1 = round-1 style synchronous rounds)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed (device-resident) step computed as DIR/<name>.npy, to compare two builds")
     return ap.parse_args()
 
 
@@ -70,7 +72,7 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return j["bf16_tflops_sustained"], j["hbm_gbs"], "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense BF16, HBM3), not a measured peak"
 
 
 def gemm_traffic_from_profile():
@@ -260,7 +262,7 @@ def torch_gpu_reference_sample(cfg, n_crops=3):
     batch 1, `generate(use_cache=False)` = one full CLIP + 7B pass per emitted token (5 here), lm_head and both query MLPs
     on all T rows, OWL-ViT, SAM decoder, heads, heat-map (VSM.py:438-553).  This is the "reference PyTorch-GPU" number the
     north-star's >= 10x is measured against; the reference itself cannot travel to the GPU box (Python sources under
-    /root/reference + transformers 4.31), so its restatement stands in.  Host preprocessing excluded (favours the baseline)."""
+    the reference + transformers 4.31), so its restatement stands in.  Host preprocessing excluded (favours the baseline)."""
     import torch
     from oracle import vsm_oracle as O
     from vstar_b200 import synth
@@ -465,10 +467,13 @@ def run_b200(args):
                 if resident:
                     if state["vqa_resident"] is None:
                         state["vqa_resident"] = stage_vqa(results)
-                    choices = [c for _, c in vqa.engine.option_losses_batch(state["vqa_resident"])]
+                    scored = vqa.engine.option_losses_batch(state["vqa_resident"])
+                    choices = [c for _, c in scored]
+                    state["last_losses"] = [l for l, _ in scored]
                 else:
                     choices = vqa_public(results)
             traj = [[tuple(s["bbox"]) for s in st.search_path] for st in states]
+            state["last"] = (results, traj, choices)
             if state["trajectories"] is None:
                 state["trajectories"] = (traj, choices)
             else:                       # in-run determinism check: every step walks the same trajectories and picks the same options
@@ -529,6 +534,8 @@ def run_b200(args):
         torch.cuda.profiler.stop()
     launches = _lib.launches - launches0
     gemm_flops, gemm_ms, gemm_n = ops.profile_end()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, st2)
     clocks = sampler.stop() if rank == 0 else None
     prefix_rows = engine._P
 
@@ -550,7 +557,7 @@ def run_b200(args):
         "gpu_launches": launches,
         "clocks": clocks,
         "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
-                     "traffic": traffic, "traffic_note": traffic_note, "kernel": "gemm_bf16_tcgen05_kernel", "launches": gemm_n,
+                     "traffic": traffic, "traffic_note": traffic_note, "kernel": "gemm_bf16_wgmma_kernel", "launches": gemm_n,
                      "gemm_time_share_of_step": gemm_ms / dev_ms if dev_ms > 0 else None,
                      "how": "sum(2*M*N*K) / sum(CUDA-event duration) over every GEMM launch of the timed region (VSM and VQA); peak = " + peak_src,
                      "whole_path_frac": value / world * flops_per_crop / (peak_tf * 1e12),
@@ -816,6 +823,31 @@ def run_b200(args):
     print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(d, state):
+    """The arrays a caller of the timed path receives from its last step: per search the final detection box, the bbox of the
+    final node, path length, success flag and the expanded-node trajectory (padded with -1); per VQA question the option
+    losses and the chosen option.  Inputs are seeded, so two runs with the same arguments compare output for output."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    results, traj, choices = state["last"]
+    out = {
+        "search_detection": np.array([r[0]["detection_result"].float().cpu().numpy() for r in results], dtype=np.float32),
+        "search_final_bbox": np.array([list(r[0]["bbox"]) for r in results], dtype=np.float64),
+        "search_path_length": np.array([float(r[1]) for r in results], dtype=np.float64),
+        "search_success": np.array([float(bool(r[2])) for r in results], dtype=np.float64),
+    }
+    n = max(len(t) for t in traj)
+    tr = np.full((len(traj), n, 4), -1.0, dtype=np.float64)
+    for i, t in enumerate(traj):
+        tr[i, :len(t)] = np.array(t, dtype=np.float64).reshape(-1, 4)
+    out["search_trajectory"] = tr
+    if choices is not None:
+        out["vqa_choice"] = np.array(choices, dtype=np.float64)
+        out["vqa_option_losses"] = np.array([np.asarray(l, dtype=np.float32) for l in state["last_losses"]], dtype=np.float32)
+    for name, arr in out.items():
+        np.save(os.path.join(d, name + ".npy"), arr)
 
 
 def vqa_probe(vqa, st2, peak_hbm, args):

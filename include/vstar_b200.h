@@ -1,4 +1,4 @@
-/* vstar_b200 C-ABI — the drop-in boundary of the B200-native V* (SEAL) visual-search hot path.
+/* vstar_b200 C-ABI — the drop-in boundary of the H100-native V* (SEAL) visual-search hot path.
  *
  * The reference (penghao-wu/vstar) is pure Python and has no FFI layer of its own: the boundary it
  * exposes is the Python API of visual_search.py / VSM.py (SURVEY.md §8b), mirrored by the host code in
@@ -23,7 +23,7 @@ extern "C" {
 #define VSB_EPI_RELU 3       /* SAM transformer MLP, text_hidden_fcs, hyper-network MLPs */
 #define VSB_EPI_SWIGLU 4     /* silu(gate)*up with gate/up rows interleaved in W (Llama MLP) */
 
-#define VSB_HEATMAP_MAX_BLOCKS 1184 /* 148 SMs x 8 */
+#define VSB_HEATMAP_MAX_BLOCKS 1184 /* blocks of the heat-map reduction (fixed: its summation order does not depend on the GPU) */
 
 const char* vsb_last_error(void);
 int vsb_version(void);
@@ -32,7 +32,7 @@ int vsb_version(void);
  * batching and frontier sharding (SURVEY.md section 8e).  0 (default): fastest kernel per shape (decode paths). */
 int vsb_set_batch_invariant(int on);
 
-/* C[M,N] = epi(A[M,K] . W[N,K]^T + bias[N]) (+ residual[M,N]); tcgen05/TMEM/TMA GEMM, bf16 operands, fp32
+/* C[M,N] = epi(A[M,K] . W[N,K]^T + bias[N]) (+ residual[M,N]); TMA + wgmma GEMM, bf16 operands, fp32
  * accumulate.  out_fp32: C/residual element type (0 = bf16, 1 = fp32).  Output-row remap (rows_per_group > 0):
  * row m -> (m / rows_per_group) * group_stride + group_offset + m % rows_per_group (used to scatter the 256
  * projected CLIP rows of each crop straight into the LLM input buffer; llava_arch.py:185-208).
@@ -48,7 +48,7 @@ int vsb_gemm_bf16(const void* A, long long lda, const void* W, long long ldw, vo
  * rowsq_in != NULL: output row m is scaled by rsqrt(sum_c rowsq_in[c*sq_ld + m] / K + eps) before bias / activation, i.e. A is the
  * UN-normalised residual stream and 1/rms is applied in the epilogue (no norm kernel, no normalised copy of the activations).
  * rowsq_out != NULL (bf16 output, N % 32 == 0): also writes the sum of squares of every stored 32-value chunk,
- * rowsq_out[(n/32)*sq_ld + row], which the next folded GEMM consumes with sq_in_chunks = N/32.  tcgen05 kernels for any M. */
+ * rowsq_out[(n/32)*sq_ld + row], which the next folded GEMM consumes with sq_in_chunks = N/32.  wgmma tile kernels for any M. */
 int vsb_gemm_rowscale_bf16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N, int K,
                            const void* bias, const void* residual, long long ldr, int epilogue, int rows_per_group, long long group_stride,
                            long long group_offset, const void* rowsq_in, int sq_in_chunks, float eps, void* rowsq_out, long long sq_ld,
@@ -69,12 +69,12 @@ int vsb_rowsq_bf16(const void* x, long long ldx, void* out_f32, int rows, int co
  * and returns the summed algorithmic flops (2*M*N*K), the summed event durations in ms and the launch count. */
 int vsb_gemm_profile_begin(void);
 int vsb_gemm_profile_end(double* flops, double* ms, long long* launches);
-/* testing / tuning hooks: force the kernel variant (1 = CUDA-core skinny kernel for M <= 8, 64/128/256 = single-CTA tile width, 512 = 2-CTA cta_group::2
- * 256x256 cluster tiles, 0 = auto) and the CTA count (0 = #SMs); tile-rasterisation band height in m-blocks (0 = auto) */
+/* testing / tuning hooks: force the kernel variant (1 = CUDA-core skinny kernel for M <= 8, 2 = mma.sync skinny kernel for M <= 16,
+ * 32/64/128/256 = wgmma tile width, 0 = auto) and the CTA count (0 = #SMs); tile-rasterisation band height in m-blocks (0 = auto) */
 int vsb_gemm_set_tuning(int force_bn, int max_ctas);
 int vsb_gemm_set_group_m(int group_m);
-/* L2 eviction hints of the 2-CTA kernel, bit mask: 1 = A tiles evict_last, 2 = W tiles evict_first, 8 = W tiles evict_last,
- * 4 = streaming (.cs) output stores; 0 = none.  The default is the setting that minimised dram__bytes on B200 (DESIGN.md). */
+/* L2 eviction hints of the tile kernel on large GEMMs (M, N >= 512, K >= 1024), bit mask: 1 = A tiles evict_last,
+ * 2 = W tiles evict_first, 8 = W tiles evict_last, 4 = streaming (.cs) output stores; 0 = none (default). */
 int vsb_gemm_set_l2_hints(int on);
 
 /* nn.LayerNorm over the last dim (fp32 stats), optional fused activation (VSB_EPI_NONE / VSB_EPI_GELU).
@@ -152,8 +152,8 @@ int vsb_attn_decode_bf16(const void* q, const void* k, const void* v, void* o, l
 int vsb_flash_attn_seg_bf16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,
                             long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk,
                             int D, float scale, const void* q_seg_i32, int seg_lo, void* stream);
-/* testing hook: 0 = auto (tcgen05 kernels for Sq >= 64, split-KV decode kernel for Sq <= 4, mma.sync kernel between),
- * 1 = mma.sync, 2 = tcgen05, 3 = tcgen05 single-tile kernel only, 4 = decode kernel */
+/* testing hook: 0 = auto (wgmma kernel for Sq >= 64, split-KV decode kernel for Sq <= 4, mma.sync kernel between),
+ * 1 = mma.sync, 2 = wgmma, 3 = wgmma with one query warpgroup per CTA only, 4 = decode kernel */
 int vsb_attn_set_impl(int impl);
 /* SAM two-way transformer attention, head_dim 16/32 (segment_anything/modeling/transformer.py:220-242)
  * and SEAL perceiver-resampler attention, head_dim 96 (LLaVA/llava/model/multimodal_projector/perceiver.py:25-77). */

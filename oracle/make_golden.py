@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — generates tests/golden/*.npz from the REAL reference.
 
-Run in the build container (where /root/reference is mounted):
+Run where a checkout of the reference is available (oracle/ref_shims.py, VSTAR_REFERENCE_ROOT):
 
     python -m oracle.make_golden
 
@@ -14,8 +14,8 @@ What it does
   4. asserts the CPU restatement (oracle/vsm_oracle.py) reproduces every one of
      them (fp32: rtol 1e-4 / atol 1e-5; ids / argmax / trajectories identical).
 
-The goldens are what pins the oracle on the GPU box, where /root/reference
-does not exist.
+The goldens are what pins the oracle wherever the reference is not available
+(every test run).
 """
 import json
 import os
@@ -385,7 +385,65 @@ def search_edge_cases():
     case_search("edge_odd", img_seed=28, w=1001, h=777, smallest=251, confidence_high=2.0)       # sizes not divisible by the grid
 
 
+def case_host_logic():
+    """results of the reference's host functions on the inputs of the drivers in tests/test_host_logic_vs_reference.py"""
+    import visual_search as RVS
+    import vstar_bench_eval as E
+    from LLaVA.llava import conversation as rc_vqa
+    from LLaVA.llava.mm_utils import tokenizer_image_object_token as ref_tok_obj
+    from VisualSearch.model.llava import conversation as rc_vsm
+    from VisualSearch.model.llava.mm_utils import tokenizer_image_token as ref_tok
+    from VisualSearch.utils.utils import expand2square as ref_e2s_vsm
+
+    from tests import test_host_logic_vs_reference as H
+    from tests.helpers import FakeNLP, NumpyScorer  # noqa: F401
+    from vstar_b200 import vsm
+    from vstar_b200.config import tiny_config
+    nlp = FakeNLP()
+    RVS.nlp = nlp
+    tok = vsm.SyntheticTokenizer(tiny_config())
+    prompts = []
+    for q in H.QUESTIONS:
+        conv = rc_vsm.conv_templates["llava_v1"].copy()
+        conv.append_message(conv.roles[0], ("<image>" + "\n" + q).replace("<image>", "<im_start><image><im_end>"))
+        conv.append_message(conv.roles[1], "")
+        llama2 = []
+        for use_se in (True, False):                 # the other template the CLI accepts (visual_search.py:48)
+            c2 = rc_vsm.conv_templates["llava_llama_2"].copy()
+            c2.messages = []
+            p2 = "<image>" + "\n" + q
+            if use_se:
+                p2 = p2.replace("<image>", "<im_start><image><im_end>")
+            c2.append_message(c2.roles[0], p2)
+            c2.append_message(c2.roles[1], "")
+            llama2.append(c2.get_prompt())
+        vqa_cases = []
+        for answer in (None, "the mug is red"):      # SEAL VQA LLM (vstar_bench_eval.py:79-85, :112-116, :136-139)
+            cv = rc_vqa.conv_templates["v1"].copy()
+            qs = "<image>" + "\n" + "Additional visual information to focus on: mug <object> at location [0.1,0.2,0.3,0.4]; dog <object>.\n" + q
+            cv.append_message(cv.roles[0], qs)
+            cv.append_message(cv.roles[1], answer)
+            vqa_cases.append([cv.get_prompt(), ref_tok_obj(cv.get_prompt(), tok, -200, return_tensors="pt").tolist()])
+        prompts.append(dict(vsm_v1=conv.get_prompt(), vsm_llama_2=llama2, vsm_ids=ref_tok(conv.get_prompt(), tok, return_tensors="pt").tolist(),
+                            vqa=vqa_cases))
+    gold = dict(
+        split_and_sub_patches=H.run_split_and_sub_patches(RVS.split_4subpatches, RVS.get_sub_patches),
+        refine_bbox_and_iou=H.run_refine_bbox_and_iou(RVS.refine_bbox, RVS.iou),
+        prioritize_pop_order=H.run_prioritize_pop_order(RVS.Prioritize),
+        prompts_and_token_splicing=prompts,
+        padding_and_patch_geometry=H.run_padding_and_patch_geometry(ref_e2s_vsm, E.expand2square, E.VQA_LLM.get_patch),
+        noun_chunks=H.run_noun_chunks(RVS.extract_noun_chunks, RVS.get_noun_chunks, RVS.tranverse, RVS.filter_chunk_list, nlp),
+        visualisation_files=H.run_visualisation_files(RVS.visual_search),
+    )
+    with open(H.GOLD, "w") as f:
+        json.dump(H.blockwise(gold), f, separators=(",", ":"))
+
+
 def main():
+    if os.environ.get("GOLDEN_ONLY") == "host_logic":
+        assert ref_shims.reference_available()
+        ref_shims.install(*hf_cfgs(O.tiny_config()))
+        return case_host_logic()
     if os.environ.get("GOLDEN_ONLY") == "search_edges":
         assert ref_shims.reference_available()
         ref_shims.install(*hf_cfgs(O.tiny_config()))
@@ -400,7 +458,7 @@ def main():
         assert ref_shims.reference_available()
         ref_shims.install(*hf_cfgs(O.tiny_config()))
         return case_bench_eval()
-    assert ref_shims.reference_available(), "needs /root/reference (build container only)"
+    assert ref_shims.reference_available(), "needs a checkout of the reference (VSTAR_REFERENCE_ROOT)"
     os.makedirs(GOLDEN_DIR, exist_ok=True)
     torch.set_num_threads(8)
     cfg = O.tiny_config()
@@ -430,6 +488,7 @@ def main():
     search_model_separated(m, sd, cfg)
     case_vqa("a", img_seed=41)
     case_bench_eval()
+    case_host_logic()
     print("golden vectors written to", GOLDEN_DIR)
 
 

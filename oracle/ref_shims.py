@@ -1,14 +1,13 @@
 """TEST INFRASTRUCTURE ONLY — import shims for the read-only reference tree.
 
-This module exists so that, IN THE BUILD CONTAINER (where /root/reference is
-mounted), the reference's own Python code can be imported under the installed
+This module exists so that, where a checkout of the reference is available
+(VSTAR_REFERENCE_ROOT), the reference's own Python code can be imported under the installed
 transformers 5.5 / torch 2.11 and used to (a) validate the CPU restatement in
 `oracle/vsm_oracle.py` and (b) generate the golden vectors committed under
 `tests/golden/` (see `oracle/make_golden.py`).
 
-Nothing under `vstar_b200/` may import this file.  /root/reference does not
-exist on the GPU box, so nothing in `-m gpu` tests / smoke() / bench.py may
-import it either.
+Nothing under `vstar_b200/` may import this file.  The tests, smoke() and bench.py
+never import it either: they read the committed goldens.
 
 Shims (SURVEY.md §8c):
   1. AutoConfig.register / AutoModelForCausalLM.register -> exist_ok=True

@@ -12,7 +12,7 @@ THE REFERENCE ITSELF: `oracle/make_golden.py` imports the reference's own
 / `visual_search()` (read-only, via `oracle/ref_shims.py`) in the build
 container, runs them on seeded random-init weights, and commits the results as
 `tests/golden/*.npz`; `tests/test_oracle_golden.py` checks this file against
-those vectors (and, when /root/reference is mounted, against the live
+those vectors (and, when the reference is available, against the live
 reference).
 
 The restatement is written with plain torch ops in the dtype of the weights it
@@ -23,7 +23,7 @@ State-dict key layout = the reference model's own `state_dict()` (which is
 also the checkpoint layout written by
 /root/reference/VisualSearch/merge_lora_weights_and_save_hf_model.py:143-151).
 
-Third-party arithmetic restated here (not under /root/reference): HF
+Third-party arithmetic restated here (not part of the reference): HF
 transformers `LlamaModel`, `CLIPVisionModel`, `OwlViTForObjectDetection` heads
 (reference pins transformers==4.31.0, requirements.txt:43); citations below use
 the installed 5.5.0 source paths `transformers/models/...` as in SURVEY.md §8a.

@@ -1,5 +1,8 @@
 """Test-only helpers (NOT product code): a numpy heat-map scorer so the search controller's ordering logic can be
 checked on a CPU-only box, and the deterministic stub VSM used by the committed search goldens."""
+import os
+import tempfile
+
 import numpy as np
 import torch
 
@@ -285,6 +288,10 @@ class StubVQA:
                     images_long, objects_long))
         self.log.append(("choice", key))
         return zlib.crc32(key.encode()) % len(options)
+
+
+# parity reports the GPU tests leave behind (informational; outside the source tree unless VSB_REPORT_DIR says otherwise)
+REPORT_DIR = os.environ.get("VSB_REPORT_DIR") or os.path.join(tempfile.gettempdir(), "vsb_reports")
 
 
 def make_bench_folder(root):

@@ -1,87 +1,12 @@
-"""The committed bench lines (profiles/r02_bench_*.json) carry every key of the bench.py contract, and bench.py's argument
-surface is the one the driver uses.  CPU only: nothing here runs the hot path."""
+"""bench.py's argument surface.  CPU only: nothing here runs the hot path."""
 import ast
-import glob
-import json
 import os
-import re
-
-import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-BASE_KEYS = {"metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
-             "dtype", "data", "config", "e2e"}
-OURS_KEYS = BASE_KEYS | {"gpu_launches", "clocks", "roofline", "cpu_baseline"}
-REJECT = {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
-
-
-def _line(path):
-    rows = [ln for ln in open(path).read().splitlines() if ln.strip().startswith("{")]
-    assert rows, path
-    return json.loads(rows[-1])
-
-
-def _ours():
-    """the headline lines (default flags); side runs with legs switched off (mid-round, free-running weak cue) are not contract lines"""
-    pat = re.compile(r"r02_bench_\dgpu(_steps\d+)?\.json$")
-    return sorted(p for p in glob.glob(os.path.join(ROOT, "profiles", "r02_bench_*gpu*.json")) if pat.search(p))
-
-
-@pytest.mark.parametrize("path", _ours(), ids=os.path.basename)
-def test_bench_line_contract(path):
-    d = _line(path)
-    need = OURS_KEYS if d["n_gpus"] == 1 else OURS_KEYS - {"cpu_baseline"}     # the CPU sample runs on rank 0 at N=1 only
-    assert need <= set(d), need - set(d)
-    assert d["metric"] == "crops_per_second" or "crops" in d["metric"]
-    assert d["unit"] == "crops/s" and d["higher_is_better"] is True and d["scaling"] == "weak"
-    assert d["dtype"] == "bf16" and "synthetic" in d["data"]
-    assert "workload" in d["config"] and "model" not in d["config"]
-    assert d["vs_baseline"] is None                                   # BASELINE.md publishes no crops/s number
-    assert d["warmup"] >= 3 and d["steps"] >= 1
-    # value is the whole-job aggregate: crops of all ranks / max-over-ranks step time
-    assert d["value"] == pytest.approx(d["crops_per_step"] * 1e3 / d["ms_per_step"], rel=1e-3)
-    e = d["e2e"]
-    assert e["unit"] == d["unit"] and e["h2d_bytes_per_step"] > 0 and e["d2h_bytes_per_step"] > 0
-    assert 0 < e["value"] < d["value"] * 1.02                          # host copies inside the timed region cannot make it faster
-    assert d["gpu_launches"] > 0
-    c = d["clocks"]
-    assert 0 < c["sm_mhz"] <= c["sm_max_mhz"] and not (REJECT & set(c["reasons"]))
-    r = d["roofline"]
-    assert r["bound"] in ("hbm", "tensor") and r["unit"] in ("GB/s", "TFLOP/s")
-    assert r["frac"] == pytest.approx(r["achieved"] / r["peak"], rel=1e-6) and 0 < r["frac"] < 1
-    assert r["traffic"] is None or r["traffic"] > 0
-    if d["n_gpus"] == 1:
-        b = d["cpu_baseline"]
-        assert b["kind"] in ("reference", "port") and b["cores"] >= 1 and b["value"] > 0 and b["sample"]
-
-
-def test_reference_arm_line():
-    d = _line(os.path.join(ROOT, "profiles", "r02_bench_reference_arm.json"))
-    assert d["impl"] == "reference" and BASE_KEYS | {"cpu_baseline"} <= set(d)
-    ours = _line(os.path.join(ROOT, "profiles", "r02_bench_1gpu.json"))
-    for k in ("metric", "unit", "higher_is_better"):
-        assert d[k] == ours[k]
-    head = ours["config"]["workload"].split(":")[0]                    # "BASELINE.json configs[2]"
-    assert d["config"]["workload"].startswith(head)
-    e = d["e2e"]
-    assert e["value"] == d["value"] == d["cpu_baseline"]["value"] and e["unit"] == d["unit"]
-    assert e["h2d_bytes_per_step"] == 0 and e["d2h_bytes_per_step"] == 0
-
-
-def test_scaling_lines_are_weak_and_monotone():
-    by_n = {}
-    for p in _ours():
-        d = _line(p)
-        by_n.setdefault(d["n_gpus"], []).append(d["value"])
-    ns = sorted(by_n)
-    assert ns[0] == 1 and len(ns) >= 2
-    best = [max(by_n[n]) for n in ns]
-    assert all(b > a for a, b in zip(best, best[1:]))
-
 
 def test_bench_argument_surface():
-    """--gpus / --steps / --warmup / --impl exist with the defaults the contract asks for (N=1, W >= 3)"""
+    """--gpus / --steps / --warmup / --impl / --dump-outputs exist with the expected defaults (N=1, W >= 3)"""
     tree = ast.parse(open(os.path.join(ROOT, "bench.py")).read())
     args = {}
     for node in ast.walk(tree):
@@ -90,5 +15,5 @@ def test_bench_argument_surface():
             kw = {k.arg: k.value for k in node.keywords}
             default = kw.get("default")
             args[name] = default.value if isinstance(default, ast.Constant) else None
-    assert {"--gpus", "--steps", "--warmup", "--impl"} <= set(args)
+    assert {"--gpus", "--steps", "--warmup", "--impl", "--dump-outputs"} <= set(args)
     assert args["--gpus"] == 1 and args["--warmup"] >= 3 and args["--steps"] >= 1

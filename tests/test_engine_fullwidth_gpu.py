@@ -7,6 +7,8 @@ import os
 
 import numpy as np
 import pytest
+
+from tests.helpers import REPORT_DIR
 import torch
 
 pytestmark = pytest.mark.gpu
@@ -64,8 +66,8 @@ def test_fullwidth_two_layer_model():
     top2 = ref_logits.topk(2, -1).values
     conf = (top2[:, 0] - top2[:, 1]) > 0.1
     assert torch.equal(am.cpu().long()[conf], ref_logits.argmax(-1)[conf])
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump({k: dict(err_new=v[0], err_ref_bf16=v[1]) for k, v in rep.items()}, open("gpurun_out/fullwidth_parity_report.json", "w"), indent=1)
+    os.makedirs(REPORT_DIR, exist_ok=True)
+    json.dump({k: dict(err_new=v[0], err_ref_bf16=v[1]) for k, v in rep.items()}, open(os.path.join(REPORT_DIR, "fullwidth_parity_report.json"), "w"), indent=1)
 
 
 def test_fulldepth_fullwidth_model():
@@ -131,8 +133,8 @@ def test_fulldepth_fullwidth_model():
                                 max_abs_logit_err=abs_err, min_top2_gap=float(gap.min()))
     rep["top_box_index"] = dict(new=int(out["pred_logits"][0].argmax()), fp32=int(o32["pred_logits"][0, :, 0].argmax()),
                                 bf16_ref=int(o16["pred_logits"][0, :, 0].argmax()))
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(rep, open("gpurun_out/fulldepth_parity_report.json", "w"), indent=1)
+    os.makedirs(REPORT_DIR, exist_ok=True)
+    json.dump(rep, open(os.path.join(REPORT_DIR, "fulldepth_parity_report.json"), "w"), indent=1)
     for name, v in rep.items():
         if "err_new" in v:
             floor = 5e-3 if name in ("hidden_loc", "seg_query", "det_query") else 1e-2

@@ -9,6 +9,8 @@ import os
 
 import numpy as np
 import pytest
+
+from tests.helpers import REPORT_DIR
 import torch
 
 pytestmark = pytest.mark.gpu
@@ -212,6 +214,6 @@ def test_cache_grows_instead_of_truncating(setup):
 
 
 def test_zz_write_report(setup):
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(REPORT, open("gpurun_out/engine_parity_report.json", "w"), indent=1)
+    os.makedirs(REPORT_DIR, exist_ok=True)
+    json.dump(REPORT, open(os.path.join(REPORT_DIR, "engine_parity_report.json"), "w"), indent=1)
     print(json.dumps(REPORT, indent=1))

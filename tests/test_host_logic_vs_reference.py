@@ -1,34 +1,39 @@
 """Differential tests of the host logic (integer geometry, priority queue order, prompt strings, placeholder splicing,
-padding, patch geometry) against the LIVE reference modules (visual_search.py:226-283,
-:378-389), on random boxes.  Runs only where /root/reference is mounted (the build container); the GPU box relies on the
-committed trajectories, which exercise the same functions end to end."""
+padding, patch geometry, noun chunks, visualisation files) against the reference modules (visual_search.py:226-283,
+:378-389), on random inputs.  Every check is a driver that takes the functions under test and returns JSON-able results;
+oracle/make_golden.py runs the drivers on the reference's own functions and stores their results (long lists as digests of
+blocks of 500 items) in tests/golden/host_logic_reference.json, and the tests run the same drivers on ours and compare."""
+import hashlib
+import json
 import os
 import queue
-import subprocess
 import sys
+import tempfile
 
 import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT) if ROOT not in sys.path else None
-from oracle import ref_shims  # noqa: E402
 
-pytestmark = pytest.mark.skipif(not ref_shims.reference_available(), reason="/root/reference not mounted")
-
-
-def load_reference():
-    """import shims patch transformers / torch globally, so the checks run in a child process (see `isolated`)"""
-    from oracle import vsm_oracle as O
-    from oracle.make_golden import hf_cfgs
-    ref_shims.install(*hf_cfgs(O.tiny_config()))
-    import visual_search as RVS          # the reference module
-    return RVS
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "host_logic_reference.json")
 
 
-def isolated(name):
-    r = subprocess.run([sys.executable, os.path.abspath(__file__), name], capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
+def jsonable(x):
+    return json.loads(json.dumps(x, default=lambda o: o.tolist() if hasattr(o, "tolist") else str(o)))
+
+
+def digest(b):
+    return hashlib.sha256(b).hexdigest()[:24]
+
+
+def blockwise(x, n=500):
+    """what the golden file stores: lists longer than n as one digest per n consecutive items, dicts key by key"""
+    if isinstance(x, dict):
+        return {k: blockwise(v, n) for k, v in x.items()}
+    if isinstance(x, list) and len(x) > n:
+        return [digest(json.dumps(x[i:i + n]).encode()) for i in range(0, len(x), n)]
+    return x
 
 
 def boxes(n, seed):
@@ -38,207 +43,191 @@ def boxes(n, seed):
         yield [int(rng.integers(0, 5000)), int(rng.integers(0, 5000)), w, h]
 
 
-def check_split_and_sub_patches():
-    ref = load_reference()
-    from vstar_b200 import visual_search as VS
-    n_14 = n_41 = 0
-    for b in list(boxes(3000, 1)) + [[0, 0, 100, 200], [0, 0, 200, 100], [3, 5, 7, 14], [3, 5, 14, 7], [0, 0, 1, 1], [0, 0, 2, 3]]:
-        nw, nh = VS.split_4subpatches(b)
-        assert (nw, nh) == ref.split_4subpatches(b)
-        n_14 += (nw, nh) == (1, 4)
-        n_41 += (nw, nh) == (4, 1)
-        got = VS.get_sub_patches(b, nw, nh)
-        want = ref.get_sub_patches(b, nw, nh)
-        assert list(got[0]) == list(want[0]) and got[1:] == want[1:]
-        # children tile the parent exactly (last row / column takes the remainder)
-        assert sum(p[2] * p[3] for p in got[0]) == b[2] * b[3]
-    assert n_14 > 100 and n_41 > 100
+SPLIT_BOXES = list(boxes(3000, 1)) + [[0, 0, 100, 200], [0, 0, 200, 100], [3, 5, 7, 14], [3, 5, 14, 7], [0, 0, 1, 1], [0, 0, 2, 3]]
+QUESTIONS = ["Please locate the red mug in this image.", "According to the common sense knowledge and possible visual cues, what is "
+             "the most likely location of the dog in the image?", "x"]
 
 
-def check_refine_bbox_and_iou():
-    ref = load_reference()
-    from vstar_b200 import visual_search as VS
+# ---------------------------------------------------------------- drivers (run on the reference by make_golden, on ours here)
+def run_split_and_sub_patches(split_4subpatches, get_sub_patches):
+    out = []
+    for b in SPLIT_BOXES:
+        nw, nh = split_4subpatches(b)
+        got = get_sub_patches(b, nw, nh)
+        out.append([[nw, nh], [list(got[0])] + list(got[1:])])
+    return jsonable(out)
+
+
+def run_refine_bbox_and_iou(refine_bbox, iou):
     rng = np.random.default_rng(2)
+    out = []
     for _ in range(2000):
         W, H = int(rng.integers(10, 4000)), int(rng.integers(10, 4000))
         b = [float(rng.uniform(-50, W)), float(rng.uniform(-50, H)), float(rng.uniform(1, W)), float(rng.uniform(1, H))]
-        assert VS.refine_bbox(list(b), W, H) == ref.refine_bbox(list(b), W, H)
         c = [float(rng.uniform(0, W)), float(rng.uniform(0, H)), float(rng.uniform(1, W)), float(rng.uniform(1, H))]
-        assert VS.iou(b, c) == ref.iou(b, c)
+        out.append([refine_bbox(list(b), W, H), iou(b, c)])
+    return jsonable(out)
 
 
-def check_prioritize_pop_order_with_ties():
-    ref = load_reference()
+def run_prioritize_pop_order(Prioritize):
     """the expansion order IS the heap order of (Prioritize(-score, item)) incl. its tie behaviour (no tiebreak key)"""
-    from vstar_b200 import visual_search as VS
     rng = np.random.default_rng(3)
+    out = []
     for trial in range(50):
         scores = np.round(rng.uniform(0, 1, 40), 1 if trial % 2 else 3).astype(np.float32)      # many exact ties
-        qa, qb = queue.PriorityQueue(), queue.PriorityQueue()
-        out_a, out_b = [], []
+        q, order = queue.PriorityQueue(), []
         for i, s in enumerate(scores):
-            qa.put(VS.Prioritize(-s, i))
-            qb.put(ref.Prioritize(-s, i))
+            q.put(Prioritize(-s, i))
             if i % 3 == 2:                    # interleave pops with pushes like the search does
-                out_a.append(qa.get().item)
-                out_b.append(qb.get().item)
-        while not qa.empty():
-            out_a.append(qa.get().item)
-            out_b.append(qb.get().item)
-        assert out_a == out_b
+                order.append(q.get().item)
+        while not q.empty():
+            order.append(q.get().item)
+        out.append(order)
+    return out
 
 
-def check_prompts_and_token_splicing():
-    """prompt strings of both conversation templates and the <image>/<object> placeholder splicing (they define T and the
-    255-row offset): ours vs the reference's conversation.py / mm_utils.py, with the synthetic word-hash tokenizer on both"""
-    load_reference()
-    from VisualSearch.model.llava import conversation as rc_vsm
-    from VisualSearch.model.llava.mm_utils import tokenizer_image_token as ref_tok
-    from LLaVA.llava import conversation as rc_vqa
-    from LLaVA.llava.mm_utils import tokenizer_image_object_token as ref_tok_obj
-    from vstar_b200 import vqa, vsm
-    from vstar_b200.config import tiny_config
-    tok = vsm.SyntheticTokenizer(tiny_config())
-    for q in ["Please locate the red mug in this image.", "According to the common sense knowledge and possible visual cues, what is "
-              "the most likely location of the dog in the image?", "x"]:
-        # VSM wrapper (visual_search.py:176-184)
-        conv = rc_vsm.conv_templates["llava_v1"].copy()
-        prompt = "<image>" + "\n" + q
-        prompt = prompt.replace("<image>", "<im_start><image><im_end>")
-        conv.append_message(conv.roles[0], prompt)
-        conv.append_message(conv.roles[1], "")
-        assert vsm.build_prompt(q, "llava_v1", True) == conv.get_prompt()
-        for use_se in (True, False):                 # the other template the CLI accepts (visual_search.py:48)
-            c2 = rc_vsm.conv_templates["llava_llama_2"].copy()
-            c2.messages = []
-            p2 = "<image>" + "\n" + q
-            if use_se:
-                p2 = p2.replace("<image>", "<im_start><image><im_end>")
-            c2.append_message(c2.roles[0], p2)
-            c2.append_message(c2.roles[1], "")
-            assert vsm.build_prompt(q, "llava_llama_2", use_se) == c2.get_prompt()
-        ours = vsm.tokenizer_image_token(conv.get_prompt(), tok)
-        theirs = ref_tok(conv.get_prompt(), tok, return_tensors="pt").tolist()
-        assert ours == theirs and ours.count(-200) == 1
-        # SEAL VQA LLM (vstar_bench_eval.py:79-85, :112-116, :136-139)
-        for answer in (None, "the mug is red"):
-            conv = rc_vqa.conv_templates["v1"].copy()
-            qs = "<image>" + "\n" + "Additional visual information to focus on: mug <object> at location [0.1,0.2,0.3,0.4]; dog <object>.\n" + q
-            conv.append_message(conv.roles[0], qs)
-            conv.append_message(conv.roles[1], answer)
-            assert vqa.build_prompt_v1(qs, answer) == conv.get_prompt()
-            ours = vqa.tokenizer_image_object_token(conv.get_prompt(), tok)
-            theirs = ref_tok_obj(conv.get_prompt(), tok, -200, return_tensors="pt").tolist()
-            assert ours == theirs and ours.count(-200) == 1 and ours.count(-300) == 2
-
-
-def check_padding_and_patch_geometry():
+def run_padding_and_patch_geometry(expand2square_vsm, expand2square_center, get_patch):
     """both expand2square variants (top-left paste for the VSM, centred for the VQA LLM) and VQA_LLM.get_patch"""
-    load_reference()
-    import vstar_bench_eval as E
-    from VisualSearch.utils.utils import expand2square as ref_e2s_vsm
     from tests.helpers import synth_image
-    from vstar_b200 import seal, vqa, vsm
-    rng = np.random.default_rng(5)
+    out = dict(vsm=[], center=[], patch=[])
     for i, (w, h) in enumerate([(300, 200), (200, 300), (256, 256), (1, 9), (513, 512)]):
         img = synth_image(50 + i, w, h)
         bg = (122, 116, 104)
-        assert np.array_equal(np.asarray(vsm.expand2square(img, bg)), np.asarray(ref_e2s_vsm(img, bg)))
-        a, la, ta = seal.expand2square_center(img, bg)
-        b, lb, tb = E.expand2square(img, bg)
-        assert (la, ta) == (lb, tb) and np.array_equal(np.asarray(a), np.asarray(b))
-    get_patch_ref = E.VQA_LLM.get_patch
-    get_patch = vqa.VQA_LLM.get_patch
+        out["vsm"].append(digest(np.ascontiguousarray(np.asarray(expand2square_vsm(img, bg))).tobytes()))
+        a, la, ta = expand2square_center(img, bg)
+        out["center"].append([la, ta, digest(np.ascontiguousarray(np.asarray(a)).tobytes())])
+    rng = np.random.default_rng(5)
     for _ in range(2000):
         W, H = int(rng.integers(50, 3000)), int(rng.integers(50, 3000))
         bbox = [float(rng.uniform(0, W)), float(rng.uniform(0, H)), float(rng.uniform(1, W)), float(rng.uniform(1, H))]
-        for scale in (None, 1.2, 0.5):
-            assert get_patch(None, bbox, W, H, patch_scale=scale) == get_patch_ref(None, bbox, W, H, patch_scale=scale)
+        out["patch"].append([get_patch(None, bbox, W, H, patch_scale=scale) for scale in (None, 1.2, 0.5)])
+    return jsonable(out)
 
 
-def check_noun_chunks():
-    """extract_noun_chunks / get_noun_chunks / filter_chunk_list (visual_search.py:54-112) with the SAME deterministic parser
-    on both sides (spaCy is not installed offline): random phrases from the rule parser's lexicon + hand-made trees"""
-    ref = load_reference()
-    from tests.helpers import FakeNLP, VQA_ANSWERS
-    from vstar_b200 import noun_chunks as NC
-    nlp = FakeNLP()
-    ref.nlp = nlp
+def noun_chunk_phrases():
+    from tests.helpers import VQA_ANSWERS, FakeNLP
     rng = np.random.default_rng(7)
     words = sorted(FakeNLP.NOUNS | FakeNLP.PRONS | FakeNLP.ADJS | FakeNLP.DETS | FakeNLP.PREPS | FakeNLP.RELS) + ["and", "somewhere", "high", "is"]
     phrases = [a.split("most likely to appear")[-1].strip().rstrip(".") for a in VQA_ANSWERS]
     for _ in range(3000):
         phrases.append(" ".join(rng.choice(words, size=int(rng.integers(1, 12)))))
-    n_multi = n_one = n_zero = 0
-    for ph in phrases:
-        got, want = NC.extract_noun_chunks(ph, nlp), ref.extract_noun_chunks(ph)
-        assert got == want, (ph, got, want)
-        n_multi += len(got) > 1
-        n_one += len(got) == 1
-        n_zero += len(got) == 0
-        doc = nlp(ph)
-        for t in doc:
-            assert NC.get_noun_chunks(t) == ref.get_noun_chunks(t) and NC.subtree_span(t) == ref.tranverse(t)
-    assert n_multi > 100 and n_one > 100 and n_zero > 10
+    return phrases
+
+
+def run_noun_chunks(extract_noun_chunks, get_noun_chunks, tranverse, filter_chunk_list, nlp):
+    """extract_noun_chunks / get_noun_chunks / filter_chunk_list (visual_search.py:54-112) with the SAME deterministic parser
+    on both sides (spaCy is not installed offline): random phrases from the rule parser's lexicon + hand-made trees.  The
+    per-token results are stored as one digest per phrase."""
+    out = dict(chunks=[], tokens=[], filtered=[])
+    for ph in noun_chunk_phrases():
+        out["chunks"].append(jsonable(extract_noun_chunks(ph)))
+        per_tok = [[jsonable(get_noun_chunks(t)), jsonable(tranverse(t))] for t in nlp(ph)]
+        out["tokens"].append(digest(json.dumps(per_tok).encode()))
+    rng = np.random.default_rng(7)
     for _ in range(2000):
         chunks = [tuple(sorted(rng.integers(0, 30, 2).tolist())) for _ in range(int(rng.integers(0, 8)))]
-        assert NC.filter_chunk_list(chunks) == ref.filter_chunk_list(chunks)
+        out["filtered"].append(jsonable(filter_chunk_list(chunks)))
+    return out
 
 
-def check_visualisation_files():
-    """visualize=True: the files visualize_search_path writes (visual_search.py:339-376) from the reference and from the product,
-    on the same stub search: same file names, byte-identical JPEGs and context_cue.txt"""
-    import tempfile
-    ref = load_reference()
-    from tests.helpers import FakeNLP, NumpyScorer, StubVSM, synth_image
-    from vstar_b200 import noun_chunks
-    from vstar_b200 import visual_search as VS
-    ref.nlp = FakeNLP()
-    noun_chunks.set_nlp(FakeNLP())
+def run_visualisation_files(visual_search):
+    """visualize=True: the files visualize_search_path writes (visual_search.py:339-376) on the same stub search: file names,
+    digests of the JPEG bytes and of context_cue.txt, path length and success flag"""
+    from tests.helpers import StubVSM, synth_image
+    out = []
     for seed, w, h, smallest, hot, kw in ((29, 640, 480, 224, None, dict(confidence_high=2.0, target_cue_threshold=9.5, target_cue_threshold_minimum=9.5)),
                                           (25, 700, 600, 224, "small", dict())):
         img = synth_image(seed, w, h)
-        with tempfile.TemporaryDirectory() as a, tempfile.TemporaryDirectory() as b:
-            ra = ref.visual_search(StubVSM(hot), img, "mug", [30, 40, 50, 60], smallest, visualize=True, save_path=a, **kw)
-            rb = VS.visual_search(StubVSM(hot), img, "mug", [30, 40, 50, 60], smallest, visualize=True, save_path=b, scorer=NumpyScorer(), **kw)
-            assert ra[1] == rb[1] and ra[2] == rb[2]
-            fa, fb = sorted(os.listdir(a)), sorted(os.listdir(b))
-            assert fa == fb and "whole_image.jpg" in fa and "context_cue.txt" in fa and any(f.endswith("_heatmap.jpg") for f in fa), (fa, fb)
-            for f in fa:
-                assert open(os.path.join(a, f), "rb").read() == open(os.path.join(b, f), "rb").read(), f
+        with tempfile.TemporaryDirectory() as d:
+            r = visual_search(StubVSM(hot), img, "mug", [30, 40, 50, 60], smallest, visualize=True, save_path=d, **kw)
+            files = sorted(os.listdir(d))
+            out.append(dict(path_length=jsonable(r[1]), success=jsonable(r[2]), files=files,
+                            digests=[digest(open(os.path.join(d, f), "rb").read()) for f in files]))
+    return out
+
+
+# ---------------------------------------------------------------- checks: our functions against the stored reference results
+@pytest.fixture(scope="module")
+def gold():
+    return json.load(open(GOLD))
+
+
+def check_split_and_sub_patches(gold):
+    from vstar_b200 import visual_search as VS
+    got = run_split_and_sub_patches(VS.split_4subpatches, VS.get_sub_patches)
+    assert blockwise(got) == gold["split_and_sub_patches"]
+    for b, ((nw, nh), (patches, *_)) in zip(SPLIT_BOXES, got):
+        assert sum(p[2] * p[3] for p in patches) == b[2] * b[3]     # children tile the parent (the last one takes the remainder)
+    shapes = [tuple(s) for s, _ in got]
+    assert shapes.count((1, 4)) > 100 and shapes.count((4, 1)) > 100
+
+
+def check_refine_bbox_and_iou(gold):
+    from vstar_b200 import visual_search as VS
+    assert blockwise(run_refine_bbox_and_iou(VS.refine_bbox, VS.iou)) == gold["refine_bbox_and_iou"]
+
+
+def check_prioritize_pop_order_with_ties(gold):
+    from vstar_b200 import visual_search as VS
+    assert blockwise(run_prioritize_pop_order(VS.Prioritize)) == gold["prioritize_pop_order"]
+
+
+def check_prompts_and_token_splicing(gold):
+    """prompt strings of both conversation templates and the <image>/<object> placeholder splicing (they define T and the
+    255-row offset): ours vs the reference's conversation.py / mm_utils.py, with the synthetic word-hash tokenizer on both"""
+    from vstar_b200 import vqa, vsm
+    from vstar_b200.config import tiny_config
+    tok = vsm.SyntheticTokenizer(tiny_config())
+    want = gold["prompts_and_token_splicing"]
+    for i, q in enumerate(QUESTIONS):
+        w = want[i]
+        p = vsm.build_prompt(q, "llava_v1", True)
+        assert p == w["vsm_v1"]
+        assert [vsm.build_prompt(q, "llava_llama_2", use_se) for use_se in (True, False)] == w["vsm_llama_2"]
+        ids = vsm.tokenizer_image_token(p, tok)
+        assert ids == w["vsm_ids"] and ids.count(-200) == 1
+        for j, answer in enumerate((None, "the mug is red")):
+            qs = "<image>" + "\n" + "Additional visual information to focus on: mug <object> at location [0.1,0.2,0.3,0.4]; dog <object>.\n" + q
+            pv = vqa.build_prompt_v1(qs, answer)
+            assert pv == w["vqa"][j][0]
+            ids = vqa.tokenizer_image_object_token(pv, tok)
+            assert ids == w["vqa"][j][1] and ids.count(-200) == 1 and ids.count(-300) == 2
+
+
+def check_padding_and_patch_geometry(gold):
+    from vstar_b200 import seal, vqa, vsm
+    got = run_padding_and_patch_geometry(vsm.expand2square, seal.expand2square_center, vqa.VQA_LLM.get_patch)
+    assert blockwise(got) == gold["padding_and_patch_geometry"]
+
+
+def check_noun_chunks(gold):
+    from tests.helpers import FakeNLP
+    from vstar_b200 import noun_chunks as NC
+    nlp = FakeNLP()
+    got = run_noun_chunks(lambda ph: NC.extract_noun_chunks(ph, nlp), NC.get_noun_chunks, NC.subtree_span, NC.filter_chunk_list, nlp)
+    want = gold["noun_chunks"]
+    for key in ("chunks", "tokens", "filtered"):
+        assert blockwise(got[key]) == want[key], key
+    n = [len(c) for c in got["chunks"]]
+    assert sum(k > 1 for k in n) > 100 and sum(k == 1 for k in n) > 100 and sum(k == 0 for k in n) > 10
+
+
+def check_visualisation_files(gold):
+    from tests.helpers import FakeNLP, NumpyScorer
+    from vstar_b200 import noun_chunks
+    from vstar_b200 import visual_search as VS
+    noun_chunks.set_nlp(FakeNLP())
+    got = run_visualisation_files(lambda *a, **k: VS.visual_search(*a, scorer=NumpyScorer(), **k))
+    assert blockwise(got) == gold["visualisation_files"]
+    for case in got:
+        f = case["files"]
+        assert "whole_image.jpg" in f and "context_cue.txt" in f and any(x.endswith("_heatmap.jpg") for x in f), f
 
 
 CHECKS = ["check_visualisation_files", "check_noun_chunks", "check_split_and_sub_patches", "check_refine_bbox_and_iou",
           "check_prioritize_pop_order_with_ties", "check_prompts_and_token_splicing", "check_padding_and_patch_geometry"]
 
 
-@pytest.fixture(scope="module")
-def live_results():
-    """all checks in ONE child process (the import shims patch transformers / torch globally, and importing the reference +
-    transformers costs ~15 s): the child prints one JSON object {check name: "ok" | traceback}"""
-    import json
-    r = subprocess.run([sys.executable, os.path.abspath(__file__), "ALL"], capture_output=True, text=True, timeout=900, cwd=ROOT)
-    lines = [ln for ln in r.stdout.splitlines() if ln.startswith("{")]
-    assert r.returncode == 0 and lines, r.stdout[-2000:] + r.stderr[-4000:]
-    return json.loads(lines[-1])
-
-
 @pytest.mark.parametrize("name", CHECKS)
-def test_against_live_reference(live_results, name):
-    assert live_results.get(name) == "ok", live_results.get(name)
-
-
-if __name__ == "__main__":
-    if sys.argv[1] == "ALL":
-        import json
-        import traceback
-        res = {}
-        for name in CHECKS:
-            try:
-                globals()[name]()
-                res[name] = "ok"
-            except Exception:
-                res[name] = traceback.format_exc()[-3000:]
-        print(json.dumps(res))
-    else:
-        globals()[sys.argv[1]]()
+def test_against_live_reference(gold, name):
+    globals()[name](gold)

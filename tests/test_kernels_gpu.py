@@ -1,4 +1,4 @@
-"""Per-kernel parity on a real B200: every C-ABI entry point against the same op in plain PyTorch
+"""Per-kernel parity on a real H100: every C-ABI entry point against the same op in plain PyTorch
 (fp32 math on the same bf16-rounded inputs).  Tolerances are written per test."""
 import math
 
@@ -62,11 +62,11 @@ def test_gemm_forced_tile(ops, bn):
 
 @pytest.mark.parametrize("M,N,K", [(256, 256, 64), (512, 512, 256), (2560, 4096, 512), (300, 514, 768), (1000, 1280, 320),
                                    (129, 257, 128), (2048, 11008, 256), (4096, 768, 768)])
-def test_gemm_2cta(ops, M, N, K):
-    """cta_group::2 kernel (256x256 cluster tiles) on even / ragged shapes"""
+def test_gemm_wide_tile(ops, M, N, K):
+    """128 x 256 tiles (the widest wgmma tile) with bias / activation / residual on even / ragged shapes"""
     from vstar_b200 import _lib
     a, w, b, r = rnd(M, K, seed=31), rnd(N, K, scale=1 / math.sqrt(K), seed=32), rnd(N, seed=33), rnd(M, N, seed=34)
-    _lib.call("vsb_gemm_set_tuning", 512, 0)
+    _lib.call("vsb_gemm_set_tuning", 256, 0)
     try:
         out = ops.gemm(a, w, out_dtype=torch.float32)
         out2 = ops.gemm(a, w, bias=b, residual=r, epilogue=ops.EPI_QUICK_GELU)
@@ -79,11 +79,11 @@ def test_gemm_2cta(ops, M, N, K):
     assert torch.allclose(out2.float(), ref2, rtol=1e-2, atol=3e-2), rel_err(out2, ref2)
 
 
-def test_gemm_2cta_persistent_few_clusters(ops):
+def test_gemm_wide_tile_persistent_few_ctas(ops):
     from vstar_b200 import _lib
     M, N, K = 1536, 2048, 448
     a, w = rnd(M, K, seed=35), rnd(N, K, scale=1 / math.sqrt(K), seed=36)
-    _lib.call("vsb_gemm_set_tuning", 512, 6)          # 3 clusters, 48 tiles -> 16 tiles each: ring + TMEM double-buffer phases
+    _lib.call("vsb_gemm_set_tuning", 256, 3)          # 3 CTAs, 96 tiles -> 32 tiles each: smem ring phases across tiles
     try:
         out = ops.gemm(a, w, out_dtype=torch.float32)
     finally:
@@ -100,7 +100,7 @@ def test_gemm_tile_rasterisation(ops, group_m):
     _lib.call("vsb_gemm_set_group_m", group_m)
     try:
         out = ops.gemm(a, w, out_dtype=torch.float32)
-        _lib.call("vsb_gemm_set_tuning", 512, 0)
+        _lib.call("vsb_gemm_set_tuning", 256, 0)
         out2 = ops.gemm(a, w, out_dtype=torch.float32)
     finally:
         _lib.call("vsb_gemm_set_group_m", 0)
@@ -110,7 +110,7 @@ def test_gemm_tile_rasterisation(ops, group_m):
 
 
 def test_gemm_persistent_many_tiles(ops):
-    """few CTAs, many tiles per CTA: exercises the smem ring phases and the TMEM double buffer"""
+    """few CTAs, many tiles per CTA: exercises the smem ring phases across tiles"""
     from vstar_b200 import _lib
     M, N, K = 1024, 1536, 448
     a, w = rnd(M, K, seed=5), rnd(N, K, scale=1 / math.sqrt(K), seed=6)
@@ -188,7 +188,7 @@ def test_attn_decode_kernel_shapes(ops, D, causal, Sq, Sk):
                                    (8, 12288, 1024), (7, 32004, 512), (9, 4096, 4096), (16, 1000, 1192), (13, 22016, 256)])
 def test_gemm_skinny(ops, M, N, K):
     """decode-sized problems take the weight-streaming kernels of gemm_skinny.cu (CUDA-core FMA kernel for M <= 2, mma.sync
-    kernel up to M = 16); both must agree with the fp32 reference AND with the tcgen05 kernel on every epilogue variant
+    kernel up to M = 16); both must agree with the fp32 reference AND with the wgmma tile kernel on every epilogue variant
     (same semantics behind vsb_gemm_bf16)"""
     from vstar_b200 import _lib
     a, w, b = rnd(M, K, seed=61), rnd(N, K, scale=1 / math.sqrt(K), seed=62), rnd(N, seed=63)
@@ -204,7 +204,7 @@ def test_gemm_skinny(ops, M, N, K):
 
     got = {}
     try:
-        for variant in ([1] if M <= 8 else []) + [2, 64]:   # 1 = FMA kernel, 2 = mma.sync kernel, 64 = tcgen05 single-CTA kernel
+        for variant in ([1] if M <= 8 else []) + [2, 64]:   # 1 = FMA kernel, 2 = mma.sync kernel, 64 = wgmma tile kernel
             _lib.call("vsb_gemm_set_tuning", variant, 0)     # forcing a skinny variant errors out if it cannot take the shape
             got[variant] = run_all()
     finally:
@@ -294,8 +294,8 @@ def test_rope_bit_exact(ops):
                                             (2, 2, 128, 64, False), (1, 3, 384, 128, False), (2, 2, 515, 64, True), (1, 2, 577, 64, False),
                                             (2, 1, 256, 64, True), (1, 2, 1000, 64, True)])
 def test_flash_attn(ops, B, H, S, D, causal, impl):
-    """impl 1 = mma.sync kernel, 2 = tcgen05 kernels (two-tile ping-pong kernel for head_dim 64, Sq > 128), 3 = tcgen05
-    single-tile kernel only (all behind vsb_flash_attn_bf16)"""
+    """impl 1 = mma.sync kernel, 2 = wgmma kernel (two query warpgroups per CTA for Sq > 64), 3 = wgmma kernel with one
+    query warpgroup per CTA only (all behind vsb_flash_attn_bf16)"""
     from vstar_b200 import _lib
     qkv = rnd(B * S, 3 * H * D, seed=40)
     _lib.call("vsb_attn_set_impl", impl)
@@ -561,7 +561,7 @@ def test_gemm_with_folded_rmsnorm(ops):
 
 def test_rows_invariant_to_batch(ops):
     """batch-invariant mode (vsb_set_batch_invariant): the first rows of a GEMM / RMSNorm are bit-identical whether the call
-    carries 3, 16, 320, 2264 or 18112 rows - i.e. the tcgen05 tile variants (32/64/128/256 wide, 2-CTA) accumulate every
+    carries 3, 16, 320, 2264 or 18112 rows - i.e. the wgmma tile variants (32/64/128/256 wide) accumulate every
     output element in the same order, and no row-count-dependent kernel family is taken.  This is what makes a crop's record
     independent of the batch it was evaluated in (speculative batching, frontier sharding)."""
     torch.manual_seed(0)
@@ -654,7 +654,7 @@ def test_llama_layers_native_runner(ops):
         _lib.call("vsb_llama_set_fuse_rope", 1)
     # tail mode: the last layer runs attention / o-proj / MLP over the last rows of every sequence only.  The cache (K/V of
     # every row, every layer) must be bit-identical; the tail rows are bit-identical when the compact GEMMs run on the same
-    # tcgen05 kernels as the full pass (more than 16 rows: B * tail = 18) and equal to bf16 rounding when the few rows take
+    # wgmma tile kernels as the full pass (more than 16 rows: B * tail = 18) and equal to bf16 rounding when the few rows take
     # the decode GEMM kernels (B * tail = 10), whose k order differs.
     cache_f = torch.zeros(nl, B, Tmax, 3 * d, dtype=BF, device="cuda")
     xf = native_stack(rnd(B * 70, d, seed=110).clone(), cache_f, 70, 0)

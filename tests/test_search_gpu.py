@@ -5,6 +5,8 @@ import os
 
 import numpy as np
 import pytest
+
+from tests.helpers import REPORT_DIR
 import torch
 
 from tests.helpers import FakeNLP, NumpyScorer, StubVSM, synth_image
@@ -115,8 +117,8 @@ def test_model_search_trajectory_vs_reference_golden(tiny_vsm, tag):
         d = (fs["detection_result"] - torch.from_numpy(g["detection_result"])).abs().max()
         PARITY[f"search_model_{tag}"]["final_bbox_err_px"] = float(d)
         assert float(d) <= 1.0          # <= 1 px at crop scale
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(PARITY, open("gpurun_out/search_parity_report.json", "w"), indent=1)
+    os.makedirs(REPORT_DIR, exist_ok=True)
+    json.dump(PARITY, open(os.path.join(REPORT_DIR, "search_parity_report.json"), "w"), indent=1)
 
 
 def test_pipelined_records_equal_synchronous_maps(tiny_vsm):

@@ -8,6 +8,8 @@ import os
 
 import numpy as np
 import pytest
+
+from tests.helpers import REPORT_DIR
 import torch
 
 pytestmark = pytest.mark.gpu
@@ -82,7 +84,7 @@ def test_vqa_forward_options_generate(setup, sub):
         assert float(last.max() - last[t]) < 3e-2
         embeds = torch.cat([embeds, emb[torch.tensor([t])].unsqueeze(0)], dim=1)
     json.dump(dict(err_new=e_new, err_ref_bf16=e_ref, losses=losses.tolist(), ref_losses=ref_l.tolist(), gen=out, ref_gen=g["gen"].tolist()),
-              open(f"gpurun_out/vqa_parity_{sub}.json", "w"))
+              open(os.path.join(REPORT_DIR, f"vqa_parity_{sub}.json"), "w"))
 
 
 def test_vqa_llm_wrapper_api(setup):

@@ -51,7 +51,7 @@ def test_tokenizer_image_object_token():
 
 
 def test_bf16_vs_fp16_option_choice_bound():
-    """The reference runs the SEAL VQA LLM in fp16 (LLaVA/llava/model/builder.py:43, vstar_bench_eval.py:93); the sm_100a kernels
+    """The reference runs the SEAL VQA LLM in fp16 (LLaVA/llava/model/builder.py:43, vstar_bench_eval.py:93); the sm_90a kernels
     compute in bf16 with fp32 accumulation.  On the goldens produced by the real reference (fp32), the oracle executed in fp16 and
     in bf16 bounds what the dtype change can do to option scoring: both stay within 2e-2 of the fp32 NLLs, bf16's error is
     within 16x of fp16's (3 fewer mantissa bits), and the chosen option is the fp32 one whenever the two best options are

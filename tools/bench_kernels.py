@@ -43,7 +43,7 @@ def main():
         ms_t = timeit(lambda: torch.matmul(a, w.t(), out=out))
         tf = 2 * M * N * K / ms / 1e9
         var = {}
-        for tag, bn in (("1cta_256", 256), ("1cta_128", 128), ("2cta", 512)):
+        for tag, bn in (("tile_256", 256), ("tile_128", 128)):
             _lib.call("vsb_gemm_set_tuning", bn, 0)
             var[tag] = round(2 * M * N * K / timeit(lambda: ops.gemm(a, w, out=out)) / 1e9, 1)
         _lib.call("vsb_gemm_set_tuning", 0, 0)
@@ -56,7 +56,7 @@ def main():
         out = torch.empty(B * S, H * D, dtype=BF, device="cuda")
         fl = 4 * B * H * S * S * D * (0.5 if causal else 1.0)
         var = {}
-        for tag, impl in (("mma_sync", 1), ("tcgen05", 2), ("tcgen05_1tile", 3)):
+        for tag, impl in (("mma_sync", 1), ("wgmma", 2), ("wgmma_1wg", 3)):
             _lib.call("vsb_attn_set_impl", impl)
             var[tag] = round(fl / timeit(lambda: ops.attn_fused_qkv(qkv, B, S, H, D, causal, D ** -0.5, out=out)) / 1e9, 1)
         _lib.call("vsb_attn_set_impl", 0)
@@ -70,8 +70,8 @@ def main():
         ms = timeit(lambda: ops.rmsnorm(x, w, 1e-6, out=y))
         res.append(dict(kernel="rmsnorm", rows=rows, cols=cols, ms=ms, gbs=rows * cols * 4 / ms / 1e6))
         print(res[-1], flush=True)
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(res, open("gpurun_out/bench_kernels.json", "w"), indent=1)
+    os.makedirs("bench_out", exist_ok=True)
+    json.dump(res, open("bench_out/bench_kernels.json", "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -1,8 +1,8 @@
-"""Latency probes for the two launch-/HBM-bound corners of the path (run on a B200):
+"""Latency probes for the two launch-/HBM-bound corners of the path (run on the GPU):
   * SEAL VQA LLM at full size (Vicuna-7B shapes, random init): prefill, greedy decode ms/token, option scoring
     (vstar_bench_eval.py:78-165) and the M=1 decode GEMMs against the HBM roofline (weights are read once per token);
   * one single-crop VSM round (the root round of every search): wall clock vs GPU time vs launches.
-Writes gpurun_out/bench_vqa.json."""
+Writes bench_out/bench_vqa.json."""
 import json
 import os
 import sys
@@ -122,8 +122,8 @@ def main():
             g, wl = ev_time(lambda: vsm.detect_regions(regions, ["Please locate the mug in this image."] * nb), iters=5, warmup=2)
             res[f"vsm_round_B{nb}"] = dict(gpu_ms=g, wall_ms=wl, launches=(_lib.launches - l0) // 7)
             print(nb, res[f"vsm_round_B{nb}"], flush=True)
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(res, open("gpurun_out/bench_vqa.json", "w"), indent=1)
+    os.makedirs("bench_out", exist_ok=True)
+    json.dump(res, open("bench_out/bench_vqa.json", "w"), indent=1)
 
 
 if __name__ == "__main__":

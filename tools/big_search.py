@@ -48,5 +48,5 @@ for size, smallest, expect in [(2048, 512, 21), (4096, 512, 85), (8192, 1024, 85
         if size == 8192 and smallest == 256 and rep == 0:
             pass
     out.append(r)
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(out, open("gpurun_out/big_search.json", "w"), indent=1)
+os.makedirs("bench_out", exist_ok=True)
+json.dump(out, open("bench_out/big_search.json", "w"), indent=1)

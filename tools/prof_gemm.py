@@ -1,7 +1,7 @@
-"""Dominant GEMM launch of the bench step under ncu (run on the GPU box):
+"""Dominant GEMM launch of the bench step under ncu (run on a GPU):
 
     ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum,gpu__time_duration.sum,sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active \
-        --clock-control none -k regex:gemm_bf16_tcgen05 --csv --log-file gpurun_out/gemm_dram_bytes.csv python tools/prof_gemm.py
+        --clock-control none -k regex:gemm_bf16_wgmma --csv --log-file bench_out/gemm_dram_bytes.csv python tools/prof_gemm.py
 
 -> copy to profiles/rNN_gemm_dram_bytes.csv; bench.py reads roofline.traffic from the LAST launch in that file.
 Shape = gate|up projection of a 64-crop frontier batch with the shared-prefix KV active (283 rows per crop): M = 18112, N = 22016

@@ -1,5 +1,5 @@
 """Aggregate an `ncu --metrics gpu__time_duration.sum --csv` launch list per kernel: launches, total ms, share, average us.
-Usage: python tools/summarize_launches.py gpurun_out/r02_step_launches.csv > profiles/r02_step_launch_summary.csv"""
+Usage: python tools/summarize_launches.py launches.csv > launch_summary.csv"""
 import csv
 import re
 import sys

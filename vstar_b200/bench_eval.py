@@ -46,9 +46,11 @@ def build_parser():
 
 
 def list_samples(folder):
-    """vstar_bench_eval.py:185-191 (os.listdir order, as the reference; annotation = image path up to the first '.')"""
+    """vstar_bench_eval.py:185-191 (os.listdir order, as the reference; annotation = image file name up to its first '.').
+    The reference cuts the whole path at its first '.', which breaks under a directory with a dot in its name; only the
+    file name is cut here."""
     files = [f for f in os.listdir(folder) if ".json" not in f]
-    return [(f, os.path.join(folder, f), os.path.join(folder, f).split(".")[0] + ".json") for f in files]
+    return [(f, os.path.join(folder, f), os.path.join(folder, f.split(".")[0] + ".json")) for f in files]
 
 
 def eval_model(args, vqa_llm=None, vsm=None, log=print, search_kwargs=None):

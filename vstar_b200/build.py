@@ -1,9 +1,9 @@
-"""Build libvstar_b200.so (hand-written sm_100a CUDA kernels + C-ABI) in-tree with nvcc.
+"""Build libvstar_b200.so (hand-written sm_90a CUDA kernels + C-ABI) in-tree with nvcc.
 
     python -m vstar_b200.build            # incremental
     python -m vstar_b200.build --force
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with gpurun.
+nvcc cross-compiles without a GPU.  Objects go to vstar_b200/build/, the library next to this file; both are git-ignored.
 """
 import os
 import subprocess
@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libvstar_b200.so")
 SOURCES = ["api.cu", "gemm_tcgen05.cu", "gemm_skinny.cu", "llama_layers.cu", "attention.cu", "attention_tc.cu", "elementwise.cu", "heads.cu", "image.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 
 
@@ -26,7 +26,7 @@ def _newer(a, b):
 def build(force=False, verbose=False):
     objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
-    deps = [os.path.join(CSRC, "common.cuh"), os.path.join(ROOT, "include", "vstar_b200.h")]
+    deps = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "wgmma.cuh"), os.path.join(ROOT, "include", "vstar_b200.h")]
     objs, procs = [], []
     for src in SOURCES:
         s = os.path.join(CSRC, src)

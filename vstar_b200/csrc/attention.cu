@@ -7,8 +7,8 @@
 //                         transformers/models/llama/modeling_llama.py:199-221 (softmax in fp32, P cast to bf16).
 //                         Round-1 implementation: FA2-style tiling (64 queries x 64 keys per step, cp.async
 //                         double-buffered K/V in XOR-swizzled shared memory, ldmatrix + mma.sync.m16n8k16).
-//                         A tcgen05/TMEM version replaces this in a later round; attention is ~5 % of the
-//                         per-crop FLOPs (BASELINE.md §3).
+//                         The wgmma kernel of attention_tc.cu takes the shapes with Sq >= 64; attention is
+//                         ~5 % of the per-crop FLOPs (BASELINE.md §3).
 //  vsb_attn_small_bf16  : tiny-head attention of the SAM two-way transformer (head_dim 16 / 32, 6 tokens
 //                         <-> 2304 image tokens); CUDA-core kernel, fp32 math.
 //                         (/root/reference/VisualSearch/model/segment_anything/modeling/transformer.py:220-242)
@@ -325,14 +325,14 @@ __global__ void __launch_bounds__(128) attn_small_kernel(const bf16* __restrict_
 
 }  // namespace
 
-// tcgen05 kernel (attention_tc.cu)
+// wgmma kernel (attention_tc.cu)
 int vsb_flash_attn_tc(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs, long long k_rs,
                       long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk, int D, int causal,
                       float scale, cudaStream_t stream);
 
 // ------------------------------------------------------------------ decode attention (Sq <= 4 new rows against a long KV cache)
 // HBM/latency-bound: one (batch, head) reads Sk rows of K and V once.  The FA2-style kernel above gives such a problem ONE
-// CTA per head (32 CTAs for Vicuna-7B, 22 us per layer at Sk = 700).  Here the keys of a head are split over a CLUSTER of 8
+// CTA per head (32 CTAs for Vicuna-7B).  Here the keys of a head are split over a CLUSTER of 8
 // CTAs (flash-decoding); each warp streams its keys with the row spread over the 32 lanes (coalesced 128/256 B rows, 4 keys
 // in flight per warp), keeps an online-softmax partial (m, l, acc) per query, warps combine through shared memory, and
 // cluster rank 0 combines the 8 CTA partials through DISTRIBUTED shared memory - no global scratch, no second kernel.
@@ -497,7 +497,7 @@ static int launch_decode(const AttnParams& p, cudaStream_t st) {
 }
 
 void vsb_attn_tc_set_variant(int v);
-static int g_attn_impl = 0;   // 0 auto, 1 = mma.sync kernel, 2 = tcgen05 kernel(s), 3 = tcgen05 single-tile kernel only, 4 = decode kernel
+static int g_attn_impl = 0;   // 0 auto, 1 = mma.sync kernel, 2 = wgmma kernel, 3 = wgmma kernel with one query warpgroup per CTA, 4 = decode kernel
 extern "C" int vsb_attn_set_impl(int impl) {
   g_attn_impl = (impl == 3) ? 2 : impl;
   vsb_attn_tc_set_variant(impl == 3 ? 1 : 0);
@@ -525,7 +525,6 @@ extern "C" int vsb_attn_decode_bf16(const void* q, const void* k, const void* v,
 
 static int launch_flash_mma(const AttnParams& p, int D, cudaStream_t st) {
   if (D == 64) {
-    // (a 128-query-row variant, 2 m16 tiles per warp, measured slower on B200: 218 registers halve the occupancy)
     const int smem = (64 + 4 * FA_BN) * 64 * 2;
     static bool set64 = false;
     if (!set64) { VSB_CUDA(cudaFuncSetAttribute(flash_attn_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); set64 = true; }

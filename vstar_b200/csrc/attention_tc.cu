@@ -1,28 +1,27 @@
-// tcgen05 flash attention (prefill shapes): softmax(Q K^T * scale [+ causal]) V, head_dim 64 / 128, bf16, fp32 softmax.
+// wgmma flash attention (prefill shapes): softmax(Q K^T * scale [+ causal]) V, head_dim 64 / 128, bf16, fp32 softmax.
 //
-// One CTA = 128 query rows of one (batch, head); keys are consumed in blocks of 128:
-//   S  = Q K_j^T          tcgen05.mma 128 x 128 x D   (A = Q tile, B = K tile, both K-major SW128 from TMA)  -> TMEM
-//   P  = exp2(S*s - m)    128 softmax threads, thread r <-> TMEM lane r <-> query row r (row max / sum are thread
-//                         local, no shuffles); P is written as bf16 into a SW128 K-major smem tile
-//   O_j = P V_j           tcgen05.mma 128 x D x 128   (A = P tile, B = V tile as an MN-major operand: V stays [key][d]) -> TMEM
-//   O  = O * corr + O_j   accumulated in REGISTERS by the softmax threads (no TMEM read-modify-write, no correction warps)
-// Warp roles: warp 0 = TMA producer (Q once, K/V ring of 2 stages via 3-D tensor maps so rows >= Sk are zero-filled),
-// warp 1 = MMA issuer, warp 2 = TMEM allocator, warps 4-7 = softmax / accumulate / epilogue.
-// head_dim 64: 112 KB smem and 256 TMEM columns per CTA -> 2 CTAs per SM overlap each other's softmax and MMA phases.
+// One CTA = NWG consumer warpgroups x 64 query rows of one (batch, head) + one producer warpgroup; keys are consumed in
+// blocks of 128 that all consumer warpgroups share:
+//   S  = Q K_j^T          wgmma m64n128k16 x D/16   (A = Q tile, B = K tile, both K-major SW128 from TMA) -> registers
+//   P  = exp2(S*s - m)    on the accumulator fragments: a row lives in the 4 threads of a quad (max / sum by 2 shuffles)
+//   O += P V_j            wgmma m64nDk16 x 8         (A = P straight from registers as bf16 fragments, B = V tile as an
+//                                                     MN-major operand: V stays [key][d]) -> O accumulates in registers
+// The online-softmax rescale is lazy: the exponent reference m_ref of a row only moves when its running max grows by more
+// than 2^8 (then O and l of that row are scaled by 2^(m_old - m_new)).
+// Warpgroup 0: one thread issues the TMA loads (Q once, K/V ring via 3-D tensor maps so rows >= Sk are zero-filled).
 //
-// Replaces the mma.sync kernel of attention.cu for Sq >= 128 (CLIP S=257, OWL-ViT S=2305, 7B prefill T~320); numerics as
+// Replaces the mma.sync kernel of attention.cu for Sq >= 64 (CLIP S=257, OWL-ViT S=2305, 7B prefill T~320); numerics as
 // the reference: scores and softmax in fp32, P rounded to bf16 before P@V (modeling_clip.py:261-329, modeling_llama.py:199-221).
 #include "common.cuh"
 #include "vstar_b200.h"
+#include "wgmma.cuh"
 
 #include <mutex>
-#include <unordered_map>
 
 namespace {
 
-constexpr int BQ = 128;     // query rows per CTA
 constexpr int BKV = 128;    // keys per block
-constexpr int SUB_BYTES = 128 * 64 * 2;   // one [128][64] bf16 SW128 sub-tile
+constexpr int SUB_BYTES = 128 * 64 * 2;   // one [128][64] bf16 SW128 K / V sub-tile
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -48,7 +47,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tm, int c0, int c1, int c2, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -56,139 +54,66 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* t
       : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) { asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major SW128 operand (A = Q / P tiles, B = K tile): SBO = 1024 B between 8-row groups (see gemm_tcgen05.cu)
+// K-major SW128 operand (A = Q tile, B = K tile): SBO = 1024 B between 8-row groups (see gemm_tcgen05.cu)
 __device__ __forceinline__ uint64_t desc_kmajor(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-// MN-major SW128 operand (B = V tile kept as [key][d]): canonical layout ((8,8,m),(8,k)):((1,8,LBO),(64,SBO)) in elements:
+// MN-major SW128 operand (B = V tile kept as [key][d]): canonical layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units:
 // 64 contiguous MN (= d) elements per 128-byte row, 8 consecutive K (= key) rows per 1024-byte swizzle atom,
 // SBO = 1024 B between 8-key groups, LBO = stride between 64-wide d blocks (one 16 KB sub-tile)
 __device__ __forceinline__ uint64_t desc_mnmajor(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(SUB_BYTES >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-// kind::f16 instruction descriptor: D fp32, A/B bf16, A K-major; b_mn = 1 -> B MN-major (bit 16)
-__host__ __device__ constexpr uint32_t make_idesc(int m, int n, int b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)b_mn << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(SUB_BYTES >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 
-struct AttnTcParams {
-  bf16* o;
-  long long o_bs, o_rs;
-  int H, Sq, Sk, causal;
-  int q_col0, k_col0, v_col0;   // column of head 0 inside the Q / K / V tensor maps (elements)
-  float scale_log2;
-};
-
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-      "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-      "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32_x8(uint32_t taddr, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32_x8(uint32_t taddr, const uint32_t* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]),
-               "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
 // one MUFU op: 2^x, |rel err| <= 2^-22, ex2(-inf) = 0
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// Budget per 128 x 128 score block: TMEM->RF moves 64 B/clk/SM and the MUFU does 16 exp2/clk/SM, i.e. >= 1024 clk per block
-// either way, against 512 clk of tensor-core time (D = 64).  So: S is read from TMEM exactly ONCE per block (all 128 columns
-// of the row live in registers), and O accumulates in TMEM across blocks (tcgen05.mma accumulate) instead of being read
-// back every block; the online-softmax rescale of O is LAZY (FlashAttention-4 style): the exponent reference m_ref is only
-// raised when the running max grows by more than 2^8, in which case the warp rescales its O rows in TMEM (ld, mul, st).
-template <int D>
+template <int N>
+__device__ __forceinline__ void fence_regs(float* r) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+
+struct AttnTcParams {
+  bf16* o;
+  long long o_bs, o_rs;
+  int H, Sq, Sk, causal;
+  float scale_log2;
+};
+
+template <int D, int NWG>
 struct ASmem {
   static constexpr int NSUB = D / 64;
   static constexpr int KV_ST = (D == 64) ? 3 : 2;
-  static constexpr int Q_BYTES = NSUB * SUB_BYTES;
+  static constexpr int Q_SUB = NWG * 64 * 128;                     // one [64 NWG][64] bf16 SW128 Q sub-tile
+  static constexpr int Q_BYTES = NSUB * Q_SUB;
   static constexpr int KV_STAGE_BYTES = 2 * NSUB * SUB_BYTES;      // K sub-tiles then V sub-tiles
-  static constexpr int P_BYTES = 2 * SUB_BYTES;                    // one 128 x 128 bf16 P tile
-  static constexpr int P_OFF = Q_BYTES + KV_ST * KV_STAGE_BYTES;
-  static constexpr int PB = (D == 64) ? 2 : 1;                     // P tile buffers (double buffered when smem allows)
-  static constexpr int RED_OFF = P_OFF + PB * P_BYTES;
-  static constexpr int RED_BYTES = 2 * 4 * 128 * 4;                // [parity][column group][row] fp32 row-max exchange
-  static constexpr int BAR_OFF = RED_OFF + RED_BYTES;
+  static constexpr int BAR_OFF = Q_BYTES + KV_ST * KV_STAGE_BYTES;
   static constexpr int TOTAL = BAR_OFF + 128;
 };
 
-template <int D>
-__global__ void __launch_bounds__(640, 1)
-attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-               const AttnTcParams p) {
-  using L = ASmem<D>;
+template <int D, int NWG>
+__global__ void __launch_bounds__(128 * (NWG + 1), 1)
+attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                  const AttnTcParams p) {
+  using L = ASmem<D, NWG>;
   constexpr int NSUB = L::NSUB;
   constexpr int ST = L::KV_ST;
-  constexpr uint32_t TMEM_COLS = 512;           // S0 @0, S1 @128, O @256 (D columns)
+  constexpr int BQ = 64 * NWG;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
   uint8_t* sKV = smem + L::Q_BYTES;
-  uint8_t* sP = smem + L::P_OFF;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
   uint64_t* q_full = bars + 0;
   uint64_t* kv_full = bars + 1;                 // [ST]
   uint64_t* kv_empty = kv_full + ST;            // [ST]
-  uint64_t* s_full = kv_empty + ST;             // [2]   S buffer written by the tensor core
-  uint64_t* s_free = s_full + 2;                // [2]   128 arrivals: all rows of the S buffer are in registers
-  uint64_t* p_full = s_free + 2;                // [2]   128 arrivals: P tile (and any O rescale) published
-  uint64_t* pv_done = p_full + 2;               // [2]   P buffer consumed / O updated by P_j V_j
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(pv_done + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
   const int off = p.Sk - p.Sq;
   int nblk = (p.Sk + BKV - 1) / BKV;
@@ -200,33 +125,21 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     if (nb < nblk) nblk = nb;
   }
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-  }
-  if (warp == 1 && lane == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < ST; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&s_full[s], 1);
-      mbar_init(&s_free[s], 16);      // one arrive per softmax warp
-      mbar_init(&p_full[s], 16);
-      mbar_init(&pv_done[s], 1);
-    }
+    for (int s = 0; s < ST; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 4 * NWG); }   // one arrive per consumer warp
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t tmem_O = tmem_base + 256;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ---------------- TMA producer
+  if (wg == 0) {
+    // ---------------- TMA producer
+    if constexpr (NWG == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(q_full, L::Q_BYTES);
 #pragma unroll
-      for (int s = 0; s < NSUB; ++s) tma_load_3d(sQ + s * SUB_BYTES, &tmQ, p.q_col0 + h * D + s * 64, q0, b, q_full);
+      for (int s = 0; s < NSUB; ++s) tma_load_3d(sQ + s * L::Q_SUB, &tmQ, h * D + s * 64, q0, b, q_full);
       int stage = 0;
       uint32_t phase = 0;
       for (int j = 0; j < nblk; ++j) {
@@ -235,449 +148,114 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
         mbar_arrive_expect_tx(&kv_full[stage], L::KV_STAGE_BYTES);
 #pragma unroll
         for (int s = 0; s < NSUB; ++s) {
-          tma_load_3d(dst + s * SUB_BYTES, &tmK, p.k_col0 + h * D + s * 64, j * BKV, b, &kv_full[stage]);
-          tma_load_3d(dst + (NSUB + s) * SUB_BYTES, &tmV, p.v_col0 + h * D + s * 64, j * BKV, b, &kv_full[stage]);
+          tma_load_3d(dst + s * SUB_BYTES, &tmK, h * D + s * 64, j * BKV, b, &kv_full[stage]);
+          tma_load_3d(dst + (NSUB + s) * SUB_BYTES, &tmV, h * D + s * 64, j * BKV, b, &kv_full[stage]);
         }
         if (++stage == ST) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ---------------- MMA issuer
-      constexpr uint32_t idesc_s = make_idesc(128, BKV, 0);
-      constexpr uint32_t idesc_o = make_idesc(128, D, 1);
-      const uint32_t aQ = smem_u32(sQ);
-      mbar_wait(q_full, 0);
-      // stage / phase of the K tile of the NEXT S to issue, and of the V tile of the next PV
-      int ks = 0, vs = 0;
-      uint32_t kph = 0;
-      auto issue_S = [&](int jj) {
-        mbar_wait(&kv_full[ks], kph);
-        if (jj >= 2) mbar_wait(&s_free[jj & 1], ((jj >> 1) - 1) & 1);     // rows of S_{jj-2} are in registers
-        tc_fence_after();
-        const uint32_t aK = smem_u32(sKV + ks * L::KV_STAGE_BYTES);
-        const uint32_t dS = tmem_base + (uint32_t)((jj & 1) * 128);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk)
-          umma_f16(dS, desc_kmajor(aQ + (kk >> 2) * SUB_BYTES + (kk & 3) * 32), desc_kmajor(aK + (kk >> 2) * SUB_BYTES + (kk & 3) * 32), idesc_s,
-                   kk > 0 ? 1u : 0u);
-        umma_commit(&s_full[jj & 1]);
-        if (++ks == ST) { ks = 0; kph ^= 1; }
-      };
-      issue_S(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) issue_S(j + 1);           // S_{j+1} runs on the tensor core while the softmax threads work on S_j
-        mbar_wait(&p_full[j & 1], (j >> 1) & 1);    // P_j published (and O rescaled if the reference max moved)
-        tc_fence_after();
-        const uint32_t aP = smem_u32(sP + (j % L::PB) * L::P_BYTES);
-        const uint32_t aV = smem_u32(sKV + vs * L::KV_STAGE_BYTES + NSUB * SUB_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < BKV / 16; ++kk)
-          umma_f16(tmem_O, desc_kmajor(aP + (kk >> 2) * SUB_BYTES + (kk & 3) * 32), desc_mnmajor(aV + kk * 2048), idesc_o, (j > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(&pv_done[j & 1]);
-        umma_commit(&kv_empty[vs]);                 // K_j (S_j retired earlier) and V_j are free once these MMAs retire
-        if (++vs == ST) vs = 0;
-      }
-    }
-  } else if (warp >= 4) {
-    // ---------------- softmax / epilogue: 16 warps = 4 TMEM lane quarters x 4 column groups of 32 keys.
-    // Thread (qtr, lane, cg) owns query row r = 32*qtr + lane and keys [32*cg, 32*cg+32) of every block: four threads share a
-    // row (row max exchanged through smem + a 128-thread named barrier), which puts 4 softmax warps on every SM sub-partition
-    // so that MUFU / TMEM-load latencies overlap.
-    const int qtr = warp & 3;
-    const int cg = (warp - 4) >> 2;
-    const int r = qtr * 32 + lane;
-    const int qrow = q0 + r;
-    const uint32_t lane_addr = (uint32_t)(qtr * 32) << 16;
-    float* red = reinterpret_cast<float*>(smem + L::RED_OFF);
-    float m_ref = 0.f, l_part = 0.f;
-    const int kmax = p.causal ? min(qrow + off, p.Sk - 1) : (p.Sk - 1);     // last visible key of this row
-    constexpr int OC = D / 4;                     // O columns owned by this column group (rescale / epilogue)
+    return;
+  }
 
-    for (int j = 0; j < nblk; ++j) {
-      const int buf = j & 1;
-      mbar_wait(&s_full[buf], (j >> 1) & 1);
-      tc_fence_after();
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + lane_addr + (uint32_t)(buf * 128 + cg * 32), v);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_free[buf]);
-      const int nvis = kmax - (j * BKV + cg * 32) + 1;     // keys [0, nvis) of this thread's 32 are visible
-      float mx = -INFINITY;
-      if (nvis >= 32) {                                    // common case: no masking work at all
+  // ---------------- consumers: warpgroup c owns query rows [64c, 64c + 64) of the CTA; thread rows r0 = 16 w + lane/4 and
+  // r0 + 8, key / d columns 8 j + 2 t + {0, 1} of every fragment block j (t = lane % 4)
+  if constexpr (NWG == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int c = wg - 1;
+  const int t = lane & 3;
+  const int rr = c * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  const int qrow[2] = {q0 + rr, q0 + rr + 8};
+  int kmax[2];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-      } else {
+  for (int hh = 0; hh < 2; ++hh) kmax[hh] = p.causal ? min(qrow[hh] + off, p.Sk - 1) : (p.Sk - 1);   // last visible key of the row
+  float m_ref[2] = {0.f, 0.f}, l_part[2] = {0.f, 0.f};
+  float o[D / 2];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          if (i >= nvis) v[i] = 0xff800000u;               // -inf: exp2 -> 0
-          mx = fmaxf(mx, __uint_as_float(v[i]));
-        }
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+  float s[BKV / 2];
+  const uint32_t aQ = smem_u32(sQ) + c * (64 * 128);
+
+  mbar_wait(q_full, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int j = 0; j < nblk; ++j) {
+    mbar_wait(&kv_full[stage], phase);
+    const uint32_t aK = smem_u32(sKV + stage * L::KV_STAGE_BYTES);
+    const uint32_t aV = aK + NSUB * SUB_BYTES;
+    // ---- S = Q K_j^T
+    fence_regs<BKV / 2>(s);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss<BKV>(s, desc_kmajor(aQ + (kk >> 2) * L::Q_SUB + (kk & 3) * 32), desc_kmajor(aK + (kk >> 2) * SUB_BYTES + (kk & 3) * 32),
+                    kk > 0 ? 1 : 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<BKV / 2>(s);
+    // ---- mask, row max (quad), lazy reference-max update
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int nvis = kmax[hh] - j * BKV + 1;        // keys [0, nvis) of the block are visible to this row
+      if (nvis < BKV) {
+#pragma unroll
+        for (int jj = 0; jj < BKV / 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (8 * jj + 2 * t + e >= nvis) s[4 * jj + 2 * hh + e] = -INFINITY;
       }
-      mx *= p.scale_log2;                                  // scale > 0: max commutes with the scaling
-      // ---- row max across the 4 column groups
-      float* rj = red + buf * 512;
-      rj[cg * 128 + r] = mx;
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + qtr) : "memory");
-      mx = fmaxf(fmaxf(rj[r], rj[128 + r]), fmaxf(rj[256 + r], rj[384 + r]));
-      // ---- lazy reference-max update (identical in the 4 threads of a row)
-      float corr = 1.f;
+#pragma unroll
+      for (int jj = 0; jj < BKV / 8; ++jj) mx[hh] = fmaxf(mx[hh], fmaxf(s[4 * jj + 2 * hh], s[4 * jj + 2 * hh + 1]));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+      mx[hh] *= p.scale_log2;                          // scale > 0: max commutes with the scaling
       if (j == 0) {
-        m_ref = (mx == -INFINITY) ? 0.f : mx;
-      } else if (mx > m_ref + 8.f) {
-        corr = exp2f(m_ref - mx);
-        m_ref = mx;
-      }
-      if (__any_sync(0xffffffffu, corr != 1.f)) {
-        // this warp's O columns *= corr, after P_{j-1} V_{j-1} has landed in O
-        mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);
-        tc_fence_after();
-        uint32_t ov[OC];
-        const uint32_t tO = tmem_O + lane_addr + cg * OC;
-        if constexpr (OC == 32) {
-          tmem_ld_32x32(tO, ov);
-        } else {
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                       : "=r"(ov[0]), "=r"(ov[1]), "=r"(ov[2]), "=r"(ov[3]), "=r"(ov[4]), "=r"(ov[5]), "=r"(ov[6]), "=r"(ov[7]), "=r"(ov[8]),
-                         "=r"(ov[9]), "=r"(ov[10]), "=r"(ov[11]), "=r"(ov[12]), "=r"(ov[13]), "=r"(ov[14]), "=r"(ov[15])
-                       : "r"(tO) : "memory");
-        }
-        tmem_ld_wait();
+        m_ref[hh] = (mx[hh] == -INFINITY) ? 0.f : mx[hh];
+      } else if (mx[hh] > m_ref[hh] + 8.f) {
+        const float corr = exp2f(m_ref[hh] - mx[hh]);
+        m_ref[hh] = mx[hh];
 #pragma unroll
-        for (int i = 0; i < OC; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * corr);
-        if constexpr (OC == 32) {
-          tmem_st_32x32(tO, ov);
-        } else {
-          asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-                       ::"r"(tO), "r"(ov[0]), "r"(ov[1]), "r"(ov[2]), "r"(ov[3]), "r"(ov[4]), "r"(ov[5]), "r"(ov[6]), "r"(ov[7]), "r"(ov[8]),
-                       "r"(ov[9]), "r"(ov[10]), "r"(ov[11]), "r"(ov[12]), "r"(ov[13]), "r"(ov[14]), "r"(ov[15]) : "memory");
-        }
-        tmem_st_wait();
-        l_part *= corr;
-      }
-      // ---- the P buffer must have been consumed (P_{j-PB} V_{j-PB} retired) before it is overwritten
-      if constexpr (L::PB == 2) {
-        if (j >= 2) mbar_wait(&pv_done[buf], ((j >> 1) - 1) & 1);
-      } else {
-        if (j >= 1) mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);
-      }
-      // ---- p = exp2(x - m_ref) (<= 2^8), partial row sum, P (bf16) -> swizzled K-major smem tile (4 x 16 B per thread)
-      uint8_t* sub = sP + (j % L::PB) * L::P_BYTES + (cg >> 1) * SUB_BYTES + r * 128;
-      float ls = 0.f;
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float p0 = ex2_approx(fmaf(__uint_as_float(v[ch * 8 + 2 * i]), p.scale_log2, -m_ref));
-          const float p1 = ex2_approx(fmaf(__uint_as_float(v[ch * 8 + 2 * i + 1]), p.scale_log2, -m_ref));
-          ls += p0 + p1;
-          pk[i] = pack_bf16x2(p0, p1);
-        }
-        const int chunk = (cg & 1) * 4 + ch;
-        *reinterpret_cast<uint4*>(sub + ((chunk ^ (r & 7)) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      }
-      l_part += ls;
-      tc_fence_before();
-      fence_proxy_async_smem();          // P (generic-proxy stores) visible to the tensor core's async-proxy reads
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[buf]);
-    }
-    // ---- epilogue: row sum across the column groups, O / l -> bf16 (this warp's D/4 columns)
-    float* rl = red + ((nblk & 1) * 512);       // parity not used by the last block's max exchange
-    rl[cg * 128 + r] = l_part;
-    asm volatile("bar.sync %0, 128;" ::"r"(1 + qtr) : "memory");
-    const float l_run = (rl[r] + rl[128 + r]) + (rl[256 + r] + rl[384 + r]);
-    const int jl = nblk - 1;
-    mbar_wait(&pv_done[jl & 1], (jl >> 1) & 1);
-    tc_fence_after();
-    const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-    uint32_t ov[OC];
-    const uint32_t tO = tmem_O + lane_addr + cg * OC;
-    if constexpr (OC == 32) {
-      tmem_ld_32x32(tO, ov);
-    } else {
-      asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                   : "=r"(ov[0]), "=r"(ov[1]), "=r"(ov[2]), "=r"(ov[3]), "=r"(ov[4]), "=r"(ov[5]), "=r"(ov[6]), "=r"(ov[7]), "=r"(ov[8]),
-                     "=r"(ov[9]), "=r"(ov[10]), "=r"(ov[11]), "=r"(ov[12]), "=r"(ov[13]), "=r"(ov[14]), "=r"(ov[15])
-                   : "r"(tO) : "memory");
-    }
-    tmem_ld_wait();
-    if (qrow < p.Sq) {
-      bf16* dst = p.o + (long long)b * p.o_bs + (long long)qrow * p.o_rs + (long long)h * D + cg * OC;
-#pragma unroll
-      for (int i = 0; i < OC / 8; ++i) {
-        uint4 w;
-        w.x = pack_bf16x2(__uint_as_float(ov[8 * i + 0]) * inv, __uint_as_float(ov[8 * i + 1]) * inv);
-        w.y = pack_bf16x2(__uint_as_float(ov[8 * i + 2]) * inv, __uint_as_float(ov[8 * i + 3]) * inv);
-        w.z = pack_bf16x2(__uint_as_float(ov[8 * i + 4]) * inv, __uint_as_float(ov[8 * i + 5]) * inv);
-        w.w = pack_bf16x2(__uint_as_float(ov[8 * i + 6]) * inv, __uint_as_float(ov[8 * i + 7]) * inv);
-        reinterpret_cast<uint4*>(dst)[i] = w;
+        for (int jj = 0; jj < D / 8; ++jj) { o[4 * jj + 2 * hh] *= corr; o[4 * jj + 2 * hh + 1] *= corr; }
+        l_part[hh] *= corr;
       }
     }
-    tc_fence_before();
+    // ---- P = exp2(s * scale - m_ref) (<= 2^8) as bf16 A fragments: block kk of 16 keys = accumulator blocks 2kk, 2kk+1
+    uint32_t pa[BKV / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {                  // q: (block 2kk + q/2, row q%2)
+        const int hh = q & 1, base = 4 * (2 * kk + (q >> 1)) + 2 * hh;
+        const float p0 = ex2_approx(fmaf(s[base], p.scale_log2, -m_ref[hh]));
+        const float p1 = ex2_approx(fmaf(s[base + 1], p.scale_log2, -m_ref[hh]));
+        l_part[hh] += p0 + p1;
+        pa[kk][q] = pack_bf16x2(p0, p1);
+      }
+    }
+    // ---- O += P V_j
+    fence_regs<D / 2>(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) wgmma_rs_tb<D>(o, pa[kk], desc_mnmajor(aV + kk * 2048), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<D / 2>(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[stage]);      // this warp is done with K_j / V_j
+    if (++stage == ST) { stage = 0; phase ^= 1; }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------- ping-pong variant (head_dim 64): two Q tiles per CTA
-// One CTA owns 256 queries = tiles A and B of one (batch, head) and streams K/V once for both.  Softmax group A (8 warps)
-// and group B (8 warps) work on different tiles, so while one group is in its TMEM-read / MUFU phase the tensor core
-// serves the other group's S = QK^T and O += PV, and the two groups' TMEM-read and MUFU phases interleave instead of
-// running back-to-back (the single-tile kernel above is bound by exactly that serialisation: XU 46 %, tensor 22 % in ncu).
-//   TMEM: S^A @0, S^B @128, O^A @256, O^B @320.  smem: Q 2x16K, K/V ring 3x32K, P^A, P^B 32K each, row-max scratch.
-// A thread owns half a score row (64 keys): row r = 32*(warp%4) + lane of its group's tile, column half (warp-4)%8/4.
-struct ASmem2 {
-  static constexpr int KV_ST = 3;
-  static constexpr int Q_BYTES = 2 * SUB_BYTES;                    // tiles A, B (128 x 64 each)
-  static constexpr int KV_STAGE_BYTES = 2 * SUB_BYTES;             // K then V
-  static constexpr int P_BYTES = 2 * SUB_BYTES;                    // 128 x 128 bf16 per group
-  static constexpr int P_OFF = Q_BYTES + KV_ST * KV_STAGE_BYTES;
-  static constexpr int RED_OFF = P_OFF + 2 * P_BYTES;
-  static constexpr int RED_BYTES = 2 * 2 * 2 * 128 * 4;            // [group][parity][half][row]
-  static constexpr int BAR_OFF = RED_OFF + RED_BYTES;
-  static constexpr int TOTAL = BAR_OFF + 128;
-};
-
-__global__ void __launch_bounds__(640, 1)
-attn_tc2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                const AttnTcParams p) {
-  using L = ASmem2;
-  constexpr int D = 64;
-  constexpr int ST = L::KV_ST;
-  constexpr uint32_t TMEM_COLS = 512;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sQ = smem;
-  uint8_t* sKV = smem + L::Q_BYTES;
-  uint8_t* sP = smem + L::P_OFF;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::BAR_OFF);
-  uint64_t* q_full = bars + 0;
-  uint64_t* kv_full = bars + 1;                 // [ST]
-  uint64_t* kv_empty = kv_full + ST;            // [ST]
-  uint64_t* s_full = kv_empty + ST;             // [2] per group
-  uint64_t* p_full = s_full + 2;                // [2] per group: 8 warp arrivals
-  uint64_t* pv_done = p_full + 2;               // [2] per group
-  uint64_t* s_free = pv_done + 2;               // [2] per group: 8 warp arrivals (S^g is in registers, its TMEM columns are free)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(s_free + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 256, h = blockIdx.y, b = blockIdx.z;
-  const int off = p.Sk - p.Sq;
-  const bool tileB = (q0 + 128) < p.Sq;         // second tile has at least one valid row (CTA-uniform)
-  int nblk = (p.Sk + BKV - 1) / BKV;
-  if (p.causal) {
-    int last_key = q0 + 255 + off;
-    if (last_key > p.Sk - 1) last_key = p.Sk - 1;
-    if (last_key < 0) last_key = 0;
-    const int nb = last_key / BKV + 1;
-    if (nb < nblk) nblk = nb;
-  }
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-  }
-  if (warp == 1 && lane == 0) {
-    mbar_init(q_full, 1);
-    for (int s = 0; s < ST; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], tileB ? 2 : 1); }   // one commit per MMA issuer
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(&s_full[g], 1);
-      mbar_init(&p_full[g], 8);
-      mbar_init(&pv_done[g], 1);
-      mbar_init(&s_free[g], 8);
+  // ---- epilogue: row sum across the quad, O / l -> bf16
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float l = l_part[hh];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = l > 0.f ? 1.f / l : 0.f;
+    if (qrow[hh] < p.Sq) {
+      bf16* dst = p.o + (long long)b * p.o_bs + (long long)qrow[hh] * p.o_rs + (long long)h * D + 2 * t;
+#pragma unroll
+      for (int jj = 0; jj < D / 8; ++jj)
+        *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
     }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ---------------- TMA producer
-      mbar_arrive_expect_tx(q_full, L::Q_BYTES);
-      tma_load_3d(sQ, &tmQ, p.q_col0 + h * D, q0, b, q_full);
-      tma_load_3d(sQ + SUB_BYTES, &tmQ, p.q_col0 + h * D, q0 + 128, b, q_full);     // rows >= Sq arrive as zeros
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < nblk; ++j) {
-        mbar_wait(&kv_empty[stage], phase ^ 1);
-        uint8_t* dst = sKV + stage * L::KV_STAGE_BYTES;
-        mbar_arrive_expect_tx(&kv_full[stage], L::KV_STAGE_BYTES);
-        tma_load_3d(dst, &tmK, p.k_col0 + h * D, j * BKV, b, &kv_full[stage]);
-        tma_load_3d(dst + SUB_BYTES, &tmV, p.v_col0 + h * D, j * BKV, b, &kv_full[stage]);
-        if (++stage == ST) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1 || (warp == 3 && tileB)) {
-    if (lane == 0) {
-      // ---------------- MMA issuer of tile g (warp 1: tile A, warp 3: tile B).  S^g_{j+1} is issued as soon as the softmax
-      // group has pulled S^g_j into registers (s_free), i.e. while it is still exponentiating block j, so the group never
-      // waits for the tensor core; PV^g_j follows when P^g_j is in shared memory.  The two issuers interleave freely.
-      const int g = warp >> 1;
-      constexpr uint32_t idesc_s = make_idesc(128, BKV, 0);
-      constexpr uint32_t idesc_o = make_idesc(128, D, 1);
-      const uint32_t aQ = smem_u32(sQ) + g * SUB_BYTES, aP = smem_u32(sP) + g * L::P_BYTES;
-      auto issue_S = [&](int stage) {
-        const uint32_t aK = smem_u32(sKV + stage * L::KV_STAGE_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk)
-          umma_f16(tmem_base + g * 128, desc_kmajor(aQ + kk * 32), desc_kmajor(aK + kk * 32), idesc_s, kk > 0 ? 1u : 0u);
-        umma_commit(&s_full[g]);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&kv_full[0], 0);
-      tc_fence_after();
-      issue_S(0);
-      int vs = 0, ks = 1 % ST;
-      uint32_t kph = (ST == 1) ? 1 : 0;
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) {
-          mbar_wait(&kv_full[ks], kph);
-          mbar_wait(&s_free[g], j & 1);
-          tc_fence_after();
-          issue_S(ks);
-        }
-        mbar_wait(&p_full[g], j & 1);
-        tc_fence_after();
-        const uint32_t aV = smem_u32(sKV + vs * L::KV_STAGE_BYTES + SUB_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < BKV / 16; ++kk)
-          umma_f16(tmem_base + 256 + g * 64, desc_kmajor(aP + (kk >> 2) * SUB_BYTES + (kk & 3) * 32), desc_mnmajor(aV + kk * 2048), idesc_o,
-                   (j > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(&pv_done[g]);
-        umma_commit(&kv_empty[vs]);                 // this tile is done with K_j / V_j
-        if (++vs == ST) vs = 0;
-        if (++ks == ST) { ks = 0; kph ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    const int g = (warp - 4) >> 3;                // softmax group == Q tile
-    if (g == 0 || tileB) {
-      const int qtr = warp & 3;
-      const int half = ((warp - 4) & 7) >> 2;     // key-column half of the block
-      const int r = qtr * 32 + lane;
-      const int qrow = q0 + g * 128 + r;
-      const uint32_t lane_addr = (uint32_t)(qtr * 32) << 16;
-      const uint32_t tS = tmem_base + lane_addr + (uint32_t)(g * 128 + half * 64);
-      const uint32_t tO = tmem_base + lane_addr + (uint32_t)(256 + g * 64 + half * 32);
-      float* red = reinterpret_cast<float*>(smem + L::RED_OFF) + g * 512;       // [parity][half][row]
-      const int bar_id = 1 + g * 4 + qtr;                                        // the 2 warps sharing these rows
-      float m_ref = 0.f, l_part = 0.f;
-      const int kmax = p.causal ? min(qrow + off, p.Sk - 1) : (p.Sk - 1);
-
-      for (int j = 0; j < nblk; ++j) {
-        mbar_wait(&s_full[g], j & 1);
-        tc_fence_after();
-        uint32_t v[64];
-        tmem_ld_32x32(tS, v);
-        tmem_ld_32x32(tS + 32, v + 32);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_free[g]);
-        const int nvis = kmax - (j * BKV + half * 64) + 1;
-        float mx = -INFINITY;
-        if (nvis >= 64) {
-#pragma unroll
-          for (int i = 0; i < 64; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 64; ++i) {
-            if (i >= nvis) v[i] = 0xff800000u;
-            mx = fmaxf(mx, __uint_as_float(v[i]));
-          }
-        }
-        mx *= p.scale_log2;
-        float* rj = red + (j & 1) * 256;
-        rj[half * 128 + r] = mx;
-        asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
-        mx = fmaxf(rj[r], rj[128 + r]);
-        float corr = 1.f;
-        if (j == 0) {
-          m_ref = (mx == -INFINITY) ? 0.f : mx;
-        } else if (mx > m_ref + 8.f) {
-          corr = exp2f(m_ref - mx);
-          m_ref = mx;
-        }
-        // P^g (single buffer) is free and O^g holds blocks < j once P_{j-1} V_{j-1} has retired
-        if (j >= 1) { mbar_wait(&pv_done[g], (j - 1) & 1); tc_fence_after(); }
-        if (__any_sync(0xffffffffu, corr != 1.f)) {
-          // rare (lazy rescale): 8 columns at a time so the 64 live score registers are not spilled around this branch
-#pragma unroll 1
-          for (int c = 0; c < 32; c += 8) {
-            uint32_t ov[8];
-            tmem_ld_32x32_x8(tO + c, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 8; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * corr);
-            tmem_st_32x32_x8(tO + c, ov);
-          }
-          tmem_st_wait();
-          l_part *= corr;
-        }
-        uint8_t* sub = sP + g * L::P_BYTES + half * SUB_BYTES + r * 128;
-        float ls = 0.f;
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {
-          uint32_t pk[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float p0 = ex2_approx(fmaf(__uint_as_float(v[ch * 8 + 2 * i]), p.scale_log2, -m_ref));
-            const float p1 = ex2_approx(fmaf(__uint_as_float(v[ch * 8 + 2 * i + 1]), p.scale_log2, -m_ref));
-            ls += p0 + p1;
-            pk[i] = pack_bf16x2(p0, p1);
-          }
-          *reinterpret_cast<uint4*>(sub + ((ch ^ (r & 7)) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        }
-        l_part += ls;
-        tc_fence_before();
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[g]);
-      }
-      // ---- epilogue
-      float* rl = red + (nblk & 1) * 256;
-      rl[half * 128 + r] = l_part;
-      asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
-      const float l_run = rl[r] + rl[128 + r];
-      const int jl = nblk - 1;
-      mbar_wait(&pv_done[g], jl & 1);
-      tc_fence_after();
-      const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-      uint32_t ov[32];
-      tmem_ld_32x32(tO, ov);
-      tmem_ld_wait();
-      if (qrow < p.Sq) {
-        bf16* dst = p.o + (long long)b * p.o_bs + (long long)qrow * p.o_rs + (long long)h * D + half * 32;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 w;
-          w.x = pack_bf16x2(__uint_as_float(ov[8 * i + 0]) * inv, __uint_as_float(ov[8 * i + 1]) * inv);
-          w.y = pack_bf16x2(__uint_as_float(ov[8 * i + 2]) * inv, __uint_as_float(ov[8 * i + 3]) * inv);
-          w.z = pack_bf16x2(__uint_as_float(ov[8 * i + 4]) * inv, __uint_as_float(ov[8 * i + 5]) * inv);
-          w.w = pack_bf16x2(__uint_as_float(ov[8 * i + 6]) * inv, __uint_as_float(ov[8 * i + 7]) * inv);
-          reinterpret_cast<uint4*>(dst)[i] = w;
-        }
-      }
-      tc_fence_before();
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
@@ -697,13 +275,14 @@ PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// 3-D view [B][S][cols] of a strided bf16 activation; box = {64 cols, 128 rows, 1}; rows >= S are zero-filled
-int make_map3(CUtensorMap* out, const void* base, long long cols, long long S, long long B, long long row_stride, long long batch_stride) {
+// 3-D view [B][S][cols] of a strided bf16 activation; box = {64 cols, box_rows rows, 1}; rows >= S are zero-filled
+int make_map3(CUtensorMap* out, const void* base, long long cols, long long S, long long B, long long row_stride, long long batch_stride,
+              int box_rows) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) { vsb_set_error("cuTensorMapEncodeTiled entry point not available"); return VSB_ERR_CUDA; }
   cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)S, (cuuint64_t)B};
   cuuint64_t gstr[2] = {(cuuint64_t)row_stride * 2, (cuuint64_t)batch_stride * 2};
-  cuuint32_t box[3] = {64, 128, 1};
+  cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -715,20 +294,24 @@ int make_map3(CUtensorMap* out, const void* base, long long cols, long long S, l
   return VSB_OK;
 }
 
-template <int D>
-int launch(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnTcParams& p, int B, cudaStream_t st) {
-  using L = ASmem<D>;
+template <int D, int NWG>
+int launch(const void* q, const CUtensorMap& tk, const CUtensorMap& tv, long long q_rs, long long q_bs, const AttnTcParams& p, int B,
+           cudaStream_t st) {
+  using L = ASmem<D, NWG>;
+  CUtensorMap tq;
+  int r = make_map3(&tq, q, (long long)p.H * D, p.Sq, B, q_rs, q_bs, 64 * NWG);
+  if (r) return r;
   static bool set = false;
-  if (!set) { VSB_CUDA(cudaFuncSetAttribute(attn_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL)); set = true; }
-  dim3 grid((p.Sq + BQ - 1) / BQ, p.H, B);
-  attn_tc_kernel<D><<<grid, 640, L::TOTAL, st>>>(tq, tk, tv, p);
+  if (!set) { VSB_CUDA(cudaFuncSetAttribute(attn_wgmma_kernel<D, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL)); set = true; }
+  dim3 grid((p.Sq + 64 * NWG - 1) / (64 * NWG), p.H, B);
+  attn_wgmma_kernel<D, NWG><<<grid, 128 * (NWG + 1), L::TOTAL, st>>>(tq, tk, tv, p);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
 
 }  // namespace
 
-static int g_tc_variant = 0;    // 0 auto (two-tile ping-pong kernel for head_dim 64), 1 = single-tile kernel only
+static int g_tc_variant = 0;    // 0 auto (two query warpgroups per CTA sharing each K/V block), 1 = one warpgroup per CTA only
 void vsb_attn_tc_set_variant(int v) { g_tc_variant = v; }
 
 // same contract as vsb_flash_attn_bf16 (called by it for the shapes this kernel covers)
@@ -736,26 +319,16 @@ int vsb_flash_attn_tc(const void* q, const void* k, const void* v, void* o, long
                       long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk, int D, int causal,
                       float scale, cudaStream_t stream) {
   // tensor maps cover [B][S][H*D] starting at the head-0 column of q / k / v
-  CUtensorMap tq, tk, tv;
-  int r = make_map3(&tq, q, (long long)H * D, Sq, B, q_rs, q_bs);
+  CUtensorMap tk, tv;
+  int r = make_map3(&tk, k, (long long)H * D, Sk, B, k_rs, k_bs, BKV);
   if (r) return r;
-  r = make_map3(&tk, k, (long long)H * D, Sk, B, k_rs, k_bs);
-  if (r) return r;
-  r = make_map3(&tv, v, (long long)H * D, Sk, B, v_rs, v_bs);
+  r = make_map3(&tv, v, (long long)H * D, Sk, B, v_rs, v_bs, BKV);
   if (r) return r;
   AttnTcParams p;
   p.o = (bf16*)o; p.o_bs = o_bs; p.o_rs = o_rs;
   p.H = H; p.Sq = Sq; p.Sk = Sk; p.causal = causal;
-  p.q_col0 = p.k_col0 = p.v_col0 = 0;
   p.scale_log2 = scale * 1.4426950408889634f;
-  if (D == 64 && g_tc_variant != 1 && Sq > 128) {
-    static bool set2 = false;
-    if (!set2) { VSB_CUDA(cudaFuncSetAttribute(attn_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ASmem2::TOTAL)); set2 = true; }
-    dim3 grid((Sq + 255) / 256, H, B);
-    attn_tc2_kernel<<<grid, 640, ASmem2::TOTAL, stream>>>(tq, tk, tv, p);
-    VSB_LAUNCH_CHECK();
-    return VSB_OK;
-  }
-  if (D == 64) return launch<64>(tq, tk, tv, p, B, stream);
-  return launch<128>(tq, tk, tv, p, B, stream);
+  const bool two = g_tc_variant != 1 && Sq > 64;
+  if (D == 64) return two ? launch<64, 2>(q, tk, tv, q_rs, q_bs, p, B, stream) : launch<64, 1>(q, tk, tv, q_rs, q_bs, p, B, stream);
+  return two ? launch<128, 2>(q, tk, tv, q_rs, q_bs, p, B, stream) : launch<128, 1>(q, tk, tv, q_rs, q_bs, p, B, stream);
 }

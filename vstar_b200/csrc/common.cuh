@@ -1,4 +1,4 @@
-// Shared device/host helpers for the vstar_b200 sm_100a kernels.
+// Shared device/host helpers for the vstar_b200 sm_90a kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -138,7 +138,7 @@ static inline int vsb_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(128) rmsnorm_kernel(const bf16* __restrict__ x
 }
 
 // few rows (decode): one 256-thread block per row so the row's loads are all in flight at once; a single warp per row
-// (above) serialises 16 dependent-latency loads and measured 11 us for one 4096-wide row.  Same arithmetic, same rounding.
+// (above) serialises 16 dependent-latency loads.  Same arithmetic, same rounding.
 __global__ void __launch_bounds__(256) rmsnorm_row_kernel(const bf16* __restrict__ x, long long ldx, const bf16* __restrict__ w,
                                                           bf16* __restrict__ y, long long ldy, int cols, float eps) {
   pdl_prologue();
@@ -504,7 +504,7 @@ extern "C" int vsb_add_rows_bf16(const void* a, const void* b, void* y, long lon
   if (rows <= 0) return VSB_OK;
   long long n8 = rows * (cols >> 3);
   int blocks = (int)((n8 + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > vsb_num_sms() * 16) blocks = vsb_num_sms() * 16;
   add_rows_kernel<<<blocks, 256, 0, STREAM(stream)>>>((const bf16*)a, (const bf16*)b, (bf16*)y, rows, cols, bmod);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
@@ -514,7 +514,7 @@ extern "C" int vsb_cast_f32_bf16(const void* x, void* y, long long n, void* stre
   VSB_CHECK_ARG(x && y, "vsb_cast_f32_bf16: null pointer");
   if (n <= 0) return VSB_OK;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > vsb_num_sms() * 16) blocks = vsb_num_sms() * 16;
   cast_f32_bf16_kernel<<<blocks, 256, 0, STREAM(stream)>>>((const float*)x, (bf16*)y, n);
   VSB_LAUNCH_CHECK();
   return VSB_OK;

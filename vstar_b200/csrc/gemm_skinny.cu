@@ -2,8 +2,8 @@
 //
 // With one to eight activation rows every weight byte is used for <= 16 flops, so the problem is HBM-bound: the job is
 // to stream W once at full bandwidth (Vicuna-7B decode reads 13.5 GB of weights per token; SURVEY.md §8d "secondary (HBM)
-// bounds").  A 128-row tcgen05 tile wastes >= 94 % of the tensor core here and, worse, leaves most SMs without enough
-// loads in flight (measured 0.15-0.46 of the HBM roofline on the decode shapes).  This kernel keeps the machine full of
+// bounds").  A 128-row tensor-core tile wastes >= 94 % of the tensor core here and, worse, leaves most SMs without enough
+// loads in flight.  This kernel keeps the machine full of
 // outstanding 16-byte loads instead:
 //   * one warp owns two adjacent weight rows (= two output columns; for the interleaved gate/up matrix exactly one SwiGLU
 //     output) and strides over K with 16 B per lane => every load instruction of a warp covers 512 contiguous bytes of a row;
@@ -11,7 +11,7 @@
 //     allocation so the weights do not wash the activation rows out of L1;
 //   * the M activation rows are re-read through L1 (they are at most 8 x 22 KB and shared by all warps of the SM);
 //   * fp32 accumulation in the same k order for every column, butterfly reduction at the end, and the same epilogue
-//     semantics as the tcgen05 kernel (bias -> activation / SwiGLU -> + residual -> bf16 / fp32, output-row remap).
+//     semantics as the wgmma kernel (bias -> activation / SwiGLU -> + residual -> bf16 / fp32, output-row remap).
 // Algorithmic bytes per launch: 2*N*K (weights) + 2*M*K + 2*M*N.
 #include "common.cuh"
 #include "vstar_b200.h"
@@ -143,9 +143,9 @@ __global__ void __launch_bounds__(SK_THREADS) gemm_skinny_kernel(const SkinnyPar
 
 
 // ---------------------------------------------------------------- M <= 16: same weight-streaming structure on mma.sync
-// From three activation rows on, the scalar kernel above is bound by its FMA / unpack instructions.  The tcgen05 tile kernel
+// From three activation rows on, the scalar kernel above is bound by its FMA / unpack instructions.  The wgmma tile kernel
 // is no better here: its 64-wide k-blocks fetch 128 B per weight row per TMA box, a DRAM-hostile pattern when nothing is
-// reused (0.26-0.31 of the HBM roofline on the N = 4096 projections at M = 16).  This variant keeps the streaming access
+// reused.  This variant keeps the streaming access
 // pattern and lets the tensor core do the arithmetic with W as the 16-row A operand of mma.sync.m16n8k16 and the (<= 8 per
 // n-tile) activation rows as the B operand:
 //   * a block owns 16 weight rows; its 8 warps interleave over K in steps of 32 (each lane loads 16 B = 8 consecutive k of

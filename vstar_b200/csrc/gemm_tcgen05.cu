@@ -1,11 +1,12 @@
 // vsb_gemm_bf16: C[M,N] = epilogue(A[M,K] . W[N,K]^T + bias) (+ residual)
 //
-// Hand-written sm_100a GEMM: TMA (cp.async.bulk.tensor, 128B swizzle) -> shared
-// memory ring -> tcgen05.mma (kind::f16, bf16 x bf16 -> fp32 in TMEM) ->
-// tcgen05.ld epilogue (bias / activation / SwiGLU / residual / row remap) ->
+// Hand-written sm_90a GEMM: TMA (cp.async.bulk.tensor, 128B swizzle) -> shared
+// memory ring (mbarrier full / empty pairs) -> wgmma.mma_async (bf16 x bf16 ->
+// fp32 in registers) -> epilogue straight from the accumulator registers
+// (bias / activation / SwiGLU / residual / row remap / folded RMSNorm / RoPE) ->
 // global.  Persistent: one CTA per SM loops over 128 x BN output tiles; the
-// TMEM accumulator is double buffered so the epilogue of tile i overlaps the
-// MMAs of tile i+1.
+// producer keeps loading the next tile's k-blocks while the consumers run the
+// epilogue of the current one.
 //
 // This one kernel carries every nn.Linear on the hot path (reference op sites
 // H1-H3, H5, H6, H8-H10, H12-H15 of SURVEY.md §2b): CLIP/OWL patch-embed
@@ -13,11 +14,13 @@
 // lm_head, the [LOC]-row MLPs, OWL class/box heads and the SAM decoder linears
 // and 3x3 convs (im2col).
 //
-// Warp roles (256 threads): warp 0 = TMA producer (1 lane), warp 1 = MMA issuer
-// (1 lane), warp 2 = TMEM alloc/dealloc, warp 3 idle, warps 4-7 = epilogue
-// (warp w owns TMEM lanes 32*(w%4) .. +31 == output rows of the tile).
+// Warp groups (384 threads): warpgroup 0 = TMA producer (1 thread issues, the
+// rest idle with a minimal register budget), warpgroups 1 and 2 = consumers:
+// consumer c issues m64nBNk16 wgmma on rows [64c, 64c + 64) of the tile and
+// stores them.
 #include "common.cuh"
 #include "vstar_b200.h"
+#include "wgmma.cuh"
 
 #include <mutex>
 #include <unordered_map>
@@ -26,7 +29,7 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;   // 64 bf16 = 128 B = one swizzle-128B row
-constexpr int UMMA_K = 16;
+constexpr int WG_K = 16;
 
 struct GemmParams {
   void* C;
@@ -36,15 +39,14 @@ struct GemmParams {
   int M, N, K;
   int epilogue;        // VSB_EPI_*
   int out_fp32;        // C (and residual) element type: 0 bf16, 1 fp32
+  int vec2;            // C (and residual) rows allow 2-element vector access at even columns
   int rows_per_group;  // output row remap: r = (m / rpg) * group_stride + group_offset + m % rpg
   long long group_stride, group_offset;
   int tiles_m, tiles_n;
   int group_m;         // tile rasterisation band height (in m-blocks)
-  // L2 eviction priorities (0 = none): the A band of a raster group is re-read by every n-block of the group, W tiles and the
-  // output stream through once per band.  Without hints the streaming traffic evicts the band: ncu showed 2.37 GB of DRAM
-  // reads for 0.33 GB of operands on the gate|up GEMM of a 64-crop batch (profiles/r02_gemm_dram_bytes_before_hints.csv).
+  // L2 eviction priorities of the A / W tile loads (0 = none) and streaming (.cs) output stores, see vsb_gemm_set_l2_hints
   unsigned long long hint_a, hint_b;
-  int stream_out;      // output stores with .cs (evict-first) semantics
+  int stream_out;
   // RMSNorm folded into the GEMM (LlamaRMSNorm with its weight pre-multiplied into W, see vsb_gemm_rowscale_bf16):
   //   rowsq_in  [sq_in_chunks][sq_ld] fp32: partial sums of squares of the A rows -> output row m is scaled by
   //             rsqrt(sum_c rowsq_in[c][m] * sq_inv_cols + sq_eps) before bias / activation
@@ -89,7 +91,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // cute::TMA::CacheHintSm90 encodings of createpolicy.fractional.L2::evict_{first,last}.b64 (fraction 1.0)
 constexpr unsigned long long L2_EVICT_FIRST = 0x12F0000000000000ull;
@@ -111,65 +112,16 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i <- lane (base+i), v[j] <- column (base+j)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128B-swizzled shared-memory operand descriptor (cute::UMMA::SmemDescriptor):
+// K-major, 128B-swizzled shared-memory operand descriptor (cute::GMMA::GmmaDescriptor):
 //   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (8 rows * 128 B = 1024)
-//   [46,48) version=1 (sm_100) | [61,64) layout = 2 (SWIZZLE_128B)
+//   [62,64) layout = 1 (SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-
-// cute::UMMA::InstrDescriptor for kind::f16: D=f32 (bits 4-5 = 1), A=B=bf16 (bits 7-9, 10-12 = 1),
-// K-major A and B (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
 }
 
 template <int BN>
@@ -178,8 +130,7 @@ struct SmemLayout {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : (BN == 64 ? 8 : 10));
-  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;           // 8 epilogue warps x EPI_WARP_BYTES staging
-  static constexpr int BAR_OFFSET = EPI_OFFSET + 8 * 2560;
+  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;  // barriers + alignment slack
 };
 
@@ -193,7 +144,7 @@ __device__ __forceinline__ float apply_act(float x, int epi) {
 }
 
 // tile rasterisation: groups of GROUP_M m-blocks x all n-blocks, m fastest inside a group, so that the CTAs running
-// concurrently share both A and W tiles in L2 (instead of one W tile and 148 distinct A tiles)
+// concurrently share both A and W tiles in L2 (instead of one W tile and 132 distinct A tiles)
 __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int group_m, int& m_blk, int& n_blk) {
   const int per_group = group_m * tiles_n;
   const int g = t / per_group;
@@ -204,294 +155,8 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   n_blk = r / gsize;
 }
 
-// ---------------------------------------------------------------- shared epilogue: 32 fp32 accumulator columns of one row
-// bias -> activation / SwiGLU -> (+residual) -> bf16 / fp32 store (16 B vector stores when aligned)
-__device__ __forceinline__ void epilogue_store(const GemmParams& p, const uint32_t* v, long long orow, int n0, bool swiglu, float rs = 1.f) {
-    float f[32];
-#pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]) * rs;
-    if (p.bias != nullptr) {
-      if (n0 + 32 <= p.N) {
-        const uint4* bp = reinterpret_cast<const uint4*>(p.bias + n0);
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) {
-          uint4 b = __ldg(bp + j4);
-          float2 t;
-          t = unpack_bf16x2(b.x); f[j4 * 8 + 0] += t.x; f[j4 * 8 + 1] += t.y;
-          t = unpack_bf16x2(b.y); f[j4 * 8 + 2] += t.x; f[j4 * 8 + 3] += t.y;
-          t = unpack_bf16x2(b.z); f[j4 * 8 + 4] += t.x; f[j4 * 8 + 5] += t.y;
-          t = unpack_bf16x2(b.w); f[j4 * 8 + 6] += t.x; f[j4 * 8 + 7] += t.y;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (n0 + j < p.N) f[j] += bf2f(p.bias[n0 + j]);
-      }
-    }
-    if (swiglu) {
-      // interleaved weight rows: even column = gate_j, odd column = up_j -> out column (n0/2 + j)
-      const int on0 = n0 >> 1;
-      const int nout = p.N >> 1;
-      float o[16];
-#pragma unroll
-      for (int j = 0; j < 16; ++j) o[j] = silu_f(f[2 * j]) * f[2 * j + 1];
-      bf16* crow = reinterpret_cast<bf16*>(p.C) + orow * p.ldc + on0;
-      if (on0 + 16 <= nout && ((reinterpret_cast<uintptr_t>(crow) & 15) == 0)) {
-        uint4 w0, w1;
-        w0.x = pack_bf16x2(o[0], o[1]); w0.y = pack_bf16x2(o[2], o[3]); w0.z = pack_bf16x2(o[4], o[5]); w0.w = pack_bf16x2(o[6], o[7]);
-        w1.x = pack_bf16x2(o[8], o[9]); w1.y = pack_bf16x2(o[10], o[11]); w1.z = pack_bf16x2(o[12], o[13]); w1.w = pack_bf16x2(o[14], o[15]);
-        reinterpret_cast<uint4*>(crow)[0] = w0;
-        reinterpret_cast<uint4*>(crow)[1] = w1;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (on0 + j < nout) crow[j] = f2bf(o[j]);
-      }
-      return;
-    }
-    if (p.epilogue == VSB_EPI_QUICK_GELU) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = quick_gelu_f(f[j]);
-    } else if (p.epilogue == VSB_EPI_RELU) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-    } else if (p.epilogue == VSB_EPI_GELU) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = gelu_erf_f(f[j]);
-    }
-    const bool full = (n0 + 32 <= p.N);
-    if (p.out_fp32) {
-      float* crow = reinterpret_cast<float*>(p.C) + orow * p.ldc + n0;
-      const float* rrow = p.residual ? reinterpret_cast<const float*>(p.residual) + orow * p.ldr + n0 : nullptr;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        if (full || n0 + j < p.N) {
-          float x = f[j];
-          if (rrow) x += rrow[j];
-          crow[j] = x;
-        }
-      }
-    } else {
-      bf16* crow = reinterpret_cast<bf16*>(p.C) + orow * p.ldc + n0;
-      const bf16* rrow = p.residual ? reinterpret_cast<const bf16*>(p.residual) + orow * p.ldr + n0 : nullptr;
-      const bool vec_ok = full && ((reinterpret_cast<uintptr_t>(crow) & 15) == 0) &&
-                          (rrow == nullptr || (reinterpret_cast<uintptr_t>(rrow) & 15) == 0);
-      if (vec_ok) {
-        if (rrow) {
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            uint4 r = reinterpret_cast<const uint4*>(rrow)[j4];
-            float2 t;
-            t = unpack_bf16x2(r.x); f[j4 * 8 + 0] += t.x; f[j4 * 8 + 1] += t.y;
-            t = unpack_bf16x2(r.y); f[j4 * 8 + 2] += t.x; f[j4 * 8 + 3] += t.y;
-            t = unpack_bf16x2(r.z); f[j4 * 8 + 4] += t.x; f[j4 * 8 + 5] += t.y;
-            t = unpack_bf16x2(r.w); f[j4 * 8 + 6] += t.x; f[j4 * 8 + 7] += t.y;
-          }
-        }
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) {
-          uint4 w;
-          w.x = pack_bf16x2(f[j4 * 8 + 0], f[j4 * 8 + 1]);
-          w.y = pack_bf16x2(f[j4 * 8 + 2], f[j4 * 8 + 3]);
-          w.z = pack_bf16x2(f[j4 * 8 + 4], f[j4 * 8 + 5]);
-          w.w = pack_bf16x2(f[j4 * 8 + 6], f[j4 * 8 + 7]);
-          reinterpret_cast<uint4*>(crow)[j4] = w;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          if (full || n0 + j < p.N) {
-            float x = f[j];
-            if (rrow) x += bf2f(rrow[j]);
-            crow[j] = f2bf(x);
-          }
-        }
-      }
-    }
-}
-
-// ---------------------------------------------------------------- coalesced epilogue through a per-warp smem stage
-// A warp owns 32 rows x 32 accumulator columns (thread = row).  Writing rows straight from registers makes every 16-byte
-// store instruction touch 32 different rows (32 half-used sectors); for short-K GEMMs (OWL-ViT / CLIP, K = 768 / 1024) the
-// epilogue, not the MMA, then bounds the kernel.  Here the bf16 row segments (64 B) go through a 32 x 80 B staging buffer
-// (80-byte pitch: conflict-free for both phases) and leave as 8 rows x 64 B per instruction, fully used sectors; the
-// residual comes in the same way.  Ragged / unaligned / fp32 outputs fall back to epilogue_store.
-constexpr int EPI_PITCH = 80;
-constexpr int EPI_WARP_BYTES = 32 * EPI_PITCH;   // 2560
-
-__device__ __forceinline__ void store_out(const GemmParams& p, uint4* dst, const uint4& w) {
-  if (p.stream_out) __stcs(dst, w); else *dst = w;
-}
-
 __device__ __forceinline__ long long remap_row(const GemmParams& p, int m) {
   return (long long)(m / p.rows_per_group) * p.group_stride + p.group_offset + (m % p.rows_per_group);
-}
-
-// m_base = first row of this warp's 32 rows; v = this thread's (row m_base+lane) 32 fp32 accumulator columns at n0
-__device__ __forceinline__ bool epilogue_fast_path(const GemmParams& p, int n0, bool swiglu) {
-  const int ocols = swiglu ? 16 : 32;                       // output columns produced by this chunk
-  const int on0 = swiglu ? (n0 >> 1) : n0;
-  const int nout = swiglu ? (p.N >> 1) : p.N;
-  return !p.out_fp32 && (on0 + ocols <= nout) && ((p.ldc & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) &&
-         (p.residual == nullptr || (((p.ldr & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0)));
-}
-
-// coalesced prefetch of the residual block (32 rows x 32 bf16) of a chunk into registers; issued one chunk ahead so the
-// DRAM/L2 latency hides behind the TMEM load and the math of the current chunk
-__device__ __forceinline__ void prefetch_residual(const GemmParams& p, int m_base, int lane, int n0, bool swiglu, uint4* r) {
-  if (p.residual == nullptr || n0 >= p.N || !epilogue_fast_path(p, n0, swiglu)) return;
-#pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int m = m_base + it * 8 + (lane >> 2);
-    r[it] = make_uint4(0, 0, 0, 0);
-    if (m < p.M) r[it] = *reinterpret_cast<const uint4*>(reinterpret_cast<const bf16*>(p.residual) + remap_row(p, m) * p.ldr + n0 + (lane & 3) * 8);
-  }
-}
-
-__device__ __forceinline__ void epilogue_store_staged(const GemmParams& p, const uint32_t* v, uint8_t* stage, int m_base, int lane, int n0,
-                                                      bool swiglu, const uint4* rpre, float rs = 1.f) {
-  const int on0 = swiglu ? (n0 >> 1) : n0;
-  const bool fast = epilogue_fast_path(p, n0, swiglu);
-  if (!fast) {                                              // warp-uniform
-    const int m = m_base + lane;
-    if (m < p.M && n0 < p.N) epilogue_store(p, v, remap_row(p, m), n0, swiglu, rs);
-    return;
-  }
-  float f[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]) * rs;
-  if (p.bias != nullptr) {
-    const uint4* bp = reinterpret_cast<const uint4*>(p.bias + n0);
-#pragma unroll
-    for (int j4 = 0; j4 < 4; ++j4) {
-      uint4 b = __ldg(bp + j4);
-      float2 t;
-      t = unpack_bf16x2(b.x); f[j4 * 8 + 0] += t.x; f[j4 * 8 + 1] += t.y;
-      t = unpack_bf16x2(b.y); f[j4 * 8 + 2] += t.x; f[j4 * 8 + 3] += t.y;
-      t = unpack_bf16x2(b.z); f[j4 * 8 + 4] += t.x; f[j4 * 8 + 5] += t.y;
-      t = unpack_bf16x2(b.w); f[j4 * 8 + 6] += t.x; f[j4 * 8 + 7] += t.y;
-    }
-  }
-  uint8_t* myrow = stage + lane * EPI_PITCH;
-  if (swiglu) {
-    // 16 outputs (32 B) per row; coalesced phase: lane -> (row = 16*it + lane/2, half = lane%2), 2 iterations
-    uint32_t o[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) o[j] = pack_bf16x2(silu_f(f[4 * j]) * f[4 * j + 1], silu_f(f[4 * j + 2]) * f[4 * j + 3]);
-    reinterpret_cast<uint4*>(myrow)[0] = make_uint4(o[0], o[1], o[2], o[3]);
-    reinterpret_cast<uint4*>(myrow)[1] = make_uint4(o[4], o[5], o[6], o[7]);
-    __syncwarp();
-#pragma unroll
-    for (int it = 0; it < 2; ++it) {
-      const int rr = it * 16 + (lane >> 1), ch = lane & 1;
-      const int m = m_base + rr;
-      if (m < p.M) {
-        const uint4 w = *reinterpret_cast<const uint4*>(stage + rr * EPI_PITCH + ch * 16);
-        store_out(p, reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(p.C) + remap_row(p, m) * p.ldc + on0 + ch * 8), w);
-      }
-    }
-    __syncwarp();
-    return;
-  }
-  if (p.epilogue == VSB_EPI_QUICK_GELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = quick_gelu_f(f[j]);
-  } else if (p.epilogue == VSB_EPI_RELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
-  } else if (p.epilogue == VSB_EPI_GELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = gelu_erf_f(f[j]);
-  }
-  if (p.residual != nullptr) {
-    // residual rows were fetched coalesced (lane -> row 8*it + lane/4, chunk lane%4) one chunk ahead: park them in the stage
-#pragma unroll
-    for (int it = 0; it < 4; ++it) *reinterpret_cast<uint4*>(stage + (it * 8 + (lane >> 2)) * EPI_PITCH + (lane & 3) * 16) = rpre[it];
-    __syncwarp();
-#pragma unroll
-    for (int j4 = 0; j4 < 4; ++j4) {
-      const uint4 r = reinterpret_cast<const uint4*>(myrow)[j4];
-      float2 t;
-      t = unpack_bf16x2(r.x); f[j4 * 8 + 0] += t.x; f[j4 * 8 + 1] += t.y;
-      t = unpack_bf16x2(r.y); f[j4 * 8 + 2] += t.x; f[j4 * 8 + 3] += t.y;
-      t = unpack_bf16x2(r.z); f[j4 * 8 + 4] += t.x; f[j4 * 8 + 5] += t.y;
-      t = unpack_bf16x2(r.w); f[j4 * 8 + 6] += t.x; f[j4 * 8 + 7] += t.y;
-    }
-    __syncwarp();
-  }
-  if (p.rowsq_out != nullptr) {
-    // sum of squares of this row's 32 output values AS STORED (bf16): the next GEMM reads exactly these and normalises with them
-    float sq = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) { const float r = rbf(f[j]); sq = fmaf(r, r, sq); }
-    const int m = m_base + lane;
-    if (m < p.M) p.rowsq_out[(long long)(n0 >> 5) * p.sq_ld + remap_row(p, m)] = sq;
-  }
-#pragma unroll
-  for (int j4 = 0; j4 < 4; ++j4) {
-    uint4 w;
-    w.x = pack_bf16x2(f[j4 * 8 + 0], f[j4 * 8 + 1]);
-    w.y = pack_bf16x2(f[j4 * 8 + 2], f[j4 * 8 + 3]);
-    w.z = pack_bf16x2(f[j4 * 8 + 4], f[j4 * 8 + 5]);
-    w.w = pack_bf16x2(f[j4 * 8 + 6], f[j4 * 8 + 7]);
-    reinterpret_cast<uint4*>(myrow)[j4] = w;
-  }
-  __syncwarp();
-#pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    const int rr = it * 8 + (lane >> 2), ch = lane & 3;
-    const int m = m_base + rr;
-    if (m < p.M) {
-      const uint4 w = *reinterpret_cast<const uint4*>(stage + rr * EPI_PITCH + ch * 16);
-      store_out(p, reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(p.C) + remap_row(p, m) * p.ldc + n0 + ch * 8), w);
-    }
-  }
-  __syncwarp();
-}
-
-// RoPE on one head half pair: a = accumulator columns [j0, j0+32) of a 128-wide head, b = columns [j0+64, j0+96) of the same row.
-// x = bf16(acc * rs) is what the un-fused path stores and rope_kernel reads back; the rotated values are returned as fp32 bit
-// patterns that are exactly representable in bf16 (the store path's rounding is then the identity).
-__device__ __forceinline__ void rope_pair(uint32_t* a, uint32_t* b, float rs, const bf16* __restrict__ cr, const bf16* __restrict__ sr) {
-#pragma unroll
-  for (int j4 = 0; j4 < 4; ++j4) {
-    const uint4 c = __ldg(reinterpret_cast<const uint4*>(cr) + j4);
-    const uint4 s = __ldg(reinterpret_cast<const uint4*>(sr) + j4);
-    const uint32_t cw[4] = {c.x, c.y, c.z, c.w}, sw[4] = {s.x, s.y, s.z, s.w};
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float2 cs = unpack_bf16x2(cw[q]), sn = unpack_bf16x2(sw[q]);
-      const int j = j4 * 8 + q * 2;
-      const float x1a = rbf(__uint_as_float(a[j]) * rs), x1b = rbf(__uint_as_float(a[j + 1]) * rs);
-      const float x2a = rbf(__uint_as_float(b[j]) * rs), x2b = rbf(__uint_as_float(b[j + 1]) * rs);
-      a[j] = __float_as_uint(rbf(rbf(x1a * cs.x) + rbf(-x2a * sn.x)));
-      a[j + 1] = __float_as_uint(rbf(rbf(x1b * cs.y) + rbf(-x2b * sn.y)));
-      b[j] = __float_as_uint(rbf(rbf(x2a * cs.x) + rbf(x1a * sn.x)));
-      b[j + 1] = __float_as_uint(rbf(rbf(x2b * cs.y) + rbf(x1b * sn.y)));
-    }
-  }
-}
-
-// Epilogue of one warp for a 256-wide q/k tile with fused RoPE: its four 32-column chunks are one 128-wide head; chunk pairs (0,2)
-// and (1,3) are rotated together.  Only the ROPE instantiations of the kernels (the QKV projection) contain this code, so the
-// register allocation of every other GEMM is untouched.
-__device__ __forceinline__ void rope_epilogue_tile(const GemmParams& p, uint32_t tbase, uint8_t* stage, int m, int m_base, int lane, int n_tile0,
-                                                int chalf, float rs) {
-  const int pos = (m < p.M) ? (p.rope_pos ? p.rope_pos[m] : p.rope_pos0 + (m % p.rope_T)) : 0;
-  const bf16* cr = p.rope_cos + (long long)pos * 64;
-  const bf16* sr = p.rope_sin + (long long)pos * 64;
-  uint4 rdummy[4];
-#pragma unroll 1
-  for (int cc = 0; cc < 2; ++cc) {
-    const int c_lo = chalf * 4 + cc, c_hi = c_lo + 2;
-    uint32_t va[32], vb[32];
-    tmem_ld_32x32(tbase + c_lo * 32, va);
-    tmem_ld_32x32(tbase + c_hi * 32, vb);
-    tmem_ld_wait();
-    rope_pair(va, vb, rs, cr + cc * 32, sr + cc * 32);
-    epilogue_store_staged(p, va, stage, m_base, lane, n_tile0 + c_lo * 32, false, rdummy, 1.f);
-    epilogue_store_staged(p, vb, stage, m_base, lane, n_tile0 + c_hi * 32, false, rdummy, 1.f);
-  }
 }
 
 // 1 / rms of A row m from the partial sums a producer GEMM (or vsb_rowsq_bf16) left behind; fixed summation order
@@ -502,52 +167,159 @@ __device__ __forceinline__ float row_rstd(const GemmParams& p, int m) {
   return rsqrtf(s * p.sq_inv_cols + p.sq_eps);
 }
 
-constexpr int GEMM_THREADS = 384;   // warps 0-3: TMA / MMA / TMEM-alloc / spare; warps 4-11: epilogue (2 per TMEM lane quarter)
+// ---------------------------------------------------------------- epilogue of one accumulator pair
+// row orow (already remapped), columns n, n+1 (n even, n < N): bias -> activation / SwiGLU -> (+residual) -> bf16 / fp32 store.
+// Returns the sum of squares of the bf16 values stored (the folded-RMSNorm row statistics).
+__device__ __forceinline__ float epilogue_pair(const GemmParams& p, long long orow, int n, float x0, float x1, bool swiglu) {
+  const bool has1 = n + 1 < p.N;
+  if (p.bias != nullptr) {
+    x0 += bf2f(p.bias[n]);
+    if (has1) x1 += bf2f(p.bias[n + 1]);
+  }
+  if (swiglu) {
+    // interleaved weight rows: even column = gate_j, odd column = up_j -> out column n/2 (N is even)
+    reinterpret_cast<bf16*>(p.C)[orow * p.ldc + (n >> 1)] = f2bf(silu_f(x0) * x1);
+    return 0.f;
+  }
+  x0 = apply_act(x0, p.epilogue);
+  x1 = apply_act(x1, p.epilogue);
+  if (p.out_fp32) {
+    float* c = reinterpret_cast<float*>(p.C) + orow * p.ldc + n;
+    const float* r = p.residual ? reinterpret_cast<const float*>(p.residual) + orow * p.ldr + n : nullptr;
+    if (has1 && p.vec2) {
+      if (r) { const float2 rv = *reinterpret_cast<const float2*>(r); x0 += rv.x; x1 += rv.y; }
+      *reinterpret_cast<float2*>(c) = make_float2(x0, x1);
+    } else {
+      if (r) { x0 += r[0]; if (has1) x1 += r[1]; }
+      c[0] = x0;
+      if (has1) c[1] = x1;
+    }
+    return 0.f;
+  }
+  bf16* c = reinterpret_cast<bf16*>(p.C) + orow * p.ldc + n;
+  const bf16* r = p.residual ? reinterpret_cast<const bf16*>(p.residual) + orow * p.ldr + n : nullptr;
+  if (has1 && p.vec2) {
+    if (r) { const float2 rv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(r)); x0 += rv.x; x1 += rv.y; }
+    const uint32_t w = pack_bf16x2(x0, x1);
+    if (p.stream_out) __stcs(reinterpret_cast<unsigned int*>(c), w); else *reinterpret_cast<uint32_t*>(c) = w;
+  } else {
+    if (r) { x0 += bf2f(r[0]); if (has1) x1 += bf2f(r[1]); }
+    c[0] = f2bf(x0);
+    if (has1) c[1] = f2bf(x1);
+  }
+  const float s0 = rbf(x0), s1 = has1 ? rbf(x1) : 0.f;
+  return fmaf(s1, s1, s0 * s0);
+}
+
+// RoPE on a 256-wide q/k tile (two heads of 128): accumulator column i of a head (i < 64) pairs with column i + 64, i.e.
+// fragment block j with j + 8.  x = bf16(acc * rs) is what the un-fused path stores and rope_kernel reads back; the rotated
+// values are exactly representable in bf16 (the store path's rounding is then the identity).
+__device__ __forceinline__ void rope_tile(const GemmParams& p, float* acc, const int* m, const float* rs, int t) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int pos = (m[h] < p.M) ? (p.rope_pos ? p.rope_pos[m[h]] : p.rope_pos0 + (m[h] % p.rope_T)) : 0;
+    const bf16* cr = p.rope_cos + (long long)pos * 64;
+    const bf16* sr = p.rope_sin + (long long)pos * 64;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int i = 8 * jj + 2 * t;
+      const float2 cs = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(cr + i)));
+      const float2 sn = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(sr + i)));
+#pragma unroll
+      for (int head = 0; head < 2; ++head) {
+        const int ja = 16 * head + jj, jb = ja + 8;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float c = e ? cs.y : cs.x, s = e ? sn.y : sn.x;
+          float& a = acc[4 * ja + 2 * h + e];
+          float& b = acc[4 * jb + 2 * h + e];
+          const float x1 = rbf(a * rs[h]), x2 = rbf(b * rs[h]);
+          a = rbf(rbf(x1 * c) + rbf(-x2 * s));
+          b = rbf(rbf(x2 * c) + rbf(x1 * s));
+        }
+      }
+    }
+  }
+}
+
+// Epilogue of one consumer thread: rows m[0], m[1] of the tile, fragment columns 8j + 2t (see wgmma.cuh)
+template <int BN, bool ROPE>
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, int m0, int n_blk, int t) {
+  const int m[2] = {m0, m0 + 8};
+  float rs[2] = {row_rstd(p, m[0]), row_rstd(p, m[1])};
+  const bool ok[2] = {m[0] < p.M, m[1] < p.M};
+  const long long orow[2] = {ok[0] ? remap_row(p, m[0]) : 0, ok[1] ? remap_row(p, m[1]) : 0};
+  const bool swiglu = (p.epilogue == VSB_EPI_SWIGLU);
+  const int n_tile0 = n_blk * BN;
+  if constexpr (ROPE) {
+    if (n_tile0 < p.rope_cols) {
+      rope_tile(p, acc, m, rs, t);
+      rs[0] = rs[1] = 1.f;
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < (BN + 31) / 32; ++c) {      // 32-column chunks (the granularity of the row statistics)
+    const int n0 = n_tile0 + 32 * c;
+    if (n0 >= p.N) break;                          // warp-uniform
+    float sq[2] = {0.f, 0.f};
+#pragma unroll
+    for (int jj = 0; jj < 4 && 8 * (4 * c + jj) < BN; ++jj) {
+      const int j = 4 * c + jj;
+      const int n = n0 + 8 * jj + 2 * t;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (ok[h] && n < p.N) sq[h] += epilogue_pair(p, orow[h], n, acc[4 * j + 2 * h] * rs[h], acc[4 * j + 2 * h + 1] * rs[h], swiglu);
+    }
+    if (p.rowsq_out != nullptr) {                  // N % 32 == 0: every chunk is complete
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 1);
+        sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 2);
+        if (t == 0 && ok[h]) p.rowsq_out[(long long)(n0 >> 5) * p.sq_ld + orow[h]] = sq[h];
+      }
+    }
+  }
+}
+
+template <int N>
+__device__ __forceinline__ void fence_acc(float* acc) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+}
+
+constexpr int GEMM_THREADS = 384;   // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma consumers + epilogue
 
 template <int BN, bool ROPE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using L = SmemLayout<BN>;
   constexpr int STAGES = L::STAGES;
-  constexpr uint32_t TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;   // double-buffered accumulator (power of 2: 128/256/512)
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
   const int num_kb = (p.K + BK - 1) / BK;
   const int num_tiles = p.tiles_m * p.tiles_n;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], 8);   // one arrive per epilogue warp
+      mbar_init(&empty_bar[s], 8);   // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -564,324 +336,42 @@ gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-          const uint32_t sb = sa + L::A_BYTES;
-          const uint64_t da = make_smem_desc(sa);
-          const uint64_t db = make_smem_desc(sb);
+    return;
+  }
+
+  // ===================== consumers =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int cw = wg - 1;                        // rows [64 cw, 64 cw + 64) of the tile
+  const int wq = (threadIdx.x >> 5) & 3;        // warp inside the warpgroup: 16 rows each
+  float acc[BN / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int m_blk, n_blk;
+    tile_coords(tile, p.tiles_m, p.tiles_n, p.group_m, m_blk, n_blk);
+    int prev = -1;
+    fence_acc<BN / 2>(acc);
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES) + cw * (64 * 128);
+      const uint32_t sb = smem_u32(smem + stage * L::STAGE_BYTES) + L::A_BYTES;
+      const uint64_t da = make_smem_desc(sa);
+      const uint64_t db = make_smem_desc(sb);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            // advance 16 bf16 = 32 B along K inside the 128B swizzle row: +2 in the (addr>>4) field
-            umma_f16(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);   // frees this smem stage once the MMAs have read it
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);       // accumulator complete
-      }
+      for (int k = 0; k < BK / WG_K; ++k)
+        // advance 16 bf16 = 32 B along K inside the 128B swizzle row: +2 in the (addr>>4) field
+        wgmma_ss<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1 : 0);
+      wgmma_commit();
+      wgmma_wait<1>();                            // the k-block before this one has been consumed: free its stage
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    // 8 warps: warp w reads TMEM lanes 32*(w%4).. (hardware rule) and the column half (w-4)/4 of the tile, so that two warps
-    // per SM sub-partition overlap TMEM-load / MUFU / store latencies (the epilogue bounds short-K GEMMs otherwise)
-    const int q = warp & 3;                 // TMEM lane quarter
-    const int chalf = (warp - 4) >> 2;      // column half
-    constexpr int CPH = (BN / 32 + 1) / 2;  // 32-column chunks per half
-    int it = 0;
-    const bool swiglu = (p.epilogue == VSB_EPI_SWIGLU);
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      int m_blk, n_blk;
-      tile_coords(tile, p.tiles_m, p.tiles_n, p.group_m, m_blk, n_blk);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int m = m_blk * BM + q * 32 + lane;
-      const float rs = row_rstd(p, m);        // (folded RMSNorm) fetched while the tile's MMAs are still running
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const bool row_ok = m < p.M;
-      long long orow = 0;
-      if (row_ok) orow = (long long)(m / p.rows_per_group) * p.group_stride + p.group_offset + (m % p.rows_per_group);
-      const int c_end = min((chalf + 1) * CPH, BN / 32);
-      const int m_base = m_blk * BM + q * 32;
-      if (ROPE && BN == 256 && n_blk * BN < p.rope_cols) {
-        if constexpr (ROPE && BN == 256)
-          rope_epilogue_tile(p, tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN), smem + L::EPI_OFFSET + (warp - 4) * EPI_WARP_BYTES,
-                             m, m_base, lane, n_blk * BN, chalf, rs);
-      } else {
-      uint4 rnext[4];
-      prefetch_residual(p, m_base, lane, n_blk * BN + chalf * CPH * 32, swiglu, rnext);
-#pragma unroll 1
-      for (int c = chalf * CPH; c < c_end; ++c) {
-        uint4 rcur[4] = {rnext[0], rnext[1], rnext[2], rnext[3]};
-        if (c + 1 < c_end) prefetch_residual(p, m_base, lane, n_blk * BN + (c + 1) * 32, swiglu, rnext);
-        uint32_t v[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN + c * 32);
-        tmem_ld_32x32(taddr, v);
-        tmem_ld_wait();
-        const int n0 = n_blk * BN + c * 32;
-        if (n0 >= p.N) continue;                      // warp-uniform
-        epilogue_store_staged(p, v, smem + L::EPI_OFFSET + (warp - 4) * EPI_WARP_BYTES, m_base, lane, n0, swiglu, rcur, rs);
-      }
-      }   // (no fused RoPE on this tile)
-      // release this accumulator buffer to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-
-// ---------------------------------------------------------------- 2-CTA (cta_group::2) variant
-// A CTA pair (cluster 2x1x1, two SMs of one TPC) computes a 256 x 256 tile: CTA r owns A rows / D rows
-// [m0 + 128 r, +128) and HALF of the B tile (W rows [n0 + 128 r, +128)); one `tcgen05.mma.cta_group::2` issued by the
-// leader CTA multiplies the 256-row A (both CTAs' smem) with the 256-row B (both halves).  Per CTA and k-block only
-// (128 + 128) x 64 bf16 = 32 KB come from L2 instead of (128 + 256) x 64: -33 % L2->SM traffic, which is what bounds the
-// single-CTA kernel on the big 7B shapes.  Synchronisation follows the CUTLASS sm100 2SM pipelines:
-//   * both CTAs' TMA loads complete_tx on the LEADER's full barrier (cta_group::2 TMA, peer bit of the mbarrier address
-//     cleared); the leader's producer arms it with the bytes of both CTAs;
-//   * the leader's tcgen05.commit multicasts to the empty barriers (and to the accumulator-full barriers) of both CTAs;
-//   * the epilogue warps of both CTAs arrive on the LEADER's accumulator-empty barrier (remote mbarrier arrive).
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // cute::Sm100MmaPeerBitMask: shared::cluster address of the pair's even CTA
-
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* tm, int c0, int c1, uint64_t* leader_bar,
-                                                unsigned long long hint = 0) {
-  if (hint)
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1), "l"(hint)
-        : "memory");
-  else
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit -> arrive on the barrier at this smem offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_2sm_mcast(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-      "}" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-
-struct Smem2 {
-  static constexpr int A_BYTES = BM * BK * 2;          // 128 rows of A
-  static constexpr int B_BYTES = 128 * BK * 2;         // this CTA's half of the 256-row B tile
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = 6;
-  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFFSET = EPI_OFFSET + 8 * 2560;
-  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;
-};
-
-template <bool ROPE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tcgen05_2cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using L = Smem2;
-  constexpr int STAGES = L::STAGES;
-  constexpr int BN2 = 256;                 // cluster tile N (and accumulator columns per CTA)
-  constexpr uint32_t TMEM_COLS = 512;      // 2 accumulator buffers x 256 columns
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = (rank == 0);
-  const int num_kb = (p.K + BK - 1) / BK;
-  const int num_tiles = p.tiles_m * p.tiles_n;       // cluster tiles (256 x 256)
-  const int cluster_id = blockIdx.x >> 1;
-  const int num_clusters = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);       // leader's producer arrive (+ tx bytes of both CTAs); unused in the peer
-      mbar_init(&empty_bar[s], 1);      // one multicast commit from the leader's MMA thread
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);      // one multicast commit
-      mbar_init(&tempty_bar[a], 16);    // 8 epilogue warps x 2 CTAs (leader's copy is the one used)
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc_2sm(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                   // peer barriers initialised + both TMEM allocations done
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        int m_blk, n_blk;
-        tile_coords(tile, p.tiles_m, p.tiles_n, p.group_m, m_blk, n_blk);
-        const int row_a = m_blk * 256 + (int)rank * 128;
-        const int row_b = n_blk * BN2 + (int)rank * 128;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * L::STAGE_BYTES;
-          uint8_t* sb = sa + L::A_BYTES;
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * L::STAGE_BYTES);
-          tma_load_2d_2sm(sa, &tmA, kb * BK, row_a, &full_bar[stage], p.hint_a);
-          tma_load_2d_2sm(sb, &tmB, kb * BK, row_b, &full_bar[stage], p.hint_b);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = make_idesc(256, BN2);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN2);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-          const uint32_t sb = sa + L::A_BYTES;
-          const uint64_t da = make_smem_desc(sa);
-          const uint64_t db = make_smem_desc(sb);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k)
-            umma_f16_2sm(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit_2sm_mcast(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm_mcast(&tfull_bar[acc]);
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue (both CTAs, own 128 rows x 256 columns) =====================
-    const int q = warp & 3;
-    const int chalf = (warp - 4) >> 2;
-    int it = 0;
-    const bool swiglu = (p.epilogue == VSB_EPI_SWIGLU);
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++it) {
-      int m_blk, n_blk;
-      tile_coords(tile, p.tiles_m, p.tiles_n, p.group_m, m_blk, n_blk);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int m = m_blk * 256 + (int)rank * 128 + q * 32 + lane;
-      const float rs = row_rstd(p, m);        // (folded RMSNorm) fetched while the tile's MMAs are still running
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const bool row_ok = m < p.M;
-      long long orow = 0;
-      if (row_ok) orow = (long long)(m / p.rows_per_group) * p.group_stride + p.group_offset + (m % p.rows_per_group);
-      const int c_end = (chalf + 1) * (BN2 / 64);
-      const int m_base = m_blk * 256 + (int)rank * 128 + q * 32;
-      if (ROPE && n_blk * BN2 < p.rope_cols) {
-        if constexpr (ROPE)
-          rope_epilogue_tile(p, tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN2), smem + L::EPI_OFFSET + (warp - 4) * EPI_WARP_BYTES,
-                             m, m_base, lane, n_blk * BN2, chalf, rs);
-      } else {
-      uint4 rnext[4];
-      prefetch_residual(p, m_base, lane, n_blk * BN2 + chalf * (BN2 / 64) * 32, swiglu, rnext);
-#pragma unroll 1
-      for (int c = chalf * (BN2 / 64); c < c_end; ++c) {
-        uint4 rcur[4] = {rnext[0], rnext[1], rnext[2], rnext[3]};
-        if (c + 1 < c_end) prefetch_residual(p, m_base, lane, n_blk * BN2 + (c + 1) * 32, swiglu, rnext);
-        uint32_t v[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN2 + c * 32);
-        tmem_ld_32x32(taddr, v);
-        tmem_ld_wait();
-        const int n0 = n_blk * BN2 + c * 32;
-        if (n0 >= p.N) continue;                      // warp-uniform
-        epilogue_store_staged(p, v, smem + L::EPI_OFFSET + (warp - 4) * EPI_WARP_BYTES, m_base, lane, n0, swiglu, rcur, rs);
-      }
-      }   // (no fused RoPE on this tile)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tempty_bar[acc], 0);     // leader's accumulator-empty barrier
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();       // nobody leaves (or frees TMEM) while the pair may still touch its smem / barriers / TMEM
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, TMEM_COLS);
+    wgmma_wait<0>();
+    fence_acc<BN / 2>(acc);
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    epilogue_tile<BN, ROPE>(p, acc, m_blk * BM + cw * 64 + wq * 16 + (lane >> 2), n_blk, lane & 3);
   }
 }
 
@@ -964,44 +454,29 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, i
   using L = SmemLayout<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    VSB_CUDA(cudaFuncSetAttribute(gemm_bf16_tcgen05_kernel<BN, ROPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
+    VSB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN, ROPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
     attr_set = true;
   }
   p.tiles_m = (p.M + BM - 1) / BM;
   p.tiles_n = (p.N + BN - 1) / BN;
   int tiles = p.tiles_m * p.tiles_n;
   int grid = tiles < max_ctas ? tiles : max_ctas;
-  gemm_bf16_tcgen05_kernel<BN, ROPE><<<grid, GEMM_THREADS, L::TOTAL, stream>>>(tmA, tmB, p);
+  gemm_bf16_wgmma_kernel<BN, ROPE><<<grid, GEMM_THREADS, L::TOTAL, stream>>>(tmA, tmB, p);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
 
-template <bool ROPE>
-int launch_gemm_2cta(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, int max_ctas, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    VSB_CUDA(cudaFuncSetAttribute(gemm_bf16_tcgen05_2cta_kernel<ROPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem2::TOTAL));
-    attr_set = true;
-  }
-  p.tiles_m = (p.M + 255) / 256;
-  p.tiles_n = (p.N + 255) / 256;
-  const int tiles = p.tiles_m * p.tiles_n;
-  int clusters = max_ctas / 2;
-  if (clusters > tiles) clusters = tiles;
-  if (clusters < 1) clusters = 1;
-  gemm_bf16_tcgen05_2cta_kernel<ROPE><<<2 * clusters, GEMM_THREADS, Smem2::TOTAL, stream>>>(tmA, tmB, p);
-  VSB_LAUNCH_CHECK();
-  return VSB_OK;
-}
-
-int g_l2_hints = 4;      // bit mask of L2 eviction hints on the 2-CTA kernel; 4 (streaming output stores) measured best (profiles/r02_gemm_l2_hint_sweep.csv)
-int g_force_bn = 0;      // 64/128/256 = single-CTA tile width; 512 = force the 2-CTA 256x256 kernel; 0 = auto
+int g_l2_hints = 0;      // bit mask of L2 eviction hints on large GEMMs (see gemm_dispatch); 0 = none
+int g_force_bn = 0;      // 32/64/128/256 = tile width; 1 / 2 = force a skinny decode kernel; 0 = auto
 int g_max_ctas = 0;
 int g_group_m = 0;
 
 }  // namespace
 
 extern "C" int vsb_gemm_set_tuning(int force_bn, int max_ctas) {
+  VSB_CHECK_ARG(force_bn == 0 || force_bn == 1 || force_bn == 2 || force_bn == 32 || force_bn == 64 || force_bn == 128 || force_bn == 256,
+                "vsb_gemm_set_tuning: force_bn %d is none of 0, 1, 2, 32, 64, 128, 256", force_bn);
+  VSB_CHECK_ARG(max_ctas >= 0, "vsb_gemm_set_tuning: max_ctas %d < 0", max_ctas);
   g_force_bn = force_bn;
   g_max_ctas = max_ctas;
   return VSB_OK;
@@ -1088,7 +563,7 @@ extern "C" int vsb_gemm_bf16(const void* A, long long lda, const void* W, long l
 //                      normalised copy of the activations
 //   rowsq_out != NULL: additionally writes, for every output row and 32-column chunk, the sum of squares of the bf16 values it
 //                      stored: rowsq_out[(n/32)*sq_ld + row]; the next folded GEMM consumes them with sq_in_chunks = N/32.
-// bf16 output, N % 32 == 0 when rowsq_out is given.  Always the tcgen05 kernels (any M).
+// bf16 output, N % 32 == 0 when rowsq_out is given.  Always the wgmma tile kernels (any M).
 extern "C" int vsb_gemm_rowscale_bf16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
                                       int K, const void* bias, const void* residual, long long ldr, int epilogue, int rows_per_group,
                                       long long group_stride, long long group_offset, const void* rowsq_in, int sq_in_chunks, float eps,
@@ -1197,15 +672,14 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
   p.rope_pos0 = rsq ? rsq->rope_pos0 : 0;
   p.rope_cols = rsq ? rsq->rope_cols : 0;
 
-  // decode-sized problems are HBM-bound on W: CUDA-core streaming kernel (gemm_skinny.cu); force_bn = 1 forces it (tests)
-  // measured (tools/bench_vqa.py, CUDA-graph timing, fraction of the HBM roofline): FMA kernel 0.57-0.96 at M = 1; mma.sync
-  // kernel 0.44-0.79 for M = 2..8 (and ahead of the tcgen05 tiles on N <= 8192 up to M = 16); tcgen05 tiles 0.26-0.76 at M = 16
+  // decode-sized problems are HBM-bound on W: weight-streaming kernels (gemm_skinny.cu): the FMA kernel at M = 1, the mma.sync
+  // kernel up to M = 8 (up to M = 16 when N <= 8192); force_bn = 1 / 2 forces one of them (tests)
   if ((K % 8) == 0 && !(vsb_batch_invariant() && g_force_bn == 0) && rsq == nullptr) {
     int variant = 0;
     if (g_force_bn == 1 && M <= 8) variant = 1;
     else if (g_force_bn == 2 && M <= 16) variant = 2;
     else if (g_force_bn == 0 && M == 1) variant = 1;
-    else if (g_force_bn == 0 && (M <= 8 || (M <= 16 && N <= 8192))) variant = 2;   // measured per shape, tools/bench_vqa.py
+    else if (g_force_bn == 0 && (M <= 8 || (M <= 16 && N <= 8192))) variant = 2;
     if (variant)
       return vsb_gemm_skinny_launch(variant, A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group,
                                     group_stride, group_offset, stream);
@@ -1236,30 +710,21 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
   CUtensorMap tmA, tmB;
   int r = make_tensor_map(&tmA, A, M, K, lda, BM);
   if (r) return r;
-  // 2-CTA 256x256 cluster tiles: chosen when the problem fills the machine with them (less L2->SM traffic per flop)
-  bool use_2cta = (g_force_bn == 512);
-  if (g_force_bn == 0 && M >= 512 && N >= 512 && K >= 1024) {   // short K: the single-CTA 128x256 kernel measured ~5 % faster
-    const long long t2 = (long long)((M + 255) / 256) * ((N + 255) / 256);
-    const long long waves2 = (t2 + sms / 2 - 1) / (sms / 2);
-    const double eff2 = (double)t2 / (double)(waves2 * (sms / 2));      // wave-quantisation efficiency of the 256x256 tiling
-    const double fill = ((double)M * N) / ((double)((M + 255) / 256 * 256) * ((N + 255) / 256 * 256));
-    use_2cta = eff2 * fill >= 0.80;
-  }
   p.hint_a = p.hint_b = 0;
   p.stream_out = 0;
-  if (use_2cta) {
-    // bit 0: A tiles evict_last (the band of A rows is re-read by every n-block of its raster group), bit 1: W tiles
-    // evict_first, bit 3: W tiles evict_last, bit 2: output stores with .cs (streaming) semantics
+  if (g_force_bn == 0 && M >= 512 && N >= 512 && K >= 1024) {
+    // large GEMMs, optional L2 policy (vsb_gemm_set_l2_hints): bit 0: A tiles evict_last (the band of A rows is re-read by every
+    // n-block of its raster group), bit 1: W tiles evict_first, bit 3: W tiles evict_last, bit 2: output stores with .cs semantics
     if (g_l2_hints & 1) p.hint_a = L2_EVICT_LAST;
     if (g_l2_hints & 2) p.hint_b = L2_EVICT_FIRST;
     if (g_l2_hints & 8) p.hint_b = L2_EVICT_LAST;
     if (g_l2_hints & 4) p.stream_out = 1;
-    p.group_m = g_group_m > 0 ? g_group_m : 16;    // 4096-row bands: measured +2 % over 2048 on the 7B shapes, A band + W still L2-friendly
-    r = make_tensor_map(&tmB, W, N, K, ldw, 128);
-    if (r) return r;
-    return p.rope_cos ? launch_gemm_2cta<true>(tmA, tmB, p, sms, stream) : launch_gemm_2cta<false>(tmA, tmB, p, sms, stream);
   }
-  if (p.rope_cos != nullptr) bn = 256;        // the fused-RoPE epilogue pairs chunks inside one 128-wide head: 256-wide tiles only
+  // 2-element (4 / 8 byte) vector access to C and the residual at even columns
+  const int esz = out_fp32 ? 4 : 2;
+  p.vec2 = (ldc % 2 == 0) && (reinterpret_cast<uintptr_t>(C) % (2 * esz) == 0) &&
+           (residual == nullptr || ((ldr % 2 == 0) && (reinterpret_cast<uintptr_t>(residual) % (2 * esz) == 0)));
+  if (p.rope_cos != nullptr) bn = 256;        // the fused-RoPE epilogue pairs columns inside one 128-wide head: 256-wide tiles only
   r = make_tensor_map(&tmB, W, N, K, ldw, bn);
   if (r) return r;
   if (bn == 256) return p.rope_cos ? launch_gemm<256, true>(tmA, tmB, p, sms, stream) : launch_gemm<256>(tmA, tmB, p, sms, stream);

@@ -566,7 +566,7 @@ extern "C" int vsb_copy2d_b16(const void* src, long long lds, void* dst, long lo
   const long long n = rows * (cols / 8);
   if (n <= 0) return VSB_OK;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > vsb_num_sms() * 8) blocks = vsb_num_sms() * 8;
   copy2d_kernel<<<(unsigned)blocks, 256, 0, STREAM(stream)>>>((const uint4*)src, lds / 8, (uint4*)dst, ldd / 8, rows, cols / 8);
   VSB_LAUNCH_CHECK();
   return VSB_OK;

@@ -1,6 +1,6 @@
 // Native runner for the Llama decoder stack on the fused-QKV cache (host code only: it sequences the kernels of this
 // library).  One C call replaces 8 x n_layers Python->ctypes round trips; at decode (one token per step, every kernel a few
-// microseconds) the Python wrappers, not the GPU, set the pace: 17 us per launch measured against 7.5 us of GPU work.
+// microseconds) the Python wrappers, not the GPU, set the pace.
 //
 // Per layer (HF LlamaDecoderLayer, transformers/models/llama/modeling_llama.py; called through
 // /root/reference/VisualSearch/model/llava/model/language_model/llava_llama.py:93-105 and
@@ -54,7 +54,7 @@ extern "C" int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, v
   // Folded RMSNorm (norm_folded: the caller multiplied ln1 into wqkv's and ln2 into wgu's columns): the QKV and gate|up GEMMs
   // read the un-normalised residual stream and scale their output rows by 1/rms in the epilogue; the o-proj and down-proj GEMMs
   // leave the per-row partial sums of squares of what they store.  Two kernels and ~0.3 GB of traffic less per layer at 64 crops.
-  // Needs the tcgen05 epilogue (row counts that would take the skinny decode kernels keep the unfused form, where ln = 1).
+  // Needs the wgmma tile epilogue (row counts that would take the skinny decode kernels keep the unfused form, where ln = 1).
   const bool fused = norm_folded && k_start == nullptr && d % 32 == 0 && (rows > 16 || vsb_batch_invariant());
   const int sqc = d / 32;                                  // partial sums per row left by a d-wide producer GEMM
   float* sq_a = reinterpret_cast<float*>(h);              // [sqc][rows]  input of the next QKV GEMM   (h itself is unused when fused)
@@ -63,7 +63,7 @@ extern "C" int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, v
     VSB_CHECK_ARG((long long)2 * sqc * rows * 4 <= rows * d * 2, "vsb_llama_layers: scratch too small for the row statistics");
     VSB_TRY(vsb_rowsq_bf16(xb, d, sq_a, (int)rows, d, stream));
   }
-  // RoPE in the QKV epilogue (head_dim 128, tcgen05 path): q / k reach the cache already rotated
+  // RoPE in the QKV epilogue (head_dim 128, wgmma tile path): q / k reach the cache already rotated
   const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && (rows > 16 || vsb_batch_invariant());
   int sq_a_chunks = 1;                                     // layer 0: one full-row sum from vsb_rowsq_bf16
   for (int li = 0; li < n_layers; ++li) {

@@ -1,5 +1,5 @@
 """VSM engine: the per-crop model evaluation of the V* guided visual search, batched over the crop
-frontier, executed entirely by the hand-written sm_100a kernels behind include/vstar_b200.h.
+frontier, executed entirely by the hand-written sm_90a kernels behind include/vstar_b200.h.
 
 Mirrors /root/reference/VisualSearch/model/VSM.py `VSMForCausalLM.inference` / `.model_forward(inference=True)`
 (:438-553, :201-364) with the restructurings SURVEY.md §2b calls out:
@@ -201,7 +201,7 @@ class CropResult:
 
 
 class LlamaClipCore:
-    """CLIP tower + Llama decoder on the sm_100a kernels with the fused-QKV cache; base of VSMEngine and VQAEngine."""
+    """CLIP tower + Llama decoder on the sm_90a kernels with the fused-QKV cache; base of VSMEngine and VQAEngine."""
 
     MAX_POSITIONS = 2048          # rows of the RoPE tables (Llama-1 / Vicuna max_position_embeddings)
 

@@ -3,7 +3,7 @@
 Same public names and conventions (SURVEY.md §8b): `parse_args`, `VSM`, `VSM.inference(image, question, mode)`,
 `visual_search(...) -> (final_step, path_length, search_successful, all_valid_boxes)`, plus the INT geometry helpers.
 
-What is different underneath (B200-first):
+What is different underneath (H100-first):
   * the controller is ITERATIVE (the reference recurses once per expanded node and dies at ~990 nodes, SURVEY.md §3B)
     but pops the very same `queue.PriorityQueue` / `Prioritize` objects in the very same push/pop sequence, so the
     expansion order (including heapq tie behaviour) is the reference's;
@@ -131,7 +131,7 @@ class Heatmap:
 
 
 class CudaScorer:
-    """Sub-patch mass of (ancestor) heat maps with the sm_100a kernels; one D2H of a few scalars per expansion."""
+    """Sub-patch mass of (ancestor) heat maps with the sm_90a kernels; one D2H of a few scalars per expansion."""
 
     def from_low_res(self, low_res, h, w):
         hm, stats = ops.heatmap(low_res.contiguous(), h, w, clamp=True, with_stats=True)

@@ -1,4 +1,4 @@
-"""SEAL VQA LLM on the sm_100a kernels — the model that brackets the visual search in `vstar_bench_eval.py`
+"""SEAL VQA LLM on the sm_90a kernels — the model that brackets the visual search in `vstar_bench_eval.py`
 (SURVEY.md §8 rows a18-a20, §8f-1).
 
   VQAWeights / VQAEngine : LlavaSearchLlamaForCausalLM (/root/reference/LLaVA/llava/model/language_model/llava_search_llama.py:56-141,
@@ -405,7 +405,7 @@ class _Past:
 class LlavaSearchModel:
     """The `model` that load_pretrained_model returns: the part of LlavaSearchLlamaForCausalLM's surface that
     /root/reference/vstar_bench_eval.py drives (generate(...) at :91-103; forward with images / with past_key_values at
-    :127-152; .config.vocab_size at :157), on the sm_100a engine.  Greedy decoding only (the benchmark uses temperature 0)."""
+    :127-152; .config.vocab_size at :157), on the sm_90a engine.  Greedy decoding only (the benchmark uses temperature 0)."""
 
     def __init__(self, engine: VQAEngine, eos_token_id=2):
         self.engine = engine

@@ -1,5 +1,5 @@
 """`VSM` — drop-in mirror of the reference's `visual_search.VSM` wrapper (/root/reference/visual_search.py:142-225)
-on top of the sm_100a engine: host-side prompt building / tokenisation / image preprocessing, the batched engine call,
+on top of the sm_90a engine: host-side prompt building / tokenisation / image preprocessing, the batched engine call,
 and the per-mode post-processing with the reference's return conventions.
 
 Also hosts the checkpoint reader for the HF key layout (SURVEY.md §8f-3) and the synthetic tokenizer used when no
@@ -585,7 +585,7 @@ class _Cfg:
 
 
 class VSMForCausalLM:
-    """Drop-in for /root/reference/VisualSearch/model/VSM.py:162-553 (inference paths only) on the sm_100a engine."""
+    """Drop-in for VisualSearch/model/VSM.py:162-553 (inference paths only) on the sm_90a engine."""
 
     def __init__(self, engine: VSMEngine, vision_tower_name="openai/clip-vit-large-patch14"):
         self.engine = engine
@@ -603,7 +603,7 @@ class VSMForCausalLM:
         """visual_search.py:157-159.  `version` = local checkpoint dir (HF shards, key layout of
         merge_lora_weights_and_save_hf_model.py:143-151); CLIP weights come from the `vision_tower` directory."""
         if torch_dtype != torch.bfloat16:
-            raise NotImplementedError("the sm_100a kernels compute in bf16 (the reference loads the VSM in bf16 too)")
+            raise NotImplementedError("the sm_90a kernels compute in bf16 (the reference loads the VSM in bf16 too)")
         cfg = config_from_hf(version)
         if loc_token_idx is not None:
             cfg.loc_token_idx = int(loc_token_idx)
