@@ -8,7 +8,11 @@
  * reference op site(s) (file:line) it replaces.
  *
  * Return value: 0 on success, negative on error (VSB_ERR_*); vsb_last_error() gives the message.
- * All matrices are row-major; "ld*" are leading dimensions in ELEMENTS; bf16 = __nv_bfloat16.
+ * All matrices are row-major; "ld*" are leading dimensions in ELEMENTS; bf16 = __nv_bfloat16, f16 = IEEE half.
+ *
+ * Every entry point the SEAL VQA LLM reaches has an _f16 twin with the _bf16 signature: same kernels instantiated for f16
+ * operands and outputs (fp32 accumulation and statistics either way), so that model runs in fp16 like the reference
+ * (LLaVA/llava/model/builder.py:43).  Pure 2-byte copies (gather_rows, patchify, copy2d) serve both types as they are.
  */
 #ifndef VSTAR_B200_H_
 #define VSTAR_B200_H_
@@ -44,6 +48,10 @@ int vsb_set_batch_invariant(int on);
 int vsb_gemm_bf16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N, int K,
                   const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
                   long long group_stride, long long group_offset, void* stream);
+/* f16 twin of vsb_gemm_bf16 (A, W, bias and a non-fp32 C / residual are f16) */
+int vsb_gemm_f16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N, int K,
+                 const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
+                 long long group_stride, long long group_offset, void* stream);
 /* vsb_gemm_bf16 with HF LlamaRMSNorm (modeling_llama.py:53-67) FOLDED IN; the norm weight must already be multiplied into W's columns.
  * rowsq_in != NULL: output row m is scaled by rsqrt(sum_c rowsq_in[c*sq_ld + m] / K + eps) before bias / activation, i.e. A is the
  * UN-normalised residual stream and 1/rms is applied in the epilogue (no norm kernel, no normalised copy of the activations).
@@ -53,6 +61,11 @@ int vsb_gemm_rowscale_bf16(const void* A, long long lda, const void* W, long lon
                            const void* bias, const void* residual, long long ldr, int epilogue, int rows_per_group, long long group_stride,
                            long long group_offset, const void* rowsq_in, int sq_in_chunks, float eps, void* rowsq_out, long long sq_ld,
                            void* stream);
+/* f16 twin of vsb_gemm_rowscale_bf16 */
+int vsb_gemm_rowscale_f16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N, int K,
+                          const void* bias, const void* residual, long long ldr, int epilogue, int rows_per_group, long long group_stride,
+                          long long group_offset, const void* rowsq_in, int sq_in_chunks, float eps, void* rowsq_out, long long sq_ld,
+                          void* stream);
 /* Fused QKV projection of a Llama layer (HF LlamaAttention q/k/v_proj + apply_rotary_pos_emb, modeling_llama.py:138-168, :199-221):
  * C = [q | k | v] = A . W^T, optional folded RMSNorm (rowsq_in as above), and rotate-half RoPE applied by the epilogue to the q and k
  * thirds (head_dim 128; cos/sin tables bf16 [max_pos, 64]; position of row m = positions[m] or pos0 + m % T), so q / k land in the KV
@@ -61,10 +74,17 @@ int vsb_gemm_qkv_rope_bf16(const void* A, long long lda, const void* W, long lon
                            int rows_per_group, long long group_stride, long long group_offset, const void* rowsq_in, int sq_in_chunks,
                            float eps, long long sq_ld, const void* cos_table, const void* sin_table, const void* positions, int T, int pos0,
                            int head_dim, void* stream);
+/* f16 twin of vsb_gemm_qkv_rope_bf16 (f16 cos/sin tables); bit-identical to vsb_gemm_f16 followed by vsb_rope_f16 */
+int vsb_gemm_qkv_rope_f16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N, int K,
+                          int rows_per_group, long long group_stride, long long group_offset, const void* rowsq_in, int sq_in_chunks,
+                          float eps, long long sq_ld, const void* cos_table, const void* sin_table, const void* positions, int T, int pos0,
+                          int head_dim, void* stream);
 /* 1 (default): vsb_llama_layers applies RoPE in the QKV GEMM epilogue (head_dim 128); 0: separate vsb_rope_bf16 launch */
 int vsb_llama_set_fuse_rope(int on);
 /* per-row sum of squares (fp32) of a bf16 matrix: the first rowsq_in of a chain of folded GEMMs (sq_in_chunks = 1) */
 int vsb_rowsq_bf16(const void* x, long long ldx, void* out_f32, int rows, int cols, void* stream);
+/* f16 twin of vsb_rowsq_bf16 */
+int vsb_rowsq_f16(const void* x, long long ldx, void* out_f32, int rows, int cols, void* stream);
 /* CUDA-event profiling of every vsb_gemm_bf16 launch (bench.py's roofline leg): begin clears the record; end synchronises
  * and returns the summed algorithmic flops (2*M*N*K), the summed event durations in ms and the launch count. */
 int vsb_gemm_profile_begin(void);
@@ -81,13 +101,21 @@ int vsb_gemm_set_l2_hints(int on);
  * HF CLIP/OWL layer_norm1/2, pre/post layernorm; SAM norm1-4, norm_final_attn; LayerNorm2d in NHWC (common.py:31-43). */
 int vsb_layernorm_bf16(const void* x, long long ldx, const void* w, const void* b, void* y, long long ldy, int rows, int cols,
                        float eps, int act, void* stream);
+/* f16 twin of vsb_layernorm_bf16 */
+int vsb_layernorm_f16(const void* x, long long ldx, const void* w, const void* b, void* y, long long ldy, int rows, int cols,
+                      float eps, int act, void* stream);
 /* HF LlamaRMSNorm (transformers/models/llama/modeling_llama.py:53-67): y = w * bf16(x * rsqrt(mean(x^2)+eps)). */
 int vsb_rmsnorm_bf16(const void* x, long long ldx, const void* w, void* y, long long ldy, int rows, int cols, float eps, void* stream);
+/* f16 twin of vsb_rmsnorm_bf16: y = w * f16(x * rsqrt(mean(x^2)+eps)), as HF LlamaRMSNorm in fp16 */
+int vsb_rmsnorm_f16(const void* x, long long ldx, const void* w, void* y, long long ldy, int rows, int cols, float eps, void* stream);
 /* rotate-half RoPE in place on the q and k thirds of a fused qkv buffer [.., 3*H*D]
  * (modeling_llama.py:117-168); cos/sin tables bf16 [max_pos, D/2]; position = positions[r] or pos0 + r % T;
  * logical row r is stored at physical row (r / T) * group_stride + group_offset + r % T (KV-cache layout). */
 int vsb_rope_bf16(void* qkv, long long ld, int rows, int T, int H, int D, int pos0, const void* cos_table, const void* sin_table,
                   const void* positions, long long group_stride, long long group_offset, void* stream);
+/* f16 twin of vsb_rope_bf16 (f16 tables; f16 rounding of each product and of the sum, as HF in fp16) */
+int vsb_rope_f16(void* qkv, long long ld, int rows, int T, int H, int D, int pos0, const void* cos_table, const void* sin_table,
+                 const void* positions, long long group_stride, long long group_offset, void* stream);
 /* embed_tokens lookup for the text slots of the spliced sequence (llava_arch.py:185-208, :235-251);
  * ids int64 [B,L] with the image placeholder at img_pos; out [B, L-1+n_img, d]. */
 int vsb_embed_splice_bf16(const void* ids, const void* table, void* out, int B, int L, int img_pos, int n_img, int d, int vocab, void* stream);
@@ -97,11 +125,17 @@ int vsb_gather_rows_bf16(const void* idx_i64, const void* table, long long ldt, 
 int vsb_patchify_bf16(const void* pixels, void* A, int B, int S, int P, int Kpad, void* stream);
 /* x[:,0] = cls + pos[0]; x[:,1:] += pos[1:] */
 int vsb_vit_add_pos_bf16(void* x, const void* cls, const void* pos, int B, int S, int C, void* stream);
+/* f16 twin of vsb_vit_add_pos_bf16 */
+int vsb_vit_add_pos_f16(void* x, const void* cls, const void* pos, int B, int S, int C, void* stream);
 /* OwlViT.get_visual_embs tail (owlvit.py:128-138): LN2(LN1(x[:,1:]) * LN1(x[:,:1])). */
 int vsb_owl_merge_bf16(const void* x, const void* w1, const void* b1, const void* w2, const void* b2, void* y, int B, int S, int C,
                        float eps, void* stream);
 int vsb_add_rows_bf16(const void* a, const void* b, void* y, long long rows, int cols, long long bmod, void* stream);
+/* f16 twin of vsb_add_rows_bf16 */
+int vsb_add_rows_f16(const void* a, const void* b, void* y, long long rows, int cols, long long bmod, void* stream);
 int vsb_cast_f32_bf16(const void* x, void* y, long long n, void* stream);
+/* f16 twin of vsb_cast_f32_bf16 (the reference's .half() of fp32 pixels) */
+int vsb_cast_f32_f16(const void* x, void* y, long long n, void* stream);
 int vsb_argmax_rows_f32(const void* x, long long ld, int rows, int n, void* idx_i32, void* val_f32, void* stream);
 /* per-row negative log-likelihood of labels under softmax(logits) — option scoring of the SEAL VQA LLM
  * (CrossEntropyLoss, /root/reference/vstar_bench_eval.py:154-159) */
@@ -133,12 +167,20 @@ typedef struct {
 int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc, int Tmax,
                      int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin, const void* positions,
                      const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded, void* scratch, void* stream);
+/* f16 twin of vsb_llama_layers: f16 weights, residual stream, cache, RoPE tables and scratch, dispatching to the _f16 kernels */
+int vsb_llama_layers_f16(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc, int Tmax,
+                         int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin, const void* positions,
+                         const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded, void* scratch, void* stream);
 
 /* softmax(QK^T*scale [+causal]) V, head_dim 64/128; element (b,s,h,d) at base + b*bs + s*rs + h*D + d.
  * HF CLIP/OWL attention (modeling_clip.py:261-329) and Llama attention (modeling_llama.py:199-221). */
 int vsb_flash_attn_bf16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,
                         long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk,
                         int D, int causal, float scale, void* stream);
+/* f16 twin of vsb_flash_attn_bf16 (P goes to P@V as f16) */
+int vsb_flash_attn_f16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,
+                       long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk,
+                       int D, int causal, float scale, void* stream);
 /* Decode attention (Sq <= 4 new rows against a long KV cache; HF Llama attention with past_key_values as driven by
  * generate(use_cache=True), /root/reference/vstar_bench_eval.py:91-103, :127-152): the keys of a head are split over a
  * cluster of 8 CTAs and combined through distributed shared memory.  k_start: optional int32 [B], first valid key of each
@@ -146,12 +188,20 @@ int vsb_flash_attn_bf16(const void* q, const void* k, const void* v, void* o, lo
 int vsb_attn_decode_bf16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,
                          long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk,
                          int D, int causal, float scale, const void* k_start, void* stream);
+/* f16 twin of vsb_attn_decode_bf16 */
+int vsb_attn_decode_f16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,
+                        long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk,
+                        int D, int causal, float scale, const void* k_start, void* stream);
 /* Causal attention with a per-row segment mask: the Sq new rows occupy keys Sk-Sq..Sk-1; row r sees keys [0, seg_lo) and
  * [q_seg[b*Sq + r], Sk-Sq+r].  One launch scores every answer option of a question on the question's cached K/V
  * (the reference runs one forward per option on past_key_values, vstar_bench_eval.py:140-152). */
 int vsb_flash_attn_seg_bf16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,
                             long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk,
                             int D, float scale, const void* q_seg_i32, int seg_lo, void* stream);
+/* f16 twin of vsb_flash_attn_seg_bf16 */
+int vsb_flash_attn_seg_f16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,
+                           long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk,
+                           int D, float scale, const void* q_seg_i32, int seg_lo, void* stream);
 /* testing hook: 0 = auto (wgmma kernel for Sq >= 64, split-KV decode kernel for Sq <= 4, mma.sync kernel between),
  * 1 = mma.sync, 2 = wgmma, 3 = wgmma with one query warpgroup per CTA only, 4 = decode kernel */
 int vsb_attn_set_impl(int impl);
@@ -159,6 +209,9 @@ int vsb_attn_set_impl(int impl);
  * and SEAL perceiver-resampler attention, head_dim 96 (LLaVA/llava/model/multimodal_projector/perceiver.py:25-77). */
 int vsb_attn_small_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o, long long ldo,
                         int B, int H, int Nq, int Nk, int D, float scale, void* stream);
+/* f16 twin of vsb_attn_small_bf16 */
+int vsb_attn_small_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o, long long ldo,
+                       int B, int H, int Nq, int Nk, int D, float scale, void* stream);
 
 /* OWL-ViT class head epilogue on y = [dense0(x) | logit_shift(x) | logit_scale(x)] (fp32) and box head epilogue
  * (modeling_owlvit.py:1043-1062; owlvit.py:63-100).  quant_bf16 != 0: logits / sigmoid scores / boxes are rounded to bf16

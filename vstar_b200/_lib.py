@@ -59,6 +59,11 @@ SIGNATURES = {
     "vsb_resample_v_u8": [c_p, c_i, c_p, c_p, c_i, c_i, c_p, c_p, c_p, ctypes.POINTER(c_f), ctypes.POINTER(c_f), c_p],
 }
 
+# f16 twins (same argument types as their _bf16 siblings): the SEAL VQA LLM in fp16
+for _name in ("vsb_gemm", "vsb_gemm_rowscale", "vsb_gemm_qkv_rope", "vsb_rowsq", "vsb_layernorm", "vsb_rmsnorm", "vsb_rope", "vsb_add_rows",
+              "vsb_vit_add_pos", "vsb_cast_f32", "vsb_flash_attn", "vsb_attn_decode", "vsb_flash_attn_seg", "vsb_attn_small"):
+    SIGNATURES[_name + "_f16"] = SIGNATURES[_name + "_bf16"]
+SIGNATURES["vsb_llama_layers_f16"] = SIGNATURES["vsb_llama_layers"]
 
 
 class LlamaLayer(ctypes.Structure):

@@ -42,6 +42,8 @@ def build_parser():
     p.add_argument("--minimum_size", default=224, type=int, help="minimum sub-image size for the termination of search")
     p.add_argument("--images-in-flight", default=8, type=int, help="images whose searches share GPU batches")
     p.add_argument("--search-batch", default=64, type=int, help="frontier crops per VSM call")
+    p.add_argument("--vqa-dtype", default="bf16", choices=("bf16", "fp16"),
+                   help="compute dtype of the SEAL VQA LLM: fp16 is the reference's (LLaVA/llava/model/builder.py:43); the VSM stays bf16")
     return p
 
 

@@ -33,15 +33,19 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t
 __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, uint32_t addr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
-__device__ __forceinline__ void mma_bf16_16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+#define VSB_MMA_16816(TY)                                                                                                    \
+  asm volatile(                                                                                                              \
+      "mma.sync.aligned.m16n8k16.row.col.f32." TY "." TY ".f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"         \
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])                                                                      \
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1))
+template <typename T>
+__device__ __forceinline__ void mma_16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
+  if constexpr (ElemT<T>::is_f16) VSB_MMA_16816(VSB_PTX_F16);
+  else VSB_MMA_16816(VSB_PTX_BF16);
 }
 
 struct AttnParams {
-  const bf16* q; const bf16* k; const bf16* v; bf16* o;
+  const void* q; const void* k; const void* v; void* o;     // element type T of the kernel (bf16 / f16)
   long long q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs;   // batch / row strides in elements; head h at +h*D
   int B, H, Sq, Sk;
   int causal;      // query i attends keys j <= i + (Sk - Sq)
@@ -56,12 +60,12 @@ struct AttnParams {
 
 constexpr int FA_BN = 64;
 
-// swizzled element offset of (row, 16B-chunk) in a [rows][D] bf16 tile
+// swizzled element offset of (row, 16B-chunk) in a [rows][D] tile of a 2-byte type
 template <int D>
 __device__ __forceinline__ int swz(int row, int chunk) { return row * D + ((chunk ^ (row & 7)) << 3); }
 
-template <int D, int ROWS>
-__device__ __forceinline__ void load_tile(bf16* s, const bf16* g, long long rs, int row0, int nrows_valid, int tid) {
+template <int D, int ROWS, typename T>
+__device__ __forceinline__ void load_tile(T* s, const T* g, long long rs, int row0, int nrows_valid, int tid) {
   constexpr int CH = D / 8;
   for (int i = tid; i < ROWS * CH; i += 128) {
     const int r = i / CH, c = i - r * CH;
@@ -73,21 +77,22 @@ __device__ __forceinline__ void load_tile(bf16* s, const bf16* g, long long rs, 
 
 // MT = m16 tiles per warp: a CTA (4 warps) owns BM = 64*MT query rows; each K/V fragment loaded from shared memory
 // (ldmatrix) is reused by the MT row tiles of the warp, halving shared-memory traffic per flop at MT = 2.
-template <int D, int MT>
+template <int D, int MT, typename T>
 __global__ void __launch_bounds__(128) flash_attn_kernel(const AttnParams p) {
+  using E = ElemT<T>;
   constexpr int BM = 64 * MT;
   extern __shared__ __align__(128) uint8_t fa_smem[];
-  bf16* sQ = reinterpret_cast<bf16*>(fa_smem);
-  bf16* sK = sQ + BM * D;               // [2][64][D]
-  bf16* sV = sK + 2 * FA_BN * D;        // [2][64][D]
+  T* sQ = reinterpret_cast<T*>(fa_smem);
+  T* sK = sQ + BM * D;                  // [2][64][D]
+  T* sV = sK + 2 * FA_BN * D;           // [2][64][D]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
   const int m_blk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int q0 = m_blk * BM;
-  const bf16* qg = p.q + (long long)b * p.q_bs + (long long)h * D;
-  const bf16* kg = p.k + (long long)b * p.k_bs + (long long)h * D;
-  const bf16* vg = p.v + (long long)b * p.v_bs + (long long)h * D;
+  const T* qg = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_bs + (long long)h * D;
+  const T* kg = reinterpret_cast<const T*>(p.k) + (long long)b * p.k_bs + (long long)h * D;
+  const T* vg = reinterpret_cast<const T*>(p.v) + (long long)b * p.v_bs + (long long)h * D;
   const int off = p.Sk - p.Sq;
 
   int n_blocks = (p.Sk + FA_BN - 1) / FA_BN;
@@ -132,8 +137,8 @@ __global__ void __launch_bounds__(128) flash_attn_kernel(const AttnParams p) {
           ldmatrix_x4(qf[mt][kk][0], qf[mt][kk][1], qf[mt][kk][2], qf[mt][kk][3],
                       smem_u32(sQ + swz<D>(wrow + mt * 16 + (lane & 15), kk * 2 + (lane >> 4))));
     }
-    const bf16* cK = sK + buf * FA_BN * D;
-    const bf16* cV = sV + buf * FA_BN * D;
+    const T* cK = sK + buf * FA_BN * D;
+    const T* cV = sV + buf * FA_BN * D;
 
     // ---- S = Q K^T : (16*MT) x 64 per warp
     float s[MT][8][4];
@@ -149,8 +154,8 @@ __global__ void __launch_bounds__(128) flash_attn_kernel(const AttnParams p) {
         ldmatrix_x4(r0, r1, r2, r3, smem_u32(cK + swz<D>(np * 16 + (lane & 7) + ((lane >> 4) << 3), kk * 2 + ((lane >> 3) & 1))));
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) {
-          mma_bf16_16816(s[mt][2 * np], qf[mt][kk], r0, r1);
-          mma_bf16_16816(s[mt][2 * np + 1], qf[mt][kk], r2, r3);
+          mma_16816<T>(s[mt][2 * np], qf[mt][kk], r0, r1);
+          mma_16816<T>(s[mt][2 * np + 1], qf[mt][kk], r2, r3);
         }
       }
     }
@@ -200,9 +205,9 @@ __global__ void __launch_bounds__(128) flash_attn_kernel(const AttnParams p) {
         const float p3 = exp2f(s[mt][i][3] - mnew[1]);
         psum[0] += p0 + p1;
         psum[1] += p2 + p3;
-        // the reference casts the softmax output to bf16 before P@V
-        pf[mt][i >> 1][(i & 1) * 2 + 0] = pack_bf16x2(p0, p1);
-        pf[mt][i >> 1][(i & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+        // the reference casts the softmax output to its dtype (bf16 / f16) before P@V
+        pf[mt][i >> 1][(i & 1) * 2 + 0] = E::pack2(p0, p1);
+        pf[mt][i >> 1][(i & 1) * 2 + 1] = E::pack2(p2, p3);
       }
 #pragma unroll
       for (int r = 0; r < 2; ++r) row_sum[mt][r] = row_sum[mt][r] * corr[r] + psum[r];
@@ -221,8 +226,8 @@ __global__ void __launch_bounds__(128) flash_attn_kernel(const AttnParams p) {
         ldmatrix_x4_trans(r0, r1, r2, r3, smem_u32(cV + swz<D>(ks * 16 + (lane & 7) + (((lane >> 3) & 1) << 3), dp * 2 + (lane >> 4))));
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) {
-          mma_bf16_16816(o_acc[mt][2 * dp], pf[mt][ks], r0, r1);
-          mma_bf16_16816(o_acc[mt][2 * dp + 1], pf[mt][ks], r2, r3);
+          mma_16816<T>(o_acc[mt][2 * dp], pf[mt][ks], r0, r1);
+          mma_16816<T>(o_acc[mt][2 * dp + 1], pf[mt][ks], r2, r3);
         }
       }
     }
@@ -243,12 +248,12 @@ __global__ void __launch_bounds__(128) flash_attn_kernel(const AttnParams p) {
 #pragma unroll
     for (int i = 0; i < D / 8; ++i) {
       const int r_lo = wrow + mt * 16 + g, r_hi = r_lo + 8;
-      *reinterpret_cast<uint32_t*>(sQ + swz<D>(r_lo, i) + 2 * t) = pack_bf16x2(o_acc[mt][i][0] * inv[0], o_acc[mt][i][1] * inv[0]);
-      *reinterpret_cast<uint32_t*>(sQ + swz<D>(r_hi, i) + 2 * t) = pack_bf16x2(o_acc[mt][i][2] * inv[1], o_acc[mt][i][3] * inv[1]);
+      *reinterpret_cast<uint32_t*>(sQ + swz<D>(r_lo, i) + 2 * t) = E::pack2(o_acc[mt][i][0] * inv[0], o_acc[mt][i][1] * inv[0]);
+      *reinterpret_cast<uint32_t*>(sQ + swz<D>(r_hi, i) + 2 * t) = E::pack2(o_acc[mt][i][2] * inv[1], o_acc[mt][i][3] * inv[1]);
     }
   }
   __syncthreads();
-  bf16* og = p.o + (long long)b * p.o_bs + (long long)h * D;
+  T* og = reinterpret_cast<T*>(p.o) + (long long)b * p.o_bs + (long long)h * D;
   constexpr int CH = D / 8;
   for (int i = tid; i < BM * CH; i += 128) {
     const int r = i / CH, c = i - r * CH;
@@ -259,11 +264,12 @@ __global__ void __launch_bounds__(128) flash_attn_kernel(const AttnParams p) {
 // ------------------------------------------------------------------------------------------------
 // small attention (SAM two-way transformer): one warp per (batch, head, query); keys strided over lanes.
 // q [B, Nq, H*D], k/v [B, Nk, H*D] contiguous rows (row stride = ld*), D in {16, 32}.
-template <int D>
-__global__ void __launch_bounds__(128) attn_small_kernel(const bf16* __restrict__ q, long long ldq, const bf16* __restrict__ k,
-                                                         long long ldk, const bf16* __restrict__ v, long long ldv,
-                                                         bf16* __restrict__ o, long long ldo, int B, int H, int Nq, int Nk,
+template <int D, typename T>
+__global__ void __launch_bounds__(128) attn_small_kernel(const T* __restrict__ q, long long ldq, const T* __restrict__ k,
+                                                         long long ldk, const T* __restrict__ v, long long ldv,
+                                                         T* __restrict__ o, long long ldo, int B, int H, int Nq, int Nk,
                                                          float scale) {
+  using E = ElemT<T>;
   const long long wid = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   const long long total = (long long)B * H * Nq;
@@ -271,11 +277,11 @@ __global__ void __launch_bounds__(128) attn_small_kernel(const bf16* __restrict_
   const int qi = wid % Nq;
   const int h = (wid / Nq) % H;
   const int b = wid / ((long long)Nq * H);
-  const bf16* qp = q + ((long long)b * Nq + qi) * ldq + h * D;
+  const T* qp = q + ((long long)b * Nq + qi) * ldq + h * D;
   float qv[D];
 #pragma unroll
   for (int d = 0; d < D; d += 2) {
-    float2 f = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(qp + d));
+    float2 f = E::unpack2(*reinterpret_cast<const uint32_t*>(qp + d));
     qv[d] = f.x * scale; qv[d + 1] = f.y * scale;
   }
   float m = -INFINITY, l = 0.f;
@@ -283,17 +289,17 @@ __global__ void __launch_bounds__(128) attn_small_kernel(const bf16* __restrict_
 #pragma unroll
   for (int d = 0; d < D; ++d) acc[d] = 0.f;
   for (int j = lane; j < Nk; j += 32) {
-    const bf16* kp = k + ((long long)b * Nk + j) * ldk + h * D;
-    const bf16* vp = v + ((long long)b * Nk + j) * ldv + h * D;
+    const T* kp = k + ((long long)b * Nk + j) * ldk + h * D;
+    const T* vp = v + ((long long)b * Nk + j) * ldv + h * D;
     float s = 0.f;
 #pragma unroll
     for (int d = 0; d < D; d += 8) {
       uint4 u = *reinterpret_cast<const uint4*>(kp + d);
       float2 f;
-      f = unpack_bf16x2(u.x); s += qv[d] * f.x + qv[d + 1] * f.y;
-      f = unpack_bf16x2(u.y); s += qv[d + 2] * f.x + qv[d + 3] * f.y;
-      f = unpack_bf16x2(u.z); s += qv[d + 4] * f.x + qv[d + 5] * f.y;
-      f = unpack_bf16x2(u.w); s += qv[d + 6] * f.x + qv[d + 7] * f.y;
+      f = E::unpack2(u.x); s += qv[d] * f.x + qv[d + 1] * f.y;
+      f = E::unpack2(u.y); s += qv[d + 2] * f.x + qv[d + 3] * f.y;
+      f = E::unpack2(u.z); s += qv[d + 4] * f.x + qv[d + 5] * f.y;
+      f = E::unpack2(u.w); s += qv[d + 6] * f.x + qv[d + 7] * f.y;
     }
     const float mn = fmaxf(m, s);
     const float c = __expf(m - mn);
@@ -303,10 +309,10 @@ __global__ void __launch_bounds__(128) attn_small_kernel(const bf16* __restrict_
     for (int d = 0; d < D; d += 8) {
       uint4 u = *reinterpret_cast<const uint4*>(vp + d);
       float2 f;
-      f = unpack_bf16x2(u.x); acc[d] = acc[d] * c + pj * f.x; acc[d + 1] = acc[d + 1] * c + pj * f.y;
-      f = unpack_bf16x2(u.y); acc[d + 2] = acc[d + 2] * c + pj * f.x; acc[d + 3] = acc[d + 3] * c + pj * f.y;
-      f = unpack_bf16x2(u.z); acc[d + 4] = acc[d + 4] * c + pj * f.x; acc[d + 5] = acc[d + 5] * c + pj * f.y;
-      f = unpack_bf16x2(u.w); acc[d + 6] = acc[d + 6] * c + pj * f.x; acc[d + 7] = acc[d + 7] * c + pj * f.y;
+      f = E::unpack2(u.x); acc[d] = acc[d] * c + pj * f.x; acc[d + 1] = acc[d + 1] * c + pj * f.y;
+      f = E::unpack2(u.y); acc[d + 2] = acc[d + 2] * c + pj * f.x; acc[d + 3] = acc[d + 3] * c + pj * f.y;
+      f = E::unpack2(u.z); acc[d + 4] = acc[d + 4] * c + pj * f.x; acc[d + 5] = acc[d + 5] * c + pj * f.y;
+      f = E::unpack2(u.w); acc[d + 6] = acc[d + 6] * c + pj * f.x; acc[d + 7] = acc[d + 7] * c + pj * f.y;
     }
     m = mn;
   }
@@ -315,17 +321,18 @@ __global__ void __launch_bounds__(128) attn_small_kernel(const bf16* __restrict_
   const float c = (m == -INFINITY) ? 0.f : __expf(m - mg);
   l = warp_sum(l * c);
   const float inv = 1.f / l;
-  bf16* op = o + ((long long)b * Nq + qi) * ldo + h * D;
+  T* op = o + ((long long)b * Nq + qi) * ldo + h * D;
 #pragma unroll
   for (int d = 0; d < D; ++d) {
     const float a = warp_sum(acc[d] * c);
-    if (lane == (d & 31)) op[d] = f2bf(a * inv);   // (d & 31): spread the writers over the lanes
+    if (lane == (d & 31)) op[d] = E::from_f(a * inv);   // (d & 31): spread the writers over the lanes
   }
 }
 
 }  // namespace
 
 // wgmma kernel (attention_tc.cu)
+template <typename T>
 int vsb_flash_attn_tc(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs, long long k_rs,
                       long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk, int D, int causal,
                       float scale, cudaStream_t stream);
@@ -344,8 +351,9 @@ constexpr int DEC_WARPS = 8;
 constexpr int DEC_MAXQ = 4;
 constexpr int DEC_U = 8;          // keys in flight per warp
 
-template <int D, int NQ>      // NQ = compile-time bound on Sq (1 for plain decode, NQ otherwise)
+template <int D, int NQ, typename T>      // NQ = compile-time bound on Sq (1 for plain decode, NQ otherwise)
 __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_kernel(const AttnParams p) {
+  using E = ElemT<T>;
   pdl_prologue();
   constexpr int EPL = D / 32;                                   // elements per lane
   cg::cluster_group cluster = cg::this_cluster();
@@ -362,9 +370,9 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_kernel(const At
   const int chunk = (p.Sk - k_first + nsplit - 1) / nsplit;
   const int k_begin = k_first + split * chunk;
   const int k_end = min(p.Sk, k_begin + chunk);
-  const bf16* qb = p.q + (long long)b * p.q_bs + (long long)h * D + lane * EPL;
-  const bf16* kb = p.k + (long long)b * p.k_bs + (long long)h * D + lane * EPL;
-  const bf16* vb = p.v + (long long)b * p.v_bs + (long long)h * D + lane * EPL;
+  const T* qb = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_bs + (long long)h * D + lane * EPL;
+  const T* kb = reinterpret_cast<const T*>(p.k) + (long long)b * p.k_bs + (long long)h * D + lane * EPL;
+  const T* vb = reinterpret_cast<const T*>(p.v) + (long long)b * p.v_bs + (long long)h * D + lane * EPL;
 
   float q[NQ][EPL], acc[NQ][EPL], m[NQ], l[NQ];
 #pragma unroll
@@ -374,12 +382,12 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_kernel(const At
 #pragma unroll
     for (int e = 0; e < EPL; ++e) {
       acc[qi][e] = 0.f;
-      q[qi][e] = (qi < p.Sq) ? bf2f(qb[(long long)qi * p.q_rs + e]) * p.scale_log2 : 0.f;
+      q[qi][e] = (qi < p.Sq) ? E::to_f(qb[(long long)qi * p.q_rs + e]) * p.scale_log2 : 0.f;
     }
   }
 
   for (int j0 = k_begin + warp; j0 < k_end; j0 += DEC_WARPS * DEC_U) {
-    // K / V rows stay packed (bf16 pairs) until they are used: 2 x EPL/2 registers per key in flight
+    // K / V rows stay packed (T pairs) until they are used: 2 x EPL/2 registers per key in flight
     uint32_t kr[DEC_U][EPL / 2], vr[DEC_U][EPL / 2];
 #pragma unroll
     for (int u = 0; u < DEC_U; ++u) {
@@ -410,7 +418,7 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_kernel(const At
           float d = 0.f;
 #pragma unroll
           for (int e = 0; e < EPL / 2; ++e) {
-            const float2 kk = unpack_bf16x2(kr[u][e]);
+            const float2 kk = E::unpack2(kr[u][e]);
             d = fmaf(q[qi][2 * e], kk.x, d);
             d = fmaf(q[qi][2 * e + 1], kk.y, d);
           }
@@ -431,7 +439,7 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_kernel(const At
             ls += pr;
 #pragma unroll
             for (int e = 0; e < EPL / 2; ++e) {
-              const float2 vv = unpack_bf16x2(vr[u][e]);
+              const float2 vv = E::unpack2(vr[u][e]);
               acc[qi][2 * e] = fmaf(pr, vv.x, acc[qi][2 * e]);
               acc[qi][2 * e + 1] = fmaf(pr, vv.y, acc[qi][2 * e + 1]);
             }
@@ -477,22 +485,22 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_kernel(const At
         a += *cluster.map_shared_rank(&c_acc[qi][d], r) * f;
         ll += *cluster.map_shared_rank(&c_l[qi], r) * f;
       }
-      p.o[(long long)b * p.o_bs + (long long)qi * p.o_rs + (long long)h * D + d] = f2bf(ll > 0.f ? a / ll : 0.f);
+      reinterpret_cast<T*>(p.o)[(long long)b * p.o_bs + (long long)qi * p.o_rs + (long long)h * D + d] = E::from_f(ll > 0.f ? a / ll : 0.f);
     }
   }
   cluster.sync();                                               // peers' shared memory must outlive rank 0's reads
 }
 
-template <int D>
+template <int D, typename T>
 static int launch_decode(const AttnParams& p, cudaStream_t st) {
   // keys of one (batch, head) are split over a cluster of 1..8 CTAs: as many as keep the machine filled about twice, but
   // not so many that a CTA gets fewer than ~64 keys (a batched decode step already has B*H independent heads)
   int splits = DEC_SPLITS;
   while (splits > 1 && ((long long)splits * p.H * p.B > 2LL * vsb_num_sms() + p.H || p.Sk / splits < 64)) splits >>= 1;
   if (p.Sq == 1)
-    VSB_CUDA(vsb_launch_pdl(attn_decode_kernel<D, 1>, dim3(splits, p.H, p.B), dim3(DEC_WARPS * 32), 0, st, splits, p));
+    VSB_CUDA(vsb_launch_pdl(attn_decode_kernel<D, 1, T>, dim3(splits, p.H, p.B), dim3(DEC_WARPS * 32), 0, st, splits, p));
   else
-    VSB_CUDA(vsb_launch_pdl(attn_decode_kernel<D, DEC_MAXQ>, dim3(splits, p.H, p.B), dim3(DEC_WARPS * 32), 0, st, splits, p));
+    VSB_CUDA(vsb_launch_pdl(attn_decode_kernel<D, DEC_MAXQ, T>, dim3(splits, p.H, p.B), dim3(DEC_WARPS * 32), 0, st, splits, p));
   return VSB_OK;
 }
 
@@ -504,7 +512,8 @@ extern "C" int vsb_attn_set_impl(int impl) {
   return VSB_OK;
 }
 
-extern "C" int vsb_attn_decode_bf16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs,
+template <typename T>
+static int attn_decode(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs,
                                     long long k_bs, long long k_rs, long long v_bs, long long v_rs, long long o_bs,
                                     long long o_rs, int B, int H, int Sq, int Sk, int D, int causal, float scale,
                                     const void* k_start, void* stream) {
@@ -515,33 +524,35 @@ extern "C" int vsb_attn_decode_bf16(const void* q, const void* k, const void* v,
                     ((uintptr_t)q & 7) == 0 && ((uintptr_t)k & 7) == 0 && ((uintptr_t)v & 7) == 0,
                 "vsb_attn_decode_bf16: q/k/v must be 8-byte aligned with strides that are multiples of 4 elements");
   AttnParams pd;
-  pd.q = (const bf16*)q; pd.k = (const bf16*)k; pd.v = (const bf16*)v; pd.o = (bf16*)o;
+  pd.q = q; pd.k = k; pd.v = v; pd.o = o;
   pd.q_bs = q_bs; pd.q_rs = q_rs; pd.k_bs = k_bs; pd.k_rs = k_rs; pd.v_bs = v_bs; pd.v_rs = v_rs; pd.o_bs = o_bs; pd.o_rs = o_rs;
   pd.B = B; pd.H = H; pd.Sq = Sq; pd.Sk = Sk; pd.causal = causal;
   pd.scale_log2 = scale * 1.4426950408889634f;
   pd.k_start = reinterpret_cast<const int*>(k_start);
-  return D == 64 ? launch_decode<64>(pd, reinterpret_cast<cudaStream_t>(stream)) : launch_decode<128>(pd, reinterpret_cast<cudaStream_t>(stream));
+  return D == 64 ? launch_decode<64, T>(pd, reinterpret_cast<cudaStream_t>(stream)) : launch_decode<128, T>(pd, reinterpret_cast<cudaStream_t>(stream));
 }
 
+template <typename T>
 static int launch_flash_mma(const AttnParams& p, int D, cudaStream_t st) {
   if (D == 64) {
     const int smem = (64 + 4 * FA_BN) * 64 * 2;
     static bool set64 = false;
-    if (!set64) { VSB_CUDA(cudaFuncSetAttribute(flash_attn_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); set64 = true; }
+    if (!set64) { VSB_CUDA(cudaFuncSetAttribute(flash_attn_kernel<64, 1, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); set64 = true; }
     dim3 grid((p.Sq + 63) / 64, p.H, p.B);
-    flash_attn_kernel<64, 1><<<grid, 128, smem, st>>>(p);
+    flash_attn_kernel<64, 1, T><<<grid, 128, smem, st>>>(p);
   } else {
     const int smem = (64 + 4 * FA_BN) * 128 * 2;
     static bool set128 = false;
-    if (!set128) { VSB_CUDA(cudaFuncSetAttribute(flash_attn_kernel<128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); set128 = true; }
+    if (!set128) { VSB_CUDA(cudaFuncSetAttribute(flash_attn_kernel<128, 1, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); set128 = true; }
     dim3 grid((p.Sq + 63) / 64, p.H, p.B);
-    flash_attn_kernel<128, 1><<<grid, 128, smem, st>>>(p);
+    flash_attn_kernel<128, 1, T><<<grid, 128, smem, st>>>(p);
   }
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
 
-extern "C" int vsb_flash_attn_bf16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs,
+template <typename T>
+static int flash_attn(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs,
                                    long long k_bs, long long k_rs, long long v_bs, long long v_rs, long long o_bs,
                                    long long o_rs, int B, int H, int Sq, int Sk, int D, int causal, float scale, void* stream) {
   VSB_CHECK_ARG(q && k && v && o, "vsb_flash_attn_bf16: null pointer");
@@ -553,23 +564,24 @@ extern "C" int vsb_flash_attn_bf16(const void* q, const void* k, const void* v, 
   VSB_CHECK_ARG(((uintptr_t)q & 15) == 0 && ((uintptr_t)k & 15) == 0 && ((uintptr_t)v & 15) == 0 && ((uintptr_t)o & 15) == 0,
                 "vsb_flash_attn_bf16: pointers must be 16-byte aligned");
   if (g_attn_impl == 4 || (g_attn_impl == 0 && Sq <= DEC_MAXQ && Sk >= 64))
-    return vsb_attn_decode_bf16(q, k, v, o, q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs, B, H, Sq, Sk, D, causal, scale, nullptr, stream);
+    return attn_decode<T>(q, k, v, o, q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs, B, H, Sq, Sk, D, causal, scale, nullptr, stream);
   if (g_attn_impl == 2 || (g_attn_impl == 0 && Sq >= 64))
-    return vsb_flash_attn_tc(q, k, v, o, q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs, B, H, Sq, Sk, D, causal, scale,
+    return vsb_flash_attn_tc<T>(q, k, v, o, q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs, B, H, Sq, Sk, D, causal, scale,
                              reinterpret_cast<cudaStream_t>(stream));
   AttnParams p;
-  p.q = (const bf16*)q; p.k = (const bf16*)k; p.v = (const bf16*)v; p.o = (bf16*)o;
+  p.q = q; p.k = k; p.v = v; p.o = o;
   p.q_bs = q_bs; p.q_rs = q_rs; p.k_bs = k_bs; p.k_rs = k_rs; p.v_bs = v_bs; p.v_rs = v_rs; p.o_bs = o_bs; p.o_rs = o_rs;
   p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk; p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
-  return launch_flash_mma(p, D, reinterpret_cast<cudaStream_t>(stream));
+  return launch_flash_mma<T>(p, D, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // Causal attention of several CONTINUATIONS of one cached prefix in one launch (answer-option scoring of the SEAL VQA LLM,
 // /root/reference/vstar_bench_eval.py:127-163, where the reference runs one forward per option on the question's
 // past_key_values): the Sq new rows sit at keys Sk-Sq .. Sk-1; row r sees keys 0..seg_lo-1 (the prefix) and
 // q_seg[b*Sq + r] .. (Sk-Sq+r) (the earlier rows of its own continuation).  mma.sync kernel (Sq is a few dozen rows).
-extern "C" int vsb_flash_attn_seg_bf16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs,
+template <typename T>
+static int flash_attn_seg(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs,
                                        long long k_bs, long long k_rs, long long v_bs, long long v_rs, long long o_bs,
                                        long long o_rs, int B, int H, int Sq, int Sk, int D, float scale, const void* q_seg_i32, int seg_lo,
                                        void* stream) {
@@ -580,16 +592,17 @@ extern "C" int vsb_flash_attn_seg_bf16(const void* q, const void* k, const void*
                     v_bs % 8 == 0 && o_bs % 8 == 0,
                 "vsb_flash_attn_seg_bf16: strides must be multiples of 8 elements (16 B)");
   AttnParams p;
-  p.q = (const bf16*)q; p.k = (const bf16*)k; p.v = (const bf16*)v; p.o = (bf16*)o;
+  p.q = q; p.k = k; p.v = v; p.o = o;
   p.q_bs = q_bs; p.q_rs = q_rs; p.k_bs = k_bs; p.k_rs = k_rs; p.v_bs = v_bs; p.v_rs = v_rs; p.o_bs = o_bs; p.o_rs = o_rs;
   p.B = B; p.H = H; p.Sq = Sq; p.Sk = Sk; p.causal = 1;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.q_seg = reinterpret_cast<const int*>(q_seg_i32);
   p.seg_lo = seg_lo;
-  return launch_flash_mma(p, D, reinterpret_cast<cudaStream_t>(stream));
+  return launch_flash_mma<T>(p, D, reinterpret_cast<cudaStream_t>(stream));
 }
 
-extern "C" int vsb_attn_small_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o,
+template <typename T>
+static int attn_small(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o,
                                    long long ldo, int B, int H, int Nq, int Nk, int D, float scale, void* stream) {
   VSB_CHECK_ARG(q && k && v && o, "vsb_attn_small_bf16: null pointer");
   VSB_CHECK_ARG(D == 16 || D == 32 || D == 96, "vsb_attn_small_bf16: head_dim %d unsupported (16/32/96)", D);
@@ -598,12 +611,53 @@ extern "C" int vsb_attn_small_bf16(const void* q, long long ldq, const void* k, 
   if (warps <= 0) return VSB_OK;
   const int blocks = (int)((warps + 3) / 4);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (D == 16)
-    attn_small_kernel<16><<<blocks, 128, 0, st>>>((const bf16*)q, ldq, (const bf16*)k, ldk, (const bf16*)v, ldv, (bf16*)o, ldo, B, H, Nq, Nk, scale);
+  if constexpr (ElemT<T>::is_f16) {
+    attn_small_kernel<96, T><<<blocks, 128, 0, st>>>((const T*)q, ldq, (const T*)k, ldk, (const T*)v, ldv, (T*)o, ldo, B, H, Nq, Nk, scale);
+  } else if (D == 16)
+    attn_small_kernel<16, T><<<blocks, 128, 0, st>>>((const T*)q, ldq, (const T*)k, ldk, (const T*)v, ldv, (T*)o, ldo, B, H, Nq, Nk, scale);
   else if (D == 32)
-    attn_small_kernel<32><<<blocks, 128, 0, st>>>((const bf16*)q, ldq, (const bf16*)k, ldk, (const bf16*)v, ldv, (bf16*)o, ldo, B, H, Nq, Nk, scale);
+    attn_small_kernel<32, T><<<blocks, 128, 0, st>>>((const T*)q, ldq, (const T*)k, ldk, (const T*)v, ldv, (T*)o, ldo, B, H, Nq, Nk, scale);
   else   // SEAL perceiver resampler: 16 heads x 96, 32 latents <-> 288 keys (LLaVA/llava/model/multimodal_projector/perceiver.py:25-77)
-    attn_small_kernel<96><<<blocks, 128, 0, st>>>((const bf16*)q, ldq, (const bf16*)k, ldk, (const bf16*)v, ldv, (bf16*)o, ldo, B, H, Nq, Nk, scale);
+    attn_small_kernel<96, T><<<blocks, 128, 0, st>>>((const T*)q, ldq, (const T*)k, ldk, (const T*)v, ldv, (T*)o, ldo, B, H, Nq, Nk, scale);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
+}
+
+// ------------------------------------------------------------------ C entry points: bf16 (VSM, default VQA engine) and f16 (VQA engine in fp16)
+#define VSB_ATTN_ENTRY(NAME, IMPL, T)                                                                                              \
+  extern "C" int NAME(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,        \
+                      long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk, \
+                      int D, int causal, float scale, void* stream) {                                                                \
+    return IMPL<T>(q, k, v, o, q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs, B, H, Sq, Sk, D, causal, scale, stream);           \
+  }
+VSB_ATTN_ENTRY(vsb_flash_attn_bf16, flash_attn, bf16)
+VSB_ATTN_ENTRY(vsb_flash_attn_f16, flash_attn, half)
+
+#define VSB_ATTN_DECODE_ENTRY(NAME, T)                                                                                             \
+  extern "C" int NAME(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,        \
+                      long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk, \
+                      int D, int causal, float scale, const void* k_start, void* stream) {                                           \
+    return attn_decode<T>(q, k, v, o, q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs, B, H, Sq, Sk, D, causal, scale, k_start, stream); \
+  }
+VSB_ATTN_DECODE_ENTRY(vsb_attn_decode_bf16, bf16)
+VSB_ATTN_DECODE_ENTRY(vsb_attn_decode_f16, half)
+
+#define VSB_ATTN_SEG_ENTRY(NAME, T)                                                                                                \
+  extern "C" int NAME(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,        \
+                      long long k_rs, long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk, \
+                      int D, float scale, const void* q_seg_i32, int seg_lo, void* stream) {                                         \
+    return flash_attn_seg<T>(q, k, v, o, q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs, B, H, Sq, Sk, D, scale, q_seg_i32, seg_lo, stream); \
+  }
+VSB_ATTN_SEG_ENTRY(vsb_flash_attn_seg_bf16, bf16)
+VSB_ATTN_SEG_ENTRY(vsb_flash_attn_seg_f16, half)
+
+extern "C" int vsb_attn_small_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o,
+                                   long long ldo, int B, int H, int Nq, int Nk, int D, float scale, void* stream) {
+  return attn_small<bf16>(q, ldq, k, ldk, v, ldv, o, ldo, B, H, Nq, Nk, D, scale, stream);
+}
+// f16: the perceiver resampler's head_dim 96 only (the SAM heads of 16 / 32 are bf16-only, like the rest of the VSM)
+extern "C" int vsb_attn_small_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o,
+                                  long long ldo, int B, int H, int Nq, int Nk, int D, float scale, void* stream) {
+  VSB_CHECK_ARG(D == 96, "vsb_attn_small_f16: head_dim %d unsupported (96)", D);
+  return attn_small<half>(q, ldq, k, ldk, v, ldv, o, ldo, B, H, Nq, Nk, D, scale, stream);
 }

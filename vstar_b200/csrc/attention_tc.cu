@@ -1,17 +1,17 @@
-// wgmma flash attention (prefill shapes): softmax(Q K^T * scale [+ causal]) V, head_dim 64 / 128, bf16, fp32 softmax.
+// wgmma flash attention (prefill shapes): softmax(Q K^T * scale [+ causal]) V, head_dim 64 / 128, bf16 or f16, fp32 softmax.
 //
 // One CTA = NWG consumer warpgroups x 64 query rows of one (batch, head) + one producer warpgroup; keys are consumed in
 // blocks of 128 that all consumer warpgroups share:
 //   S  = Q K_j^T          wgmma m64n128k16 x D/16   (A = Q tile, B = K tile, both K-major SW128 from TMA) -> registers
 //   P  = exp2(S*s - m)    on the accumulator fragments: a row lives in the 4 threads of a quad (max / sum by 2 shuffles)
-//   O += P V_j            wgmma m64nDk16 x 8         (A = P straight from registers as bf16 fragments, B = V tile as an
+//   O += P V_j            wgmma m64nDk16 x 8         (A = P straight from registers as T fragments, B = V tile as an
 //                                                     MN-major operand: V stays [key][d]) -> O accumulates in registers
 // The online-softmax rescale is lazy: the exponent reference m_ref of a row only moves when its running max grows by more
 // than 2^8 (then O and l of that row are scaled by 2^(m_old - m_new)).
 // Warpgroup 0: one thread issues the TMA loads (Q once, K/V ring via 3-D tensor maps so rows >= Sk are zero-filled).
 //
 // Replaces the mma.sync kernel of attention.cu for Sq >= 64 (CLIP S=257, OWL-ViT S=2305, 7B prefill T~320); numerics as
-// the reference: scores and softmax in fp32, P rounded to bf16 before P@V (modeling_clip.py:261-329, modeling_llama.py:199-221).
+// the reference: scores and softmax in fp32, P rounded to T before P@V (modeling_clip.py:261-329, modeling_llama.py:199-221).
 #include "common.cuh"
 #include "vstar_b200.h"
 #include "wgmma.cuh"
@@ -80,7 +80,7 @@ __device__ __forceinline__ void fence_regs(float* r) {
 }
 
 struct AttnTcParams {
-  bf16* o;
+  void* o;
   long long o_bs, o_rs;
   int H, Sq, Sk, causal;
   float scale_log2;
@@ -97,7 +97,7 @@ struct ASmem {
   static constexpr int TOTAL = BAR_OFF + 128;
 };
 
-template <int D, int NWG>
+template <int D, int NWG, typename T>
 __global__ void __launch_bounds__(128 * (NWG + 1), 1)
 attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                   const AttnTcParams p) {
@@ -186,7 +186,7 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk)
-      wgmma_ss<BKV>(s, desc_kmajor(aQ + (kk >> 2) * L::Q_SUB + (kk & 3) * 32), desc_kmajor(aK + (kk >> 2) * SUB_BYTES + (kk & 3) * 32),
+      wgmma_ss<BKV, T>(s, desc_kmajor(aQ + (kk >> 2) * L::Q_SUB + (kk & 3) * 32), desc_kmajor(aK + (kk >> 2) * SUB_BYTES + (kk & 3) * 32),
                     kk > 0 ? 1 : 0);
     wgmma_commit();
     wgmma_wait<0>();
@@ -218,7 +218,7 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         l_part[hh] *= corr;
       }
     }
-    // ---- P = exp2(s * scale - m_ref) (<= 2^8) as bf16 A fragments: block kk of 16 keys = accumulator blocks 2kk, 2kk+1
+    // ---- P = exp2(s * scale - m_ref) (<= 2^8) as T A fragments: block kk of 16 keys = accumulator blocks 2kk, 2kk+1
     uint32_t pa[BKV / 16][4];
 #pragma unroll
     for (int kk = 0; kk < BKV / 16; ++kk) {
@@ -228,14 +228,14 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         const float p0 = ex2_approx(fmaf(s[base], p.scale_log2, -m_ref[hh]));
         const float p1 = ex2_approx(fmaf(s[base + 1], p.scale_log2, -m_ref[hh]));
         l_part[hh] += p0 + p1;
-        pa[kk][q] = pack_bf16x2(p0, p1);
+        pa[kk][q] = ElemT<T>::pack2(p0, p1);
       }
     }
     // ---- O += P V_j
     fence_regs<D / 2>(o);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < BKV / 16; ++kk) wgmma_rs_tb<D>(o, pa[kk], desc_mnmajor(aV + kk * 2048), 1);
+    for (int kk = 0; kk < BKV / 16; ++kk) wgmma_rs_tb<D, T>(o, pa[kk], desc_mnmajor(aV + kk * 2048), 1);
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs<D / 2>(o);
@@ -243,7 +243,7 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     if (lane == 0) mbar_arrive(&kv_empty[stage]);      // this warp is done with K_j / V_j
     if (++stage == ST) { stage = 0; phase ^= 1; }
   }
-  // ---- epilogue: row sum across the quad, O / l -> bf16
+  // ---- epilogue: row sum across the quad, O / l -> T
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     float l = l_part[hh];
@@ -251,10 +251,10 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = l > 0.f ? 1.f / l : 0.f;
     if (qrow[hh] < p.Sq) {
-      bf16* dst = p.o + (long long)b * p.o_bs + (long long)qrow[hh] * p.o_rs + (long long)h * D + 2 * t;
+      T* dst = reinterpret_cast<T*>(p.o) + (long long)b * p.o_bs + (long long)qrow[hh] * p.o_rs + (long long)h * D + 2 * t;
 #pragma unroll
       for (int jj = 0; jj < D / 8; ++jj)
-        *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+        *reinterpret_cast<uint32_t*>(dst + 8 * jj) = ElemT<T>::pack2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
     }
   }
 }
@@ -275,16 +275,16 @@ PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// 3-D view [B][S][cols] of a strided bf16 activation; box = {64 cols, box_rows rows, 1}; rows >= S are zero-filled
+// 3-D view [B][S][cols] of a strided 2-byte activation; box = {64 cols, box_rows rows, 1}; rows >= S are zero-filled
 int make_map3(CUtensorMap* out, const void* base, long long cols, long long S, long long B, long long row_stride, long long batch_stride,
-              int box_rows) {
+              int box_rows, CUtensorMapDataType dtype) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) { vsb_set_error("cuTensorMapEncodeTiled entry point not available"); return VSB_ERR_CUDA; }
   cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)S, (cuuint64_t)B};
   cuuint64_t gstr[2] = {(cuuint64_t)row_stride * 2, (cuuint64_t)batch_stride * 2};
   cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = enc(out, dtype, 3, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     vsb_set_error("cuTensorMapEncodeTiled(3d) failed (%d): base=%p cols=%lld S=%lld B=%lld rs=%lld bs=%lld", (int)r, base, cols, S, B,
@@ -294,17 +294,17 @@ int make_map3(CUtensorMap* out, const void* base, long long cols, long long S, l
   return VSB_OK;
 }
 
-template <int D, int NWG>
+template <int D, int NWG, typename T>
 int launch(const void* q, const CUtensorMap& tk, const CUtensorMap& tv, long long q_rs, long long q_bs, const AttnTcParams& p, int B,
            cudaStream_t st) {
   using L = ASmem<D, NWG>;
   CUtensorMap tq;
-  int r = make_map3(&tq, q, (long long)p.H * D, p.Sq, B, q_rs, q_bs, 64 * NWG);
+  int r = make_map3(&tq, q, (long long)p.H * D, p.Sq, B, q_rs, q_bs, 64 * NWG, ElemT<T>::tma);
   if (r) return r;
   static bool set = false;
-  if (!set) { VSB_CUDA(cudaFuncSetAttribute(attn_wgmma_kernel<D, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL)); set = true; }
+  if (!set) { VSB_CUDA(cudaFuncSetAttribute(attn_wgmma_kernel<D, NWG, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL)); set = true; }
   dim3 grid((p.Sq + 64 * NWG - 1) / (64 * NWG), p.H, B);
-  attn_wgmma_kernel<D, NWG><<<grid, 128 * (NWG + 1), L::TOTAL, st>>>(tq, tk, tv, p);
+  attn_wgmma_kernel<D, NWG, T><<<grid, 128 * (NWG + 1), L::TOTAL, st>>>(tq, tk, tv, p);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
@@ -314,21 +314,26 @@ int launch(const void* q, const CUtensorMap& tk, const CUtensorMap& tv, long lon
 static int g_tc_variant = 0;    // 0 auto (two query warpgroups per CTA sharing each K/V block), 1 = one warpgroup per CTA only
 void vsb_attn_tc_set_variant(int v) { g_tc_variant = v; }
 
-// same contract as vsb_flash_attn_bf16 (called by it for the shapes this kernel covers)
+// same contract as vsb_flash_attn_bf16 / vsb_flash_attn_f16 (called by them for the shapes this kernel covers)
+template <typename T>
 int vsb_flash_attn_tc(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs, long long k_rs,
                       long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk, int D, int causal,
                       float scale, cudaStream_t stream) {
   // tensor maps cover [B][S][H*D] starting at the head-0 column of q / k / v
   CUtensorMap tk, tv;
-  int r = make_map3(&tk, k, (long long)H * D, Sk, B, k_rs, k_bs, BKV);
+  int r = make_map3(&tk, k, (long long)H * D, Sk, B, k_rs, k_bs, BKV, ElemT<T>::tma);
   if (r) return r;
-  r = make_map3(&tv, v, (long long)H * D, Sk, B, v_rs, v_bs, BKV);
+  r = make_map3(&tv, v, (long long)H * D, Sk, B, v_rs, v_bs, BKV, ElemT<T>::tma);
   if (r) return r;
   AttnTcParams p;
-  p.o = (bf16*)o; p.o_bs = o_bs; p.o_rs = o_rs;
+  p.o = o; p.o_bs = o_bs; p.o_rs = o_rs;
   p.H = H; p.Sq = Sq; p.Sk = Sk; p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
   const bool two = g_tc_variant != 1 && Sq > 64;
-  if (D == 64) return two ? launch<64, 2>(q, tk, tv, q_rs, q_bs, p, B, stream) : launch<64, 1>(q, tk, tv, q_rs, q_bs, p, B, stream);
-  return two ? launch<128, 2>(q, tk, tv, q_rs, q_bs, p, B, stream) : launch<128, 1>(q, tk, tv, q_rs, q_bs, p, B, stream);
+  if (D == 64) return two ? launch<64, 2, T>(q, tk, tv, q_rs, q_bs, p, B, stream) : launch<64, 1, T>(q, tk, tv, q_rs, q_bs, p, B, stream);
+  return two ? launch<128, 2, T>(q, tk, tv, q_rs, q_bs, p, B, stream) : launch<128, 1, T>(q, tk, tv, q_rs, q_bs, p, B, stream);
 }
+template int vsb_flash_attn_tc<bf16>(const void*, const void*, const void*, void*, long long, long long, long long, long long, long long,
+                                     long long, long long, long long, int, int, int, int, int, int, float, cudaStream_t);
+template int vsb_flash_attn_tc<half>(const void*, const void*, const void*, void*, long long, long long, long long, long long, long long,
+                                     long long, long long, long long, int, int, int, int, int, int, float, cudaStream_t);

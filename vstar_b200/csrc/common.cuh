@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -48,6 +49,40 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&u);
   return __bfloat1622float2(v);
 }
+
+// ---------------------------------------------------------------- element types of the kernels that run in bf16 or f16
+// T = bf16 (the VSM and the default VQA engine) or half (the SEAL VQA LLM in fp16, the reference's dtype).  The templated
+// kernels take every conversion from here, so their bf16 instantiations are the code they were before the f16 variants.
+#define VSB_PTX_BF16 "bf16"
+#define VSB_PTX_F16 "f16"
+template <typename T>
+struct ElemT;
+template <>
+struct ElemT<bf16> {
+  static constexpr bool is_f16 = false;
+  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;   // wgmma / mma.sync operand type: VSB_PTX_BF16
+  static __device__ __forceinline__ float to_f(bf16 x) { return bf2f(x); }
+  static __device__ __forceinline__ bf16 from_f(float x) { return f2bf(x); }
+  static __device__ __forceinline__ float round(float x) { return rbf(x); }
+  static __device__ __forceinline__ uint32_t pack2(float lo, float hi) { return pack_bf16x2(lo, hi); }
+  static __device__ __forceinline__ float2 unpack2(uint32_t u) { return unpack_bf16x2(u); }
+};
+template <>
+struct ElemT<half> {
+  static constexpr bool is_f16 = true;
+  static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;    // wgmma / mma.sync operand type: VSB_PTX_F16
+  static __device__ __forceinline__ float to_f(half x) { return __half2float(x); }
+  static __device__ __forceinline__ half from_f(float x) { return __float2half_rn(x); }
+  static __device__ __forceinline__ float round(float x) { return __half2float(__float2half_rn(x)); }
+  static __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
+    __half2 v = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&v);
+  }
+  static __device__ __forceinline__ float2 unpack2(uint32_t u) {
+    __half2 v = *reinterpret_cast<__half2*>(&u);
+    return __half22float2(v);
+  }
+};
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

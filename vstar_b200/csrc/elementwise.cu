@@ -12,8 +12,9 @@ namespace {
 // The whole row lives in the warp's registers (MAXV 16-byte vectors per lane), statistics by warp shuffles only - no
 // shared memory, no __syncthreads - and every lane has MAXV independent 16 B loads in flight, which is what an HBM-bound
 // row kernel needs (the previous block-per-row version sat at ~2.5 TB/s).
-template <int MAXV>
-__device__ __forceinline__ int load_row(const bf16* __restrict__ xr, int nvec, int lane, float (*v)[8]) {
+template <int MAXV, typename T>
+__device__ __forceinline__ int load_row(const T* __restrict__ xr, int nvec, int lane, float (*v)[8]) {
+  using E = ElemT<T>;
   int cnt = 0;
 #pragma unroll
   for (int i = 0; i < MAXV; ++i) {
@@ -21,37 +22,46 @@ __device__ __forceinline__ int load_row(const bf16* __restrict__ xr, int nvec, i
     if (vi < nvec) {
       const uint4 u = *reinterpret_cast<const uint4*>(xr + vi * 8);
       float2 t;
-      t = unpack_bf16x2(u.x); v[i][0] = t.x; v[i][1] = t.y;
-      t = unpack_bf16x2(u.y); v[i][2] = t.x; v[i][3] = t.y;
-      t = unpack_bf16x2(u.z); v[i][4] = t.x; v[i][5] = t.y;
-      t = unpack_bf16x2(u.w); v[i][6] = t.x; v[i][7] = t.y;
+      t = E::unpack2(u.x); v[i][0] = t.x; v[i][1] = t.y;
+      t = E::unpack2(u.y); v[i][2] = t.x; v[i][3] = t.y;
+      t = E::unpack2(u.z); v[i][4] = t.x; v[i][5] = t.y;
+      t = E::unpack2(u.w); v[i][6] = t.x; v[i][7] = t.y;
       ++cnt;
     }
   }
   return cnt;
 }
 
+template <typename T>
 __device__ __forceinline__ void unpack8(const uint4 u, float* f) {
+  using E = ElemT<T>;
   float2 t;
-  t = unpack_bf16x2(u.x); f[0] = t.x; f[1] = t.y;
-  t = unpack_bf16x2(u.y); f[2] = t.x; f[3] = t.y;
-  t = unpack_bf16x2(u.z); f[4] = t.x; f[5] = t.y;
-  t = unpack_bf16x2(u.w); f[6] = t.x; f[7] = t.y;
+  t = E::unpack2(u.x); f[0] = t.x; f[1] = t.y;
+  t = E::unpack2(u.y); f[2] = t.x; f[3] = t.y;
+  t = E::unpack2(u.z); f[4] = t.x; f[5] = t.y;
+  t = E::unpack2(u.w); f[6] = t.x; f[7] = t.y;
+}
+template <typename T>
+__device__ __forceinline__ uint4 pack8(const float* o) {
+  using E = ElemT<T>;
+  uint4 u;
+  u.x = E::pack2(o[0], o[1]); u.y = E::pack2(o[2], o[3]); u.z = E::pack2(o[4], o[5]); u.w = E::pack2(o[6], o[7]);
+  return u;
 }
 
-// y = (x - mean) * rsqrt(var + eps) * w + b ; fp32 statistics (two-pass over registers), bf16 in/out, optional GELU
-template <int MAXV>
-__global__ void __launch_bounds__(128) layernorm_kernel(const bf16* __restrict__ x, long long ldx, const bf16* __restrict__ w,
-                                                        const bf16* __restrict__ b, bf16* __restrict__ y, long long ldy,
+// y = (x - mean) * rsqrt(var + eps) * w + b ; fp32 statistics (two-pass over registers), T (bf16 / f16) in/out, optional GELU
+template <int MAXV, typename T>
+__global__ void __launch_bounds__(128) layernorm_kernel(const T* __restrict__ x, long long ldx, const T* __restrict__ w,
+                                                        const T* __restrict__ b, T* __restrict__ y, long long ldy,
                                                         int rows, int cols, float eps, int act) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (row >= rows) return;
-  const bf16* xr = x + (long long)row * ldx;
-  bf16* yr = y + (long long)row * ldy;
+  const T* xr = x + (long long)row * ldx;
+  T* yr = y + (long long)row * ldy;
   const int nvec = cols >> 3;
   float v[MAXV][8];
-  load_row<MAXV>(xr, nvec, lane, v);
+  load_row<MAXV, T>(xr, nvec, lane, v);
   float s = 0.f;
 #pragma unroll
   for (int i = 0; i < MAXV; ++i)
@@ -73,32 +83,31 @@ __global__ void __launch_bounds__(128) layernorm_kernel(const bf16* __restrict__
     const int vi = lane + i * 32;
     if (vi < nvec) {
       float wf[8], bfv[8], o[8];
-      unpack8(__ldg(reinterpret_cast<const uint4*>(w + vi * 8)), wf);
-      unpack8(__ldg(reinterpret_cast<const uint4*>(b + vi * 8)), bfv);
+      unpack8<T>(__ldg(reinterpret_cast<const uint4*>(w + vi * 8)), wf);
+      unpack8<T>(__ldg(reinterpret_cast<const uint4*>(b + vi * 8)), bfv);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         o[j] = (v[i][j] - mean) * rstd * wf[j] + bfv[j];
         if (act == VSB_EPI_GELU) o[j] = gelu_erf_f(o[j]);
       }
-      uint4 ou;
-      ou.x = pack_bf16x2(o[0], o[1]); ou.y = pack_bf16x2(o[2], o[3]); ou.z = pack_bf16x2(o[4], o[5]); ou.w = pack_bf16x2(o[6], o[7]);
-      *reinterpret_cast<uint4*>(yr + vi * 8) = ou;
+      *reinterpret_cast<uint4*>(yr + vi * 8) = pack8<T>(o);
     }
   }
 }
 
-// HF LlamaRMSNorm: y = w * bf16( x * rsqrt(mean(x^2) + eps) )     (transformers/models/llama/modeling_llama.py:53-67)
-template <int MAXV>
-__global__ void __launch_bounds__(128) rmsnorm_kernel(const bf16* __restrict__ x, long long ldx, const bf16* __restrict__ w,
-                                                      bf16* __restrict__ y, long long ldy, int rows, int cols, float eps) {
+// HF LlamaRMSNorm: y = w * T( x * rsqrt(mean(x^2) + eps) )     (transformers/models/llama/modeling_llama.py:53-67)
+template <int MAXV, typename T>
+__global__ void __launch_bounds__(128) rmsnorm_kernel(const T* __restrict__ x, long long ldx, const T* __restrict__ w,
+                                                      T* __restrict__ y, long long ldy, int rows, int cols, float eps) {
+  using E = ElemT<T>;
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (row >= rows) return;
-  const bf16* xr = x + (long long)row * ldx;
-  bf16* yr = y + (long long)row * ldy;
+  const T* xr = x + (long long)row * ldx;
+  T* yr = y + (long long)row * ldy;
   const int nvec = cols >> 3;
   float v[MAXV][8];
-  load_row<MAXV>(xr, nvec, lane, v);
+  load_row<MAXV, T>(xr, nvec, lane, v);
   float sq = 0.f;
 #pragma unroll
   for (int i = 0; i < MAXV; ++i)
@@ -112,24 +121,24 @@ __global__ void __launch_bounds__(128) rmsnorm_kernel(const bf16* __restrict__ x
     const int vi = lane + i * 32;
     if (vi < nvec) {
       float wf[8], o[8];
-      unpack8(__ldg(reinterpret_cast<const uint4*>(w + vi * 8)), wf);
+      unpack8<T>(__ldg(reinterpret_cast<const uint4*>(w + vi * 8)), wf);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = wf[j] * rbf(v[i][j] * rstd);
-      uint4 ou;
-      ou.x = pack_bf16x2(o[0], o[1]); ou.y = pack_bf16x2(o[2], o[3]); ou.z = pack_bf16x2(o[4], o[5]); ou.w = pack_bf16x2(o[6], o[7]);
-      *reinterpret_cast<uint4*>(yr + vi * 8) = ou;
+      for (int j = 0; j < 8; ++j) o[j] = wf[j] * E::round(v[i][j] * rstd);
+      *reinterpret_cast<uint4*>(yr + vi * 8) = pack8<T>(o);
     }
   }
 }
 
 // few rows (decode): one 256-thread block per row so the row's loads are all in flight at once; a single warp per row
 // (above) serialises 16 dependent-latency loads.  Same arithmetic, same rounding.
-__global__ void __launch_bounds__(256) rmsnorm_row_kernel(const bf16* __restrict__ x, long long ldx, const bf16* __restrict__ w,
-                                                          bf16* __restrict__ y, long long ldy, int cols, float eps) {
+template <typename T>
+__global__ void __launch_bounds__(256) rmsnorm_row_kernel(const T* __restrict__ x, long long ldx, const T* __restrict__ w,
+                                                          T* __restrict__ y, long long ldy, int cols, float eps) {
+  using E = ElemT<T>;
   pdl_prologue();
   __shared__ float red[32];
-  const bf16* xr = x + (long long)blockIdx.x * ldx;
-  bf16* yr = y + (long long)blockIdx.x * ldy;
+  const T* xr = x + (long long)blockIdx.x * ldx;
+  T* yr = y + (long long)blockIdx.x * ldy;
   const int nvec = cols >> 3;
   constexpr int MAXV = 4;                      // cols <= 8192
   float v[MAXV][8], wf[MAXV][8];
@@ -138,8 +147,8 @@ __global__ void __launch_bounds__(256) rmsnorm_row_kernel(const bf16* __restrict
   for (int i = 0; i < MAXV; ++i) {
     const int vi = threadIdx.x + i * 256;
     if (vi < nvec) {
-      unpack8(*reinterpret_cast<const uint4*>(xr + vi * 8), v[i]);
-      unpack8(__ldg(reinterpret_cast<const uint4*>(w + vi * 8)), wf[i]);
+      unpack8<T>(*reinterpret_cast<const uint4*>(xr + vi * 8), v[i]);
+      unpack8<T>(__ldg(reinterpret_cast<const uint4*>(w + vi * 8)), wf[i]);
 #pragma unroll
       for (int j = 0; j < 8; ++j) sq += v[i][j] * v[i][j];
     }
@@ -151,37 +160,37 @@ __global__ void __launch_bounds__(256) rmsnorm_row_kernel(const bf16* __restrict
     if (vi < nvec) {
       float o[8];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = wf[i][j] * rbf(v[i][j] * rstd);
-      uint4 ou;
-      ou.x = pack_bf16x2(o[0], o[1]); ou.y = pack_bf16x2(o[2], o[3]); ou.z = pack_bf16x2(o[4], o[5]); ou.w = pack_bf16x2(o[6], o[7]);
-      *reinterpret_cast<uint4*>(yr + vi * 8) = ou;
+      for (int j = 0; j < 8; ++j) o[j] = wf[i][j] * E::round(v[i][j] * rstd);
+      *reinterpret_cast<uint4*>(yr + vi * 8) = pack8<T>(o);
     }
   }
 }
 
 // ------------------------------------------------------------------ RoPE (rotate-half), in place on q and k
-// x' = bf16( bf16(x*cos) + bf16(rot(x)*sin) ); cos/sin come from host-built bf16 tables [max_pos, D/2]
+// x' = T( T(x*cos) + T(rot(x)*sin) ); cos/sin come from host-built T tables [max_pos, D/2]
 // (built with the same fp32 torch ops as HF: transformers/models/llama/modeling_llama.py:117-168),
-// so the rotation is bit-identical to the reference's bf16 path.  Row layout: [.., 3*H*D] = q | k | v.
+// so the rotation is bit-identical to the reference's bf16 / fp16 path.  Row layout: [.., 3*H*D] = q | k | v.
 // logical row r (0..rows) lives at physical row (r / T) * group_stride + group_offset + r % T (KV-cache layout
 // [B, Tmax, 3*H*D]); its position = positions[r] if given else pos0 + (r % T)
-__global__ void rope_kernel(bf16* __restrict__ qkv, long long ld, int rows, int T, int H, int D, int pos0,
-                            const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t, const int* __restrict__ positions,
+template <typename E_T>
+__global__ void rope_kernel(E_T* __restrict__ qkv, long long ld, int rows, int T, int H, int D, int pos0,
+                            const E_T* __restrict__ cos_t, const E_T* __restrict__ sin_t, const int* __restrict__ positions,
                             long long group_stride, long long group_offset) {
+  using E = ElemT<E_T>;
   pdl_prologue();
   const int row = blockIdx.x;
   if (row >= rows) return;
   const int pos = positions ? positions[row] : pos0 + (row % T);
   const int half = D >> 1;
   const int hv = half >> 3;                 // 16-byte vectors per half head
-  bf16* base = qkv + ((long long)(row / T) * group_stride + group_offset + (row % T)) * ld;
-  const bf16* cr = cos_t + (long long)pos * half;
-  const bf16* sr = sin_t + (long long)pos * half;
+  E_T* base = qkv + ((long long)(row / T) * group_stride + group_offset + (row % T)) * ld;
+  const E_T* cr = cos_t + (long long)pos * half;
+  const E_T* sr = sin_t + (long long)pos * half;
   // one thread = 8 consecutive (i, i+half) pairs of one head of q or k
   for (int idx = threadIdx.x; idx < 2 * H * hv; idx += blockDim.x) {
     const int hh = idx / hv;                // 0..2H-1 : q heads then k heads (contiguous: k starts at H*D)
     const int v = idx - hh * hv;
-    bf16* p = base + (long long)hh * D + v * 8;
+    E_T* p = base + (long long)hh * D + v * 8;
     const uint4 a = *reinterpret_cast<const uint4*>(p);
     const uint4 b = *reinterpret_cast<const uint4*>(p + half);
     const uint4 c = __ldg(reinterpret_cast<const uint4*>(cr + v * 8));
@@ -190,9 +199,9 @@ __global__ void rope_kernel(bf16* __restrict__ qkv, long long ld, int rows, int 
     uint32_t oa[4], ob[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const float2 x1 = unpack_bf16x2(aw[j]), x2 = unpack_bf16x2(bw[j]), cs = unpack_bf16x2(cw[j]), sn = unpack_bf16x2(sw[j]);
-      oa[j] = pack_bf16x2(rbf(x1.x * cs.x) + rbf(-x2.x * sn.x), rbf(x1.y * cs.y) + rbf(-x2.y * sn.y));
-      ob[j] = pack_bf16x2(rbf(x2.x * cs.x) + rbf(x1.x * sn.x), rbf(x2.y * cs.y) + rbf(x1.y * sn.y));
+      const float2 x1 = E::unpack2(aw[j]), x2 = E::unpack2(bw[j]), cs = E::unpack2(cw[j]), sn = E::unpack2(sw[j]);
+      oa[j] = E::pack2(E::round(x1.x * cs.x) + E::round(-x2.x * sn.x), E::round(x1.y * cs.y) + E::round(-x2.y * sn.y));
+      ob[j] = E::pack2(E::round(x2.x * cs.x) + E::round(x1.x * sn.x), E::round(x2.y * cs.y) + E::round(x1.y * sn.y));
     }
     *reinterpret_cast<uint4*>(p) = make_uint4(oa[0], oa[1], oa[2], oa[3]);
     *reinterpret_cast<uint4*>(p + half) = make_uint4(ob[0], ob[1], ob[2], ob[3]);
@@ -251,16 +260,18 @@ __global__ void patchify_kernel(const bf16* __restrict__ px, bf16* __restrict__ 
   }
 }
 
-// x[b,0,:] = cls + pos[0]; x[b,1+i,:] = bf16(x[b,1+i,:]) + pos[1+i]   (bf16 add like the reference)
-__global__ void vit_add_pos_kernel(bf16* __restrict__ x, const bf16* __restrict__ cls, const bf16* __restrict__ pos, int B,
+// x[b,0,:] = cls + pos[0]; x[b,1+i,:] = T(x[b,1+i,:]) + pos[1+i]   (T add like the reference)
+template <typename T>
+__global__ void vit_add_pos_kernel(T* __restrict__ x, const T* __restrict__ cls, const T* __restrict__ pos, int B,
                                    int S, int C) {
+  using E = ElemT<T>;
   const long long row = blockIdx.x;   // b*S + s
   const int s = row % S;
-  bf16* xr = x + row * C;
-  const bf16* pr = pos + (long long)s * C;
+  T* xr = x + row * C;
+  const T* pr = pos + (long long)s * C;
   for (int i = threadIdx.x; i < C; i += blockDim.x) {
-    const float a = (s == 0) ? bf2f(cls[i]) : bf2f(xr[i]);
-    xr[i] = f2bf(a + bf2f(pr[i]));
+    const float a = (s == 0) ? E::to_f(cls[i]) : E::to_f(xr[i]);
+    xr[i] = E::from_f(a + E::to_f(pr[i]));
   }
 }
 
@@ -309,9 +320,11 @@ __global__ void __launch_bounds__(128) owl_merge_kernel(const bf16* __restrict__
   for (int k = threadIdx.x; k < C; k += 128, ++cnt) yr[k] = f2bf((m[cnt] - mm) * rm * bf2f(w2[k]) + bf2f(b2[k]));
 }
 
-// y[r,:] = a[r,:] + b[r % bmod, :]   (bf16)
-__global__ void add_rows_kernel(const bf16* __restrict__ a, const bf16* __restrict__ b, bf16* __restrict__ y, long long rows,
+// y[r,:] = a[r,:] + b[r % bmod, :]   (T = bf16 / f16)
+template <typename T>
+__global__ void add_rows_kernel(const T* __restrict__ a, const T* __restrict__ b, T* __restrict__ y, long long rows,
                                 int cols, long long bmod) {
+  using E = ElemT<T>;
   const long long n8 = (long long)rows * (cols >> 3);
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
     const long long r = i / (cols >> 3);
@@ -320,17 +333,18 @@ __global__ void add_rows_kernel(const bf16* __restrict__ a, const bf16* __restri
     uint4 ub = __ldg(reinterpret_cast<const uint4*>(b) + (r % bmod) * (cols >> 3) + c8);
     float2 p, q;
     uint4 o;
-    p = unpack_bf16x2(ua.x); q = unpack_bf16x2(ub.x); o.x = pack_bf16x2(p.x + q.x, p.y + q.y);
-    p = unpack_bf16x2(ua.y); q = unpack_bf16x2(ub.y); o.y = pack_bf16x2(p.x + q.x, p.y + q.y);
-    p = unpack_bf16x2(ua.z); q = unpack_bf16x2(ub.z); o.z = pack_bf16x2(p.x + q.x, p.y + q.y);
-    p = unpack_bf16x2(ua.w); q = unpack_bf16x2(ub.w); o.w = pack_bf16x2(p.x + q.x, p.y + q.y);
+    p = E::unpack2(ua.x); q = E::unpack2(ub.x); o.x = E::pack2(p.x + q.x, p.y + q.y);
+    p = E::unpack2(ua.y); q = E::unpack2(ub.y); o.y = E::pack2(p.x + q.x, p.y + q.y);
+    p = E::unpack2(ua.z); q = E::unpack2(ub.z); o.z = E::pack2(p.x + q.x, p.y + q.y);
+    p = E::unpack2(ua.w); q = E::unpack2(ub.w); o.w = E::pack2(p.x + q.x, p.y + q.y);
     reinterpret_cast<uint4*>(y)[i] = o;
   }
 }
 
-// fp32 -> bf16 / bf16 -> fp32 casts (pixel upload path)
-__global__ void cast_f32_bf16_kernel(const float* __restrict__ x, bf16* __restrict__ y, long long n) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) y[i] = f2bf(x[i]);
+// fp32 -> T casts (pixel upload path)
+template <typename T>
+__global__ void cast_f32_kernel(const float* __restrict__ x, T* __restrict__ y, long long n) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) y[i] = ElemT<T>::from_f(x[i]);
 }
 
 // argmax over rows of fp32 logits [rows, n] -> idx (int32) and value
@@ -386,74 +400,80 @@ __global__ void __launch_bounds__(256) nll_rows_kernel(const float* __restrict__
 
 #define STREAM(s) reinterpret_cast<cudaStream_t>(s)
 
-extern "C" int vsb_layernorm_bf16(const void* x, long long ldx, const void* w, const void* b, void* y, long long ldy, int rows,
+template <typename T>
+static int layernorm(const void* x, long long ldx, const void* w, const void* b, void* y, long long ldy, int rows,
                                   int cols, float eps, int act, void* stream) {
   VSB_CHECK_ARG(x && w && b && y, "vsb_layernorm_bf16: null pointer");
   VSB_CHECK_ARG(cols % 8 == 0 && cols <= 128 * 8 * 4 && ldx % 8 == 0 && ldy % 8 == 0, "vsb_layernorm_bf16: cols=%d must be a multiple of 8 and <= 4096", cols);
   if (rows <= 0) return VSB_OK;
   const int blocks = (rows + 3) / 4;
   if (cols <= 1024)
-    layernorm_kernel<4><<<blocks, 128, 0, STREAM(stream)>>>((const bf16*)x, ldx, (const bf16*)w, (const bf16*)b, (bf16*)y, ldy, rows, cols, eps, act);
+    layernorm_kernel<4, T><<<blocks, 128, 0, STREAM(stream)>>>((const T*)x, ldx, (const T*)w, (const T*)b, (T*)y, ldy, rows, cols, eps, act);
   else
-    layernorm_kernel<16><<<blocks, 128, 0, STREAM(stream)>>>((const bf16*)x, ldx, (const bf16*)w, (const bf16*)b, (bf16*)y, ldy, rows, cols, eps, act);
+    layernorm_kernel<16, T><<<blocks, 128, 0, STREAM(stream)>>>((const T*)x, ldx, (const T*)w, (const T*)b, (T*)y, ldy, rows, cols, eps, act);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
 
-extern "C" int vsb_rmsnorm_bf16(const void* x, long long ldx, const void* w, void* y, long long ldy, int rows, int cols,
+template <typename T>
+static int rmsnorm(const void* x, long long ldx, const void* w, void* y, long long ldy, int rows, int cols,
                                 float eps, void* stream) {
   VSB_CHECK_ARG(x && w && y, "vsb_rmsnorm_bf16: null pointer");
   VSB_CHECK_ARG(cols % 8 == 0 && cols <= 128 * 8 * 4 && ldx % 8 == 0 && ldy % 8 == 0, "vsb_rmsnorm_bf16: cols=%d must be a multiple of 8 and <= 4096", cols);
   if (rows <= 0) return VSB_OK;
   const int blocks = (rows + 3) / 4;
   if (rows <= 32 && cols >= 2048 && cols <= 8192 && !vsb_batch_invariant()) {
-    VSB_CUDA(vsb_launch_pdl(rmsnorm_row_kernel, dim3(rows), dim3(256), 0, STREAM(stream), 1, (const bf16*)x, ldx, (const bf16*)w, (bf16*)y,
+    VSB_CUDA(vsb_launch_pdl(rmsnorm_row_kernel<T>, dim3(rows), dim3(256), 0, STREAM(stream), 1, (const T*)x, ldx, (const T*)w, (T*)y,
                             ldy, cols, eps));
     return VSB_OK;
   }
   if (cols <= 1024)
-    rmsnorm_kernel<4><<<blocks, 128, 0, STREAM(stream)>>>((const bf16*)x, ldx, (const bf16*)w, (bf16*)y, ldy, rows, cols, eps);
+    rmsnorm_kernel<4, T><<<blocks, 128, 0, STREAM(stream)>>>((const T*)x, ldx, (const T*)w, (T*)y, ldy, rows, cols, eps);
   else
-    rmsnorm_kernel<16><<<blocks, 128, 0, STREAM(stream)>>>((const bf16*)x, ldx, (const bf16*)w, (bf16*)y, ldy, rows, cols, eps);
+    rmsnorm_kernel<16, T><<<blocks, 128, 0, STREAM(stream)>>>((const T*)x, ldx, (const T*)w, (T*)y, ldy, rows, cols, eps);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
 
 // sum of squares of every row (fp32), the input side of a folded RMSNorm (vsb_gemm_rowscale_bf16 with sq_in_chunks = 1);
 // one warp per row, fixed summation order
-__global__ void __launch_bounds__(128) rowsq_kernel(const bf16* __restrict__ x, long long ldx, float* __restrict__ out, int rows, int cols) {
+template <typename T>
+__global__ void __launch_bounds__(128) rowsq_kernel(const T* __restrict__ x, long long ldx, float* __restrict__ out, int rows, int cols) {
+  using E = ElemT<T>;
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
-  const bf16* xr = x + (long long)row * ldx;
+  const T* xr = x + (long long)row * ldx;
   float s = 0.f;
   for (int c = lane * 8; c < cols; c += 256) {
     const uint4 v = *reinterpret_cast<const uint4*>(xr + c);
     float2 t;
-    t = unpack_bf16x2(v.x); s = fmaf(t.x, t.x, s); s = fmaf(t.y, t.y, s);
-    t = unpack_bf16x2(v.y); s = fmaf(t.x, t.x, s); s = fmaf(t.y, t.y, s);
-    t = unpack_bf16x2(v.z); s = fmaf(t.x, t.x, s); s = fmaf(t.y, t.y, s);
-    t = unpack_bf16x2(v.w); s = fmaf(t.x, t.x, s); s = fmaf(t.y, t.y, s);
+    t = E::unpack2(v.x); s = fmaf(t.x, t.x, s); s = fmaf(t.y, t.y, s);
+    t = E::unpack2(v.y); s = fmaf(t.x, t.x, s); s = fmaf(t.y, t.y, s);
+    t = E::unpack2(v.z); s = fmaf(t.x, t.x, s); s = fmaf(t.y, t.y, s);
+    t = E::unpack2(v.w); s = fmaf(t.x, t.x, s); s = fmaf(t.y, t.y, s);
   }
   s = warp_sum(s);
   if (lane == 0) out[row] = s;
 }
 
-extern "C" int vsb_rowsq_bf16(const void* x, long long ldx, void* out_f32, int rows, int cols, void* stream) {
+template <typename T>
+static int rowsq(const void* x, long long ldx, void* out_f32, int rows, int cols, void* stream) {
   VSB_CHECK_ARG(x && out_f32 && cols % 8 == 0 && ldx % 8 == 0, "vsb_rowsq_bf16: bad args (cols, ldx multiples of 8)");
   if (rows <= 0) return VSB_OK;
-  rowsq_kernel<<<(rows + 3) / 4, 128, 0, STREAM(stream)>>>((const bf16*)x, ldx, (float*)out_f32, rows, cols);
+  rowsq_kernel<T><<<(rows + 3) / 4, 128, 0, STREAM(stream)>>>((const T*)x, ldx, (float*)out_f32, rows, cols);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
 
-extern "C" int vsb_rope_bf16(void* qkv, long long ld, int rows, int T, int H, int D, int pos0, const void* cos_table,
+template <typename E_T>
+static int rope(void* qkv, long long ld, int rows, int T, int H, int D, int pos0, const void* cos_table,
                              const void* sin_table, const void* positions, long long group_stride, long long group_offset,
                              void* stream) {
   VSB_CHECK_ARG(qkv && cos_table && sin_table && rows >= 0 && T > 0 && H > 0 && D % 16 == 0 && ld % 8 == 0, "vsb_rope_bf16: bad args (D % 16, ld % 8)");
   if (rows == 0) return VSB_OK;
-  VSB_CUDA(vsb_launch_pdl(rope_kernel, dim3(rows), dim3(256), 0, STREAM(stream), 1, (bf16*)qkv, ld, rows, T, H, D, pos0,
-                          (const bf16*)cos_table, (const bf16*)sin_table, (const int*)positions, group_stride, group_offset));
+  VSB_CUDA(vsb_launch_pdl(rope_kernel<E_T>, dim3(rows), dim3(256), 0, STREAM(stream), 1, (E_T*)qkv, ld, rows, T, H, D, pos0,
+                          (const E_T*)cos_table, (const E_T*)sin_table, (const int*)positions, group_stride, group_offset));
   return VSB_OK;
 }
 
@@ -483,9 +503,10 @@ extern "C" int vsb_patchify_bf16(const void* pixels, void* A, int B, int S, int 
   return VSB_OK;
 }
 
-extern "C" int vsb_vit_add_pos_bf16(void* x, const void* cls, const void* pos, int B, int S, int C, void* stream) {
+template <typename T>
+static int vit_add_pos(void* x, const void* cls, const void* pos, int B, int S, int C, void* stream) {
   VSB_CHECK_ARG(x && cls && pos, "vsb_vit_add_pos_bf16: null pointer");
-  vit_add_pos_kernel<<<B * S, 128, 0, STREAM(stream)>>>((bf16*)x, (const bf16*)cls, (const bf16*)pos, B, S, C);
+  vit_add_pos_kernel<T><<<B * S, 128, 0, STREAM(stream)>>>((T*)x, (const T*)cls, (const T*)pos, B, S, C);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
@@ -499,23 +520,25 @@ extern "C" int vsb_owl_merge_bf16(const void* x, const void* w1, const void* b1,
   return VSB_OK;
 }
 
-extern "C" int vsb_add_rows_bf16(const void* a, const void* b, void* y, long long rows, int cols, long long bmod, void* stream) {
+template <typename T>
+static int add_rows(const void* a, const void* b, void* y, long long rows, int cols, long long bmod, void* stream) {
   VSB_CHECK_ARG(a && b && y && cols % 8 == 0 && bmod > 0, "vsb_add_rows_bf16: bad args");
   if (rows <= 0) return VSB_OK;
   long long n8 = rows * (cols >> 3);
   int blocks = (int)((n8 + 255) / 256);
   if (blocks > vsb_num_sms() * 16) blocks = vsb_num_sms() * 16;
-  add_rows_kernel<<<blocks, 256, 0, STREAM(stream)>>>((const bf16*)a, (const bf16*)b, (bf16*)y, rows, cols, bmod);
+  add_rows_kernel<T><<<blocks, 256, 0, STREAM(stream)>>>((const T*)a, (const T*)b, (T*)y, rows, cols, bmod);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
 
-extern "C" int vsb_cast_f32_bf16(const void* x, void* y, long long n, void* stream) {
+template <typename T>
+static int cast_f32(const void* x, void* y, long long n, void* stream) {
   VSB_CHECK_ARG(x && y, "vsb_cast_f32_bf16: null pointer");
   if (n <= 0) return VSB_OK;
   int blocks = (int)((n + 255) / 256);
   if (blocks > vsb_num_sms() * 16) blocks = vsb_num_sms() * 16;
-  cast_f32_bf16_kernel<<<blocks, 256, 0, STREAM(stream)>>>((const float*)x, (bf16*)y, n);
+  cast_f32_kernel<T><<<blocks, 256, 0, STREAM(stream)>>>((const float*)x, (T*)y, n);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
@@ -535,3 +558,47 @@ extern "C" int vsb_argmax_rows_f32(const void* x, long long ld, int rows, int n,
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
+
+// ------------------------------------------------------------------ C entry points: bf16 and f16 (the VQA engine in fp16)
+extern "C" int vsb_layernorm_bf16(const void* x, long long ldx, const void* w, const void* b, void* y, long long ldy, int rows, int cols,
+                                  float eps, int act, void* stream) {
+  return layernorm<bf16>(x, ldx, w, b, y, ldy, rows, cols, eps, act, stream);
+}
+extern "C" int vsb_layernorm_f16(const void* x, long long ldx, const void* w, const void* b, void* y, long long ldy, int rows, int cols,
+                                 float eps, int act, void* stream) {
+  return layernorm<half>(x, ldx, w, b, y, ldy, rows, cols, eps, act, stream);
+}
+extern "C" int vsb_rmsnorm_bf16(const void* x, long long ldx, const void* w, void* y, long long ldy, int rows, int cols, float eps, void* stream) {
+  return rmsnorm<bf16>(x, ldx, w, y, ldy, rows, cols, eps, stream);
+}
+extern "C" int vsb_rmsnorm_f16(const void* x, long long ldx, const void* w, void* y, long long ldy, int rows, int cols, float eps, void* stream) {
+  return rmsnorm<half>(x, ldx, w, y, ldy, rows, cols, eps, stream);
+}
+extern "C" int vsb_rowsq_bf16(const void* x, long long ldx, void* out_f32, int rows, int cols, void* stream) {
+  return rowsq<bf16>(x, ldx, out_f32, rows, cols, stream);
+}
+extern "C" int vsb_rowsq_f16(const void* x, long long ldx, void* out_f32, int rows, int cols, void* stream) {
+  return rowsq<half>(x, ldx, out_f32, rows, cols, stream);
+}
+extern "C" int vsb_rope_bf16(void* qkv, long long ld, int rows, int T, int H, int D, int pos0, const void* cos_table, const void* sin_table,
+                             const void* positions, long long group_stride, long long group_offset, void* stream) {
+  return rope<bf16>(qkv, ld, rows, T, H, D, pos0, cos_table, sin_table, positions, group_stride, group_offset, stream);
+}
+extern "C" int vsb_rope_f16(void* qkv, long long ld, int rows, int T, int H, int D, int pos0, const void* cos_table, const void* sin_table,
+                            const void* positions, long long group_stride, long long group_offset, void* stream) {
+  return rope<half>(qkv, ld, rows, T, H, D, pos0, cos_table, sin_table, positions, group_stride, group_offset, stream);
+}
+extern "C" int vsb_vit_add_pos_bf16(void* x, const void* cls, const void* pos, int B, int S, int C, void* stream) {
+  return vit_add_pos<bf16>(x, cls, pos, B, S, C, stream);
+}
+extern "C" int vsb_vit_add_pos_f16(void* x, const void* cls, const void* pos, int B, int S, int C, void* stream) {
+  return vit_add_pos<half>(x, cls, pos, B, S, C, stream);
+}
+extern "C" int vsb_add_rows_bf16(const void* a, const void* b, void* y, long long rows, int cols, long long bmod, void* stream) {
+  return add_rows<bf16>(a, b, y, rows, cols, bmod, stream);
+}
+extern "C" int vsb_add_rows_f16(const void* a, const void* b, void* y, long long rows, int cols, long long bmod, void* stream) {
+  return add_rows<half>(a, b, y, rows, cols, bmod, stream);
+}
+extern "C" int vsb_cast_f32_bf16(const void* x, void* y, long long n, void* stream) { return cast_f32<bf16>(x, y, n, stream); }
+extern "C" int vsb_cast_f32_f16(const void* x, void* y, long long n, void* stream) { return cast_f32<half>(x, y, n, stream); }

@@ -18,11 +18,12 @@
 
 namespace {
 
+template <typename T>
 struct SkinnyParams {
-  const bf16* A;
-  const bf16* W;
+  const T* A;
+  const T* W;
   void* C;
-  const bf16* bias;
+  const T* bias;
   const void* residual;
   long long lda, ldw, ldc, ldr;
   int M, N, K;
@@ -39,19 +40,30 @@ __device__ __forceinline__ uint4 ld_stream16(const void* p) {
   return v;
 }
 
+template <typename T>
 __device__ __forceinline__ void unpack8(const uint4& u, float* f) {
-  // bf16 -> fp32 is a 16-bit shift: low half = element 0
-  f[0] = __uint_as_float(u.x << 16); f[1] = __uint_as_float(u.x & 0xffff0000u);
-  f[2] = __uint_as_float(u.y << 16); f[3] = __uint_as_float(u.y & 0xffff0000u);
-  f[4] = __uint_as_float(u.z << 16); f[5] = __uint_as_float(u.z & 0xffff0000u);
-  f[6] = __uint_as_float(u.w << 16); f[7] = __uint_as_float(u.w & 0xffff0000u);
+  if constexpr (ElemT<T>::is_f16) {
+    // f16 -> fp32 needs a real conversion (cvt) per element
+    float2 t;
+    t = ElemT<T>::unpack2(u.x); f[0] = t.x; f[1] = t.y;
+    t = ElemT<T>::unpack2(u.y); f[2] = t.x; f[3] = t.y;
+    t = ElemT<T>::unpack2(u.z); f[4] = t.x; f[5] = t.y;
+    t = ElemT<T>::unpack2(u.w); f[6] = t.x; f[7] = t.y;
+  } else {
+    // bf16 -> fp32 is a 16-bit shift: low half = element 0
+    f[0] = __uint_as_float(u.x << 16); f[1] = __uint_as_float(u.x & 0xffff0000u);
+    f[2] = __uint_as_float(u.y << 16); f[3] = __uint_as_float(u.y & 0xffff0000u);
+    f[4] = __uint_as_float(u.z << 16); f[5] = __uint_as_float(u.z & 0xffff0000u);
+    f[6] = __uint_as_float(u.w << 16); f[7] = __uint_as_float(u.w & 0xffff0000u);
+  }
 }
 
 constexpr int SK_THREADS = 256;
 constexpr int SK_UNROLL = 8;      // 16 B loads in flight per lane and weight row
 
-template <int MT>
-__global__ void __launch_bounds__(SK_THREADS) gemm_skinny_kernel(const SkinnyParams p) {
+template <int MT, typename T>
+__global__ void __launch_bounds__(SK_THREADS) gemm_skinny_kernel(const SkinnyParams<T> p) {
+  using E = ElemT<T>;
   pdl_prologue();
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * SK_THREADS + threadIdx.x) >> 5;
@@ -83,14 +95,14 @@ __global__ void __launch_bounds__(SK_THREADS) gemm_skinny_kernel(const SkinnyPar
         const int c = c0 + u * 32;
         if (c < kchunks) {
           float fa[8], fb[8];
-          unpack8(wa[u], fa);
-          unpack8(wb[u], fb);
+          unpack8<T>(wa[u], fa);
+          unpack8<T>(wb[u], fb);
 #pragma unroll
           for (int m = 0; m < MT; ++m) {
             if (m < p.M) {
               const uint4 av = __ldg(reinterpret_cast<const uint4*>(p.A + (long long)m * p.lda) + c);
               float x[8];
-              unpack8(av, x);
+              unpack8<T>(av, x);
 #pragma unroll
               for (int i = 0; i < 8; ++i) {
                 acc[m][0] = fmaf(x[i], fa[i], acc[m][0]);
@@ -120,12 +132,12 @@ __global__ void __launch_bounds__(SK_THREADS) gemm_skinny_kernel(const SkinnyPar
     const int m = lane >> 1, c = lane & 1;
     const int n = n0 + c;
     const bool valid = (m < p.M) && (m < MT) && (n < p.N);
-    if (valid && p.bias != nullptr) mine += bf2f(p.bias[n]);
+    if (valid && p.bias != nullptr) mine += E::to_f(p.bias[n]);
     const float up = __shfl_down_sync(0xffffffffu, mine, 1);        // SwiGLU: odd column = up_j
     if (!valid) continue;
     const long long orow = (long long)(m / p.rows_per_group) * p.group_stride + p.group_offset + (m % p.rows_per_group);
     if (p.epilogue == VSB_EPI_SWIGLU) {
-      if (c == 0) reinterpret_cast<bf16*>(p.C)[orow * p.ldc + (n0 >> 1)] = f2bf(silu_f(mine) * up);
+      if (c == 0) reinterpret_cast<T*>(p.C)[orow * p.ldc + (n0 >> 1)] = E::from_f(silu_f(mine) * up);
       continue;
     }
     if (p.epilogue == VSB_EPI_QUICK_GELU) mine = quick_gelu_f(mine);
@@ -135,8 +147,8 @@ __global__ void __launch_bounds__(SK_THREADS) gemm_skinny_kernel(const SkinnyPar
       if (p.residual) mine += reinterpret_cast<const float*>(p.residual)[orow * p.ldr + n];
       reinterpret_cast<float*>(p.C)[orow * p.ldc + n] = mine;
     } else {
-      if (p.residual) mine += bf2f(reinterpret_cast<const bf16*>(p.residual)[orow * p.ldr + n]);
-      reinterpret_cast<bf16*>(p.C)[orow * p.ldc + n] = f2bf(mine);
+      if (p.residual) mine += E::to_f(reinterpret_cast<const T*>(p.residual)[orow * p.ldr + n]);
+      reinterpret_cast<T*>(p.C)[orow * p.ldc + n] = E::from_f(mine);
     }
   }
 }
@@ -153,18 +165,23 @@ __global__ void __launch_bounds__(SK_THREADS) gemm_skinny_kernel(const SkinnyPar
 //   * the k order inside an MMA is permuted consistently for A and B (lane t's 16 bytes feed k-slots {2t,2t+1,2t+8,2t+9} of
 //     two MMAs), which is legal because the contraction is order-free and makes every global load a 16-byte vector;
 //   * the warp's accumulators already hold complete dot products over its k-steps; the 8 warps are summed through shared memory.
-__device__ __forceinline__ void mma_bf16_16816(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+#define VSB_MMA_16816(TY)                                                                                                         \
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32." TY "." TY ".f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};" \
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])                                                                \
+               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1))
+template <typename T>
+__device__ __forceinline__ void mma_16816(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  if constexpr (ElemT<T>::is_f16) VSB_MMA_16816(VSB_PTX_F16);
+  else VSB_MMA_16816(VSB_PTX_BF16);
 }
 
 constexpr int SM_ROWS = 16;       // weight rows per block
 constexpr int SM_WARPS = 8;
 constexpr int SM_UNROLL = 4;
 
-template <int NT>                  // n-tiles of 8 activation rows: M <= 8 * NT
-__global__ void __launch_bounds__(SM_WARPS * 32) gemm_skinny_mma_kernel(const SkinnyParams p) {
+template <int NT, typename T>      // n-tiles of 8 activation rows: M <= 8 * NT
+__global__ void __launch_bounds__(SM_WARPS * 32) gemm_skinny_mma_kernel(const SkinnyParams<T> p) {
+  using E = ElemT<T>;
   pdl_prologue();
   __shared__ float red[SM_WARPS][NT][SM_ROWS][8 + 1];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -176,9 +193,9 @@ __global__ void __launch_bounds__(SM_WARPS * 32) gemm_skinny_mma_kernel(const Sk
   for (int grp = blockIdx.x; grp < ngroups; grp += gridDim.x) {
     const int n0 = grp * SM_ROWS;
     const bool r0ok = (n0 + g) < p.N, r1ok = (n0 + g + 8) < p.N;
-    const bf16* w0 = p.W + (long long)(r0ok ? n0 + g : 0) * p.ldw + t * 8;
-    const bf16* w1 = p.W + (long long)(r1ok ? n0 + g + 8 : 0) * p.ldw + t * 8;
-    const bf16* arow[NT];
+    const T* w0 = p.W + (long long)(r0ok ? n0 + g : 0) * p.ldw + t * 8;
+    const T* w1 = p.W + (long long)(r1ok ? n0 + g + 8 : 0) * p.ldw + t * 8;
+    const T* arow[NT];
     bool aok[NT];
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
@@ -205,8 +222,8 @@ __global__ void __launch_bounds__(SM_WARPS * 32) gemm_skinny_mma_kernel(const Sk
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt) {
           const uint4 av = (ok && aok[nt]) ? __ldg(reinterpret_cast<const uint4*>(arow[nt] + k)) : zero;
-          mma_bf16_16816(c[nt], wa[u].x, wb[u].x, wa[u].y, wb[u].y, av.x, av.y);
-          mma_bf16_16816(c[nt], wa[u].z, wb[u].z, wa[u].w, wb[u].w, av.z, av.w);
+          mma_16816<T>(c[nt], wa[u].x, wb[u].x, wa[u].y, wb[u].y, av.x, av.y);
+          mma_16816<T>(c[nt], wa[u].z, wb[u].z, wa[u].w, wb[u].w, av.z, av.w);
         }
       }
     }
@@ -232,12 +249,12 @@ __global__ void __launch_bounds__(SM_WARPS * 32) gemm_skinny_mma_kernel(const Sk
       const int na = n0 + 2 * rp, nb = na + 1;
       if (m < p.M && na < p.N) {
         if (p.bias != nullptr) {
-          v0 += bf2f(p.bias[na]);
-          if (nb < p.N) v1 += bf2f(p.bias[nb]);
+          v0 += E::to_f(p.bias[na]);
+          if (nb < p.N) v1 += E::to_f(p.bias[nb]);
         }
         const long long orow = (long long)(m / p.rows_per_group) * p.group_stride + p.group_offset + (m % p.rows_per_group);
         if (p.epilogue == VSB_EPI_SWIGLU) {
-          reinterpret_cast<bf16*>(p.C)[orow * p.ldc + (na >> 1)] = f2bf(silu_f(v0) * v1);
+          reinterpret_cast<T*>(p.C)[orow * p.ldc + (na >> 1)] = E::from_f(silu_f(v0) * v1);
         } else {
           float vv[2] = {v0, v1};
 #pragma unroll
@@ -252,8 +269,8 @@ __global__ void __launch_bounds__(SM_WARPS * 32) gemm_skinny_mma_kernel(const Sk
               if (p.residual) x += reinterpret_cast<const float*>(p.residual)[orow * p.ldr + n];
               reinterpret_cast<float*>(p.C)[orow * p.ldc + n] = x;
             } else {
-              if (p.residual) x += bf2f(reinterpret_cast<const bf16*>(p.residual)[orow * p.ldr + n]);
-              reinterpret_cast<bf16*>(p.C)[orow * p.ldc + n] = f2bf(x);
+              if (p.residual) x += E::to_f(reinterpret_cast<const T*>(p.residual)[orow * p.ldr + n]);
+              reinterpret_cast<T*>(p.C)[orow * p.ldc + n] = E::from_f(x);
             }
           }
         }
@@ -265,16 +282,17 @@ __global__ void __launch_bounds__(SM_WARPS * 32) gemm_skinny_mma_kernel(const Sk
 
 }  // namespace
 
-// called by vsb_gemm_bf16 (gemm_tcgen05.cu), K % 8 == 0, arguments already validated there.
+// called by vsb_gemm_bf16 / vsb_gemm_f16 (gemm_tcgen05.cu), K % 8 == 0, arguments already validated there.
 // variant 1: CUDA-core kernel (M <= 8); variant 2: mma.sync kernel (M <= 16)
+template <typename T>
 int vsb_gemm_skinny_launch(int variant, const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
                            int K, const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
                            long long group_stride, long long group_offset, cudaStream_t stream) {
-  SkinnyParams p;
-  p.A = reinterpret_cast<const bf16*>(A);
-  p.W = reinterpret_cast<const bf16*>(W);
+  SkinnyParams<T> p;
+  p.A = reinterpret_cast<const T*>(A);
+  p.W = reinterpret_cast<const T*>(W);
   p.C = C;
-  p.bias = reinterpret_cast<const bf16*>(bias);
+  p.bias = reinterpret_cast<const T*>(bias);
   p.residual = residual;
   p.lda = lda; p.ldw = ldw; p.ldc = ldc; p.ldr = ldr;
   p.M = M; p.N = N; p.K = K;
@@ -286,8 +304,8 @@ int vsb_gemm_skinny_launch(int variant, const void* A, long long lda, const void
   if (variant == 2) {
     const int ngroups = (N + SM_ROWS - 1) / SM_ROWS;
     const int blocks2 = ngroups < vsb_num_sms() * 8 ? ngroups : vsb_num_sms() * 8;
-    if (M <= 8) VSB_CUDA(vsb_launch_pdl(gemm_skinny_mma_kernel<1>, dim3(blocks2), dim3(SM_WARPS * 32), 0, stream, 1, p));
-    else VSB_CUDA(vsb_launch_pdl(gemm_skinny_mma_kernel<2>, dim3(blocks2), dim3(SM_WARPS * 32), 0, stream, 1, p));
+    if (M <= 8) VSB_CUDA(vsb_launch_pdl(gemm_skinny_mma_kernel<1, T>, dim3(blocks2), dim3(SM_WARPS * 32), 0, stream, 1, p));
+    else VSB_CUDA(vsb_launch_pdl(gemm_skinny_mma_kernel<2, T>, dim3(blocks2), dim3(SM_WARPS * 32), 0, stream, 1, p));
     return VSB_OK;
   }
   const int npairs = (N + 1) / 2;
@@ -295,9 +313,13 @@ int vsb_gemm_skinny_launch(int variant, const void* A, long long lda, const void
   int blocks = (npairs + warps_per_block - 1) / warps_per_block;
   const int cap = vsb_num_sms() * 8;                    // grid-stride beyond 8 resident blocks per SM
   if (blocks > cap) blocks = cap;
-  if (M <= 1) VSB_CUDA(vsb_launch_pdl(gemm_skinny_kernel<1>, dim3(blocks), dim3(SK_THREADS), 0, stream, 1, p));
-  else if (M <= 2) VSB_CUDA(vsb_launch_pdl(gemm_skinny_kernel<2>, dim3(blocks), dim3(SK_THREADS), 0, stream, 1, p));
-  else if (M <= 4) VSB_CUDA(vsb_launch_pdl(gemm_skinny_kernel<4>, dim3(blocks), dim3(SK_THREADS), 0, stream, 1, p));
-  else VSB_CUDA(vsb_launch_pdl(gemm_skinny_kernel<8>, dim3(blocks), dim3(SK_THREADS), 0, stream, 1, p));
+  if (M <= 1) VSB_CUDA(vsb_launch_pdl(gemm_skinny_kernel<1, T>, dim3(blocks), dim3(SK_THREADS), 0, stream, 1, p));
+  else if (M <= 2) VSB_CUDA(vsb_launch_pdl(gemm_skinny_kernel<2, T>, dim3(blocks), dim3(SK_THREADS), 0, stream, 1, p));
+  else if (M <= 4) VSB_CUDA(vsb_launch_pdl(gemm_skinny_kernel<4, T>, dim3(blocks), dim3(SK_THREADS), 0, stream, 1, p));
+  else VSB_CUDA(vsb_launch_pdl(gemm_skinny_kernel<8, T>, dim3(blocks), dim3(SK_THREADS), 0, stream, 1, p));
   return VSB_OK;
 }
+template int vsb_gemm_skinny_launch<bf16>(int, const void*, long long, const void*, long long, void*, long long, int, int, int, const void*,
+                                          const void*, long long, int, int, int, long long, long long, cudaStream_t);
+template int vsb_gemm_skinny_launch<half>(int, const void*, long long, const void*, long long, void*, long long, int, int, int, const void*,
+                                          const void*, long long, int, int, int, long long, long long, cudaStream_t);

@@ -1,7 +1,7 @@
-// vsb_gemm_bf16: C[M,N] = epilogue(A[M,K] . W[N,K]^T + bias) (+ residual)
+// vsb_gemm_bf16 / vsb_gemm_f16: C[M,N] = epilogue(A[M,K] . W[N,K]^T + bias) (+ residual)
 //
 // Hand-written sm_90a GEMM: TMA (cp.async.bulk.tensor, 128B swizzle) -> shared
-// memory ring (mbarrier full / empty pairs) -> wgmma.mma_async (bf16 x bf16 ->
+// memory ring (mbarrier full / empty pairs) -> wgmma.mma_async (bf16 or f16 ->
 // fp32 in registers) -> epilogue straight from the accumulator registers
 // (bias / activation / SwiGLU / residual / row remap / folded RMSNorm / RoPE) ->
 // global.  Persistent: one CTA per SM loops over 128 x BN output tiles; the
@@ -31,14 +31,15 @@ constexpr int BM = 128;
 constexpr int BK = 64;   // 64 bf16 = 128 B = one swizzle-128B row
 constexpr int WG_K = 16;
 
+template <typename T>      // operand type: bf16 or half
 struct GemmParams {
   void* C;
-  const bf16* bias;
+  const T* bias;
   const void* residual;
   long long ldc, ldr;
   int M, N, K;
   int epilogue;        // VSB_EPI_*
-  int out_fp32;        // C (and residual) element type: 0 bf16, 1 fp32
+  int out_fp32;        // C (and residual) element type: 0 T (bf16 / f16), 1 fp32
   int vec2;            // C (and residual) rows allow 2-element vector access at even columns
   int rows_per_group;  // output row remap: r = (m / rpg) * group_stride + group_offset + m % rpg
   long long group_stride, group_offset;
@@ -57,9 +58,9 @@ struct GemmParams {
   int sq_in_chunks;
   float sq_inv_cols, sq_eps;
   // rotate-half RoPE applied by the epilogue to the output columns [0, rope_cols) (the q | k thirds of a fused QKV projection,
-  // heads of 128 columns): same bf16 arithmetic as rope_kernel (elementwise.cu) on the same bf16 GEMM results => identical bits
-  const bf16* rope_cos;       // [max_pos][64] bf16
-  const bf16* rope_sin;
+  // heads of 128 columns): same T arithmetic as rope_kernel (elementwise.cu) on the same T GEMM results => identical bits
+  const T* rope_cos;          // [max_pos][64] T
+  const T* rope_sin;
   const int* rope_pos;        // optional position of every A row; else rope_pos0 + m % rope_T
   int rope_T, rope_pos0, rope_cols;
 };
@@ -155,12 +156,14 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   n_blk = r / gsize;
 }
 
-__device__ __forceinline__ long long remap_row(const GemmParams& p, int m) {
+template <typename T>
+__device__ __forceinline__ long long remap_row(const GemmParams<T>& p, int m) {
   return (long long)(m / p.rows_per_group) * p.group_stride + p.group_offset + (m % p.rows_per_group);
 }
 
 // 1 / rms of A row m from the partial sums a producer GEMM (or vsb_rowsq_bf16) left behind; fixed summation order
-__device__ __forceinline__ float row_rstd(const GemmParams& p, int m) {
+template <typename T>
+__device__ __forceinline__ float row_rstd(const GemmParams<T>& p, int m) {
   if (p.rowsq_in == nullptr || m >= p.M) return 1.f;
   float s = 0.f;
   for (int c = 0; c < p.sq_in_chunks; ++c) s += p.rowsq_in[(long long)c * p.sq_ld + m];
@@ -168,17 +171,19 @@ __device__ __forceinline__ float row_rstd(const GemmParams& p, int m) {
 }
 
 // ---------------------------------------------------------------- epilogue of one accumulator pair
-// row orow (already remapped), columns n, n+1 (n even, n < N): bias -> activation / SwiGLU -> (+residual) -> bf16 / fp32 store.
-// Returns the sum of squares of the bf16 values stored (the folded-RMSNorm row statistics).
-__device__ __forceinline__ float epilogue_pair(const GemmParams& p, long long orow, int n, float x0, float x1, bool swiglu) {
+// row orow (already remapped), columns n, n+1 (n even, n < N): bias -> activation / SwiGLU -> (+residual) -> T / fp32 store.
+// Returns the sum of squares of the T values stored (the folded-RMSNorm row statistics).
+template <typename T>
+__device__ __forceinline__ float epilogue_pair(const GemmParams<T>& p, long long orow, int n, float x0, float x1, bool swiglu) {
+  using E = ElemT<T>;
   const bool has1 = n + 1 < p.N;
   if (p.bias != nullptr) {
-    x0 += bf2f(p.bias[n]);
-    if (has1) x1 += bf2f(p.bias[n + 1]);
+    x0 += E::to_f(p.bias[n]);
+    if (has1) x1 += E::to_f(p.bias[n + 1]);
   }
   if (swiglu) {
     // interleaved weight rows: even column = gate_j, odd column = up_j -> out column n/2 (N is even)
-    reinterpret_cast<bf16*>(p.C)[orow * p.ldc + (n >> 1)] = f2bf(silu_f(x0) * x1);
+    reinterpret_cast<T*>(p.C)[orow * p.ldc + (n >> 1)] = E::from_f(silu_f(x0) * x1);
     return 0.f;
   }
   x0 = apply_act(x0, p.epilogue);
@@ -196,35 +201,37 @@ __device__ __forceinline__ float epilogue_pair(const GemmParams& p, long long or
     }
     return 0.f;
   }
-  bf16* c = reinterpret_cast<bf16*>(p.C) + orow * p.ldc + n;
-  const bf16* r = p.residual ? reinterpret_cast<const bf16*>(p.residual) + orow * p.ldr + n : nullptr;
+  T* c = reinterpret_cast<T*>(p.C) + orow * p.ldc + n;
+  const T* r = p.residual ? reinterpret_cast<const T*>(p.residual) + orow * p.ldr + n : nullptr;
   if (has1 && p.vec2) {
-    if (r) { const float2 rv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(r)); x0 += rv.x; x1 += rv.y; }
-    const uint32_t w = pack_bf16x2(x0, x1);
+    if (r) { const float2 rv = E::unpack2(*reinterpret_cast<const uint32_t*>(r)); x0 += rv.x; x1 += rv.y; }
+    const uint32_t w = E::pack2(x0, x1);
     if (p.stream_out) __stcs(reinterpret_cast<unsigned int*>(c), w); else *reinterpret_cast<uint32_t*>(c) = w;
   } else {
-    if (r) { x0 += bf2f(r[0]); if (has1) x1 += bf2f(r[1]); }
-    c[0] = f2bf(x0);
-    if (has1) c[1] = f2bf(x1);
+    if (r) { x0 += E::to_f(r[0]); if (has1) x1 += E::to_f(r[1]); }
+    c[0] = E::from_f(x0);
+    if (has1) c[1] = E::from_f(x1);
   }
-  const float s0 = rbf(x0), s1 = has1 ? rbf(x1) : 0.f;
+  const float s0 = E::round(x0), s1 = has1 ? E::round(x1) : 0.f;
   return fmaf(s1, s1, s0 * s0);
 }
 
 // RoPE on a 256-wide q/k tile (two heads of 128): accumulator column i of a head (i < 64) pairs with column i + 64, i.e.
-// fragment block j with j + 8.  x = bf16(acc * rs) is what the un-fused path stores and rope_kernel reads back; the rotated
-// values are exactly representable in bf16 (the store path's rounding is then the identity).
-__device__ __forceinline__ void rope_tile(const GemmParams& p, float* acc, const int* m, const float* rs, int t) {
+// fragment block j with j + 8.  x = T(acc * rs) is what the un-fused path stores and rope_kernel reads back; the rotated
+// values are exactly representable in T (the store path's rounding is then the identity).
+template <typename T>
+__device__ __forceinline__ void rope_tile(const GemmParams<T>& p, float* acc, const int* m, const float* rs, int t) {
+  using E = ElemT<T>;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int pos = (m[h] < p.M) ? (p.rope_pos ? p.rope_pos[m[h]] : p.rope_pos0 + (m[h] % p.rope_T)) : 0;
-    const bf16* cr = p.rope_cos + (long long)pos * 64;
-    const bf16* sr = p.rope_sin + (long long)pos * 64;
+    const T* cr = p.rope_cos + (long long)pos * 64;
+    const T* sr = p.rope_sin + (long long)pos * 64;
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
       const int i = 8 * jj + 2 * t;
-      const float2 cs = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(cr + i)));
-      const float2 sn = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(sr + i)));
+      const float2 cs = E::unpack2(__ldg(reinterpret_cast<const unsigned int*>(cr + i)));
+      const float2 sn = E::unpack2(__ldg(reinterpret_cast<const unsigned int*>(sr + i)));
 #pragma unroll
       for (int head = 0; head < 2; ++head) {
         const int ja = 16 * head + jj, jb = ja + 8;
@@ -233,9 +240,9 @@ __device__ __forceinline__ void rope_tile(const GemmParams& p, float* acc, const
           const float c = e ? cs.y : cs.x, s = e ? sn.y : sn.x;
           float& a = acc[4 * ja + 2 * h + e];
           float& b = acc[4 * jb + 2 * h + e];
-          const float x1 = rbf(a * rs[h]), x2 = rbf(b * rs[h]);
-          a = rbf(rbf(x1 * c) + rbf(-x2 * s));
-          b = rbf(rbf(x2 * c) + rbf(x1 * s));
+          const float x1 = E::round(a * rs[h]), x2 = E::round(b * rs[h]);
+          a = E::round(E::round(x1 * c) + E::round(-x2 * s));
+          b = E::round(E::round(x2 * c) + E::round(x1 * s));
         }
       }
     }
@@ -243,8 +250,8 @@ __device__ __forceinline__ void rope_tile(const GemmParams& p, float* acc, const
 }
 
 // Epilogue of one consumer thread: rows m[0], m[1] of the tile, fragment columns 8j + 2t (see wgmma.cuh)
-template <int BN, bool ROPE>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, int m0, int n_blk, int t) {
+template <int BN, bool ROPE, typename T>
+__device__ __forceinline__ void epilogue_tile(const GemmParams<T>& p, float* acc, int m0, int n_blk, int t) {
   const int m[2] = {m0, m0 + 8};
   float rs[2] = {row_rstd(p, m[0]), row_rstd(p, m[1])};
   const bool ok[2] = {m[0] < p.M, m[1] < p.M};
@@ -253,7 +260,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
   const int n_tile0 = n_blk * BN;
   if constexpr (ROPE) {
     if (n_tile0 < p.rope_cols) {
-      rope_tile(p, acc, m, rs, t);
+      rope_tile<T>(p, acc, m, rs, t);
       rs[0] = rs[1] = 1.f;
     }
   }
@@ -268,7 +275,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
       const int n = n0 + 8 * jj + 2 * t;
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        if (ok[h] && n < p.N) sq[h] += epilogue_pair(p, orow[h], n, acc[4 * j + 2 * h] * rs[h], acc[4 * j + 2 * h + 1] * rs[h], swiglu);
+        if (ok[h] && n < p.N) sq[h] += epilogue_pair<T>(p, orow[h], n, acc[4 * j + 2 * h] * rs[h], acc[4 * j + 2 * h + 1] * rs[h], swiglu);
     }
     if (p.rowsq_out != nullptr) {                  // N % 32 == 0: every chunk is complete
 #pragma unroll
@@ -289,9 +296,9 @@ __device__ __forceinline__ void fence_acc(float* acc) {
 
 constexpr int GEMM_THREADS = 384;   // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma consumers + epilogue
 
-template <int BN, bool ROPE = false>
+template <int BN, bool ROPE, typename T>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams<T> p) {
   using L = SmemLayout<BN>;
   constexpr int STAGES = L::STAGES;
 
@@ -361,7 +368,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
 #pragma unroll
       for (int k = 0; k < BK / WG_K; ++k)
         // advance 16 bf16 = 32 B along K inside the 128B swizzle row: +2 in the (addr>>4) field
-        wgmma_ss<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1 : 0);
+        wgmma_ss<BN, T>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1 : 0);
       wgmma_commit();
       wgmma_wait<1>();                            // the k-block before this one has been consumed: free its stage
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
@@ -371,7 +378,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     wgmma_wait<0>();
     fence_acc<BN / 2>(acc);
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
-    epilogue_tile<BN, ROPE>(p, acc, m_blk * BM + cw * 64 + wq * 16 + (lane >> 2), n_blk, lane & 3);
+    epilogue_tile<BN, ROPE, T>(p, acc, m_blk * BM + cw * 64 + wq * 16 + (lane >> 2), n_blk, lane & 3);
   }
 }
 
@@ -397,15 +404,16 @@ struct MapKey {
   const void* ptr;
   long long rows, cols, ld;
   int box_rows;
+  CUtensorMapDataType dtype;
   bool operator==(const MapKey& o) const {
-    return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows;
+    return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && dtype == o.dtype;
   }
 };
 struct MapKeyHash {
   size_t operator()(const MapKey& k) const {
     size_t h = std::hash<const void*>()(k.ptr);
     h ^= std::hash<long long>()(k.rows * 1315423911LL + k.cols) + 0x9e3779b97f4a7c15ULL + (h << 6) + (h >> 2);
-    h ^= std::hash<long long>()(k.ld * 31 + k.box_rows) + 0x9e3779b97f4a7c15ULL + (h << 6) + (h >> 2);
+    h ^= std::hash<long long>()((k.ld * 31 + k.box_rows) * 4 + (int)k.dtype) + 0x9e3779b97f4a7c15ULL + (h << 6) + (h >> 2);
     return h;
   }
 };
@@ -413,9 +421,9 @@ struct MapKeyHash {
 std::mutex g_map_mu;
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_map_cache;
 
-// 2D bf16 row-major [rows, cols] with leading dimension ld (elements); box = {64 cols, box_rows}
-int make_tensor_map(CUtensorMap* out, const void* ptr, long long rows, long long cols, long long ld, int box_rows) {
-  MapKey key{ptr, rows, cols, ld, box_rows};
+// 2D row-major [rows, cols] of a 2-byte type with leading dimension ld (elements); box = {64 cols, box_rows}
+int make_tensor_map(CUtensorMap* out, const void* ptr, long long rows, long long cols, long long ld, int box_rows, CUtensorMapDataType dtype) {
+  MapKey key{ptr, rows, cols, ld, box_rows, dtype};
   {
     std::lock_guard<std::mutex> g(g_map_mu);
     auto it = g_map_cache.find(key);
@@ -433,7 +441,7 @@ int make_tensor_map(CUtensorMap* out, const void* ptr, long long rows, long long
   cuuint64_t gstride[1] = {(cuuint64_t)ld * 2};
   cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+  CUresult r = enc(out, dtype, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -449,19 +457,19 @@ int make_tensor_map(CUtensorMap* out, const void* ptr, long long rows, long long
   return VSB_OK;
 }
 
-template <int BN, bool ROPE = false>
-int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, int max_ctas, cudaStream_t stream) {
+template <int BN, bool ROPE, typename T>
+int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams<T>& p, int max_ctas, cudaStream_t stream) {
   using L = SmemLayout<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    VSB_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN, ROPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
+    VSB_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, ROPE, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
     attr_set = true;
   }
   p.tiles_m = (p.M + BM - 1) / BM;
   p.tiles_n = (p.N + BN - 1) / BN;
   int tiles = p.tiles_m * p.tiles_n;
   int grid = tiles < max_ctas ? tiles : max_ctas;
-  gemm_bf16_wgmma_kernel<BN, ROPE><<<grid, GEMM_THREADS, L::TOTAL, stream>>>(tmA, tmB, p);
+  gemm_wgmma_kernel<BN, ROPE, T><<<grid, GEMM_THREADS, L::TOTAL, stream>>>(tmA, tmB, p);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }
@@ -491,6 +499,7 @@ extern "C" int vsb_gemm_set_group_m(int group_m) {
   return VSB_OK;
 }
 
+template <typename T>
 int vsb_gemm_skinny_launch(int variant, const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
                            int K, const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
                            long long group_stride, long long group_offset, cudaStream_t stream);
@@ -535,16 +544,18 @@ struct RowSq {          // folded-RMSNorm side channels of a GEMM (see vsb_gemm_
   long long ld = 0;
   int in_chunks = 0;
   float inv_cols = 0.f, eps = 0.f;
-  const bf16* rope_cos = nullptr;
-  const bf16* rope_sin = nullptr;
+  const void* rope_cos = nullptr;
+  const void* rope_sin = nullptr;
   const int* rope_pos = nullptr;
   int rope_T = 1, rope_pos0 = 0, rope_cols = 0;
 };
 
+template <typename T>
 static int gemm_dispatch(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N, int K,
                          const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
                          long long group_stride, long long group_offset, const RowSq* rsq, void* stream_);
 
+template <typename T>
 static int gemm_profiled(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N, int K,
                          const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
                          long long group_stride, long long group_offset, const RowSq* rsq, void* stream_);
@@ -553,8 +564,15 @@ extern "C" int vsb_gemm_bf16(const void* A, long long lda, const void* W, long l
                              int N, int K, const void* bias, const void* residual, long long ldr, int epilogue,
                              int out_fp32, int rows_per_group, long long group_stride, long long group_offset,
                              void* stream_) {
-  return gemm_profiled(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group, group_stride, group_offset,
+  return gemm_profiled<bf16>(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group, group_stride, group_offset,
                        nullptr, stream_);
+}
+extern "C" int vsb_gemm_f16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M,
+                            int N, int K, const void* bias, const void* residual, long long ldr, int epilogue,
+                            int out_fp32, int rows_per_group, long long group_stride, long long group_offset,
+                            void* stream_) {
+  return gemm_profiled<half>(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group, group_stride,
+                             group_offset, nullptr, stream_);
 }
 
 // GEMM with LlamaRMSNorm folded in (the norm weight must already be multiplied into W's columns):
@@ -563,8 +581,9 @@ extern "C" int vsb_gemm_bf16(const void* A, long long lda, const void* W, long l
 //                      normalised copy of the activations
 //   rowsq_out != NULL: additionally writes, for every output row and 32-column chunk, the sum of squares of the bf16 values it
 //                      stored: rowsq_out[(n/32)*sq_ld + row]; the next folded GEMM consumes them with sq_in_chunks = N/32.
-// bf16 output, N % 32 == 0 when rowsq_out is given.  Always the wgmma tile kernels (any M).
-extern "C" int vsb_gemm_rowscale_bf16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
+// T output, N % 32 == 0 when rowsq_out is given.  Always the wgmma tile kernels (any M).
+template <typename T>
+static int gemm_rowscale(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
                                       int K, const void* bias, const void* residual, long long ldr, int epilogue, int rows_per_group,
                                       long long group_stride, long long group_offset, const void* rowsq_in, int sq_in_chunks, float eps,
                                       void* rowsq_out, long long sq_ld, void* stream_) {
@@ -580,18 +599,33 @@ extern "C" int vsb_gemm_rowscale_bf16(const void* A, long long lda, const void* 
   r.in_chunks = sq_in_chunks;
   r.inv_cols = 1.f / (float)K;
   r.eps = eps;
-  return gemm_profiled(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, 0, rows_per_group, group_stride, group_offset, &r,
-                       stream_);
+  return gemm_profiled<T>(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, 0, rows_per_group, group_stride, group_offset, &r,
+                          stream_);
+}
+extern "C" int vsb_gemm_rowscale_bf16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
+                                      int K, const void* bias, const void* residual, long long ldr, int epilogue, int rows_per_group,
+                                      long long group_stride, long long group_offset, const void* rowsq_in, int sq_in_chunks, float eps,
+                                      void* rowsq_out, long long sq_ld, void* stream_) {
+  return gemm_rowscale<bf16>(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, rows_per_group, group_stride, group_offset,
+                             rowsq_in, sq_in_chunks, eps, rowsq_out, sq_ld, stream_);
+}
+extern "C" int vsb_gemm_rowscale_f16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
+                                     int K, const void* bias, const void* residual, long long ldr, int epilogue, int rows_per_group,
+                                     long long group_stride, long long group_offset, const void* rowsq_in, int sq_in_chunks, float eps,
+                                     void* rowsq_out, long long sq_ld, void* stream_) {
+  return gemm_rowscale<half>(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, rows_per_group, group_stride, group_offset,
+                             rowsq_in, sq_in_chunks, eps, rowsq_out, sq_ld, stream_);
 }
 
 // Fused QKV projection of a Llama layer: C = [q | k | v] = (A . W^T) with optional folded RMSNorm (rowsq_in, as
 // vsb_gemm_rowscale_bf16) and rotate-half RoPE applied by the epilogue to the q and k thirds (columns [0, 2N/3), head_dim 128):
 // the q/k rows land in the KV cache already rotated, vsb_rope_bf16 does not run.  Bit-identical to GEMM followed by vsb_rope_bf16.
-extern "C" int vsb_gemm_qkv_rope_bf16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
+template <typename T>
+static int gemm_qkv_rope(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
                                       int K, int rows_per_group, long long group_stride, long long group_offset, const void* rowsq_in,
                                       int sq_in_chunks, float eps, long long sq_ld, const void* cos_table, const void* sin_table,
-                                      const void* positions, int T, int pos0, int head_dim, void* stream_) {
-  VSB_CHECK_ARG(cos_table && sin_table && head_dim == 128 && T > 0, "vsb_gemm_qkv_rope_bf16: head_dim must be 128 (got %d)", head_dim);
+                                      const void* positions, int rope_T, int pos0, int head_dim, void* stream_) {
+  VSB_CHECK_ARG(cos_table && sin_table && head_dim == 128 && rope_T > 0, "vsb_gemm_qkv_rope_bf16: head_dim must be 128 (got %d)", head_dim);
   VSB_CHECK_ARG(N % 768 == 0 && ldc % 8 == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0, "vsb_gemm_qkv_rope_bf16: N = 3*d with d %% 256 == 0");
   VSB_CHECK_ARG(!rowsq_in || (sq_in_chunks > 0 && sq_ld >= M), "vsb_gemm_qkv_rope_bf16: bad row statistics");
   RowSq r;
@@ -600,35 +634,51 @@ extern "C" int vsb_gemm_qkv_rope_bf16(const void* A, long long lda, const void* 
   r.in_chunks = sq_in_chunks;
   r.inv_cols = 1.f / (float)K;
   r.eps = eps;
-  r.rope_cos = reinterpret_cast<const bf16*>(cos_table);
-  r.rope_sin = reinterpret_cast<const bf16*>(sin_table);
+  r.rope_cos = cos_table;
+  r.rope_sin = sin_table;
   r.rope_pos = reinterpret_cast<const int*>(positions);
-  r.rope_T = T;
+  r.rope_T = rope_T;
   r.rope_pos0 = pos0;
   r.rope_cols = N / 3 * 2;
-  return gemm_profiled(A, lda, W, ldw, C, ldc, M, N, K, nullptr, nullptr, 0, VSB_EPI_NONE, 0, rows_per_group, group_stride, group_offset, &r,
-                       stream_);
+  return gemm_profiled<T>(A, lda, W, ldw, C, ldc, M, N, K, nullptr, nullptr, 0, VSB_EPI_NONE, 0, rows_per_group, group_stride, group_offset,
+                          &r, stream_);
+}
+extern "C" int vsb_gemm_qkv_rope_bf16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
+                                      int K, int rows_per_group, long long group_stride, long long group_offset, const void* rowsq_in,
+                                      int sq_in_chunks, float eps, long long sq_ld, const void* cos_table, const void* sin_table,
+                                      const void* positions, int T, int pos0, int head_dim, void* stream_) {
+  return gemm_qkv_rope<bf16>(A, lda, W, ldw, C, ldc, M, N, K, rows_per_group, group_stride, group_offset, rowsq_in, sq_in_chunks, eps, sq_ld,
+                             cos_table, sin_table, positions, T, pos0, head_dim, stream_);
+}
+extern "C" int vsb_gemm_qkv_rope_f16(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N,
+                                     int K, int rows_per_group, long long group_stride, long long group_offset, const void* rowsq_in,
+                                     int sq_in_chunks, float eps, long long sq_ld, const void* cos_table, const void* sin_table,
+                                     const void* positions, int T, int pos0, int head_dim, void* stream_) {
+  return gemm_qkv_rope<half>(A, lda, W, ldw, C, ldc, M, N, K, rows_per_group, group_stride, group_offset, rowsq_in, sq_in_chunks, eps, sq_ld,
+                             cos_table, sin_table, positions, T, pos0, head_dim, stream_);
 }
 
+template <typename T>
 static int gemm_profiled(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M, int N, int K,
                          const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
                          long long group_stride, long long group_offset, const RowSq* rsq, void* stream_) {
   if (!g_prof_on)
-    return gemm_dispatch(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group, group_stride,
-                         group_offset, rsq, stream_);
+    return gemm_dispatch<T>(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group, group_stride,
+                            group_offset, rsq, stream_);
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ProfRec r;
   VSB_CUDA(cudaEventCreate(&r.a));
   VSB_CUDA(cudaEventCreate(&r.b));
   r.flops = 2.0 * (double)M * (double)N * (double)K;
   VSB_CUDA(cudaEventRecord(r.a, stream));
-  const int rc = gemm_dispatch(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group, group_stride,
+  const int rc = gemm_dispatch<T>(A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group, group_stride,
                                group_offset, rsq, stream_);
   VSB_CUDA(cudaEventRecord(r.b, stream));
   g_prof.push_back(r);
   return rc;
 }
 
+template <typename T>
 static int gemm_dispatch(const void* A, long long lda, const void* W, long long ldw, void* C, long long ldc, int M,
                              int N, int K, const void* bias, const void* residual, long long ldr, int epilogue,
                              int out_fp32, int rows_per_group, long long group_stride, long long group_offset,
@@ -641,15 +691,15 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
   VSB_CHECK_ARG((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0,
                 "vsb_gemm_bf16: A/W must be 16-byte aligned");
   VSB_CHECK_ARG(epilogue >= VSB_EPI_NONE && epilogue <= VSB_EPI_SWIGLU, "vsb_gemm_bf16: bad epilogue %d", epilogue);
-  VSB_CHECK_ARG(!(epilogue == VSB_EPI_SWIGLU && (out_fp32 || residual || (N & 1))), "vsb_gemm_bf16: SwiGLU epilogue is bf16, no residual, even N");
+  VSB_CHECK_ARG(!(epilogue == VSB_EPI_SWIGLU && (out_fp32 || residual || (N & 1))), "vsb_gemm_bf16: SwiGLU epilogue is bf16 / f16, no residual, even N");
   if (rows_per_group <= 0) {
     rows_per_group = M;
     group_stride = 0;
     group_offset = 0;
   }
-  GemmParams p;
+  GemmParams<T> p;
   p.C = C;
-  p.bias = reinterpret_cast<const bf16*>(bias);
+  p.bias = reinterpret_cast<const T*>(bias);
   p.residual = residual;
   p.ldc = ldc;
   p.ldr = ldr;
@@ -665,8 +715,8 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
   p.sq_in_chunks = rsq ? rsq->in_chunks : 0;
   p.sq_inv_cols = rsq ? rsq->inv_cols : 0.f;
   p.sq_eps = rsq ? rsq->eps : 0.f;
-  p.rope_cos = rsq ? rsq->rope_cos : nullptr;
-  p.rope_sin = rsq ? rsq->rope_sin : nullptr;
+  p.rope_cos = rsq ? reinterpret_cast<const T*>(rsq->rope_cos) : nullptr;
+  p.rope_sin = rsq ? reinterpret_cast<const T*>(rsq->rope_sin) : nullptr;
   p.rope_pos = rsq ? rsq->rope_pos : nullptr;
   p.rope_T = rsq ? rsq->rope_T : 1;
   p.rope_pos0 = rsq ? rsq->rope_pos0 : 0;
@@ -681,7 +731,7 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
     else if (g_force_bn == 0 && M == 1) variant = 1;
     else if (g_force_bn == 0 && (M <= 8 || (M <= 16 && N <= 8192))) variant = 2;
     if (variant)
-      return vsb_gemm_skinny_launch(variant, A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group,
+      return vsb_gemm_skinny_launch<T>(variant, A, lda, W, ldw, C, ldc, M, N, K, bias, residual, ldr, epilogue, out_fp32, rows_per_group,
                                     group_stride, group_offset, stream);
   }
   VSB_CHECK_ARG(g_force_bn != 1 && g_force_bn != 2, "vsb_gemm_bf16: skinny kernel forced but M=%d too large or K %% 8 != 0", M);
@@ -708,7 +758,7 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
   if (g_force_bn == 0 && bn == 64 && (long long)((M + BM - 1) / BM) * ((N + 63) / 64) <= sms / 2 && N >= 64) bn = 32;
   p.group_m = g_group_m > 0 ? g_group_m : 16;      // 2048-row bands (single-CTA tiles)
   CUtensorMap tmA, tmB;
-  int r = make_tensor_map(&tmA, A, M, K, lda, BM);
+  int r = make_tensor_map(&tmA, A, M, K, lda, BM, ElemT<T>::tma);
   if (r) return r;
   p.hint_a = p.hint_b = 0;
   p.stream_out = 0;
@@ -725,10 +775,11 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
   p.vec2 = (ldc % 2 == 0) && (reinterpret_cast<uintptr_t>(C) % (2 * esz) == 0) &&
            (residual == nullptr || ((ldr % 2 == 0) && (reinterpret_cast<uintptr_t>(residual) % (2 * esz) == 0)));
   if (p.rope_cos != nullptr) bn = 256;        // the fused-RoPE epilogue pairs columns inside one 128-wide head: 256-wide tiles only
-  r = make_tensor_map(&tmB, W, N, K, ldw, bn);
+  r = make_tensor_map(&tmB, W, N, K, ldw, bn, ElemT<T>::tma);
   if (r) return r;
-  if (bn == 256) return p.rope_cos ? launch_gemm<256, true>(tmA, tmB, p, sms, stream) : launch_gemm<256>(tmA, tmB, p, sms, stream);
-  if (bn == 128) return launch_gemm<128>(tmA, tmB, p, sms, stream);
-  if (bn == 32) return launch_gemm<32>(tmA, tmB, p, sms, stream);
-  return launch_gemm<64>(tmA, tmB, p, sms, stream);
+  if (bn == 256)
+    return p.rope_cos ? launch_gemm<256, true, T>(tmA, tmB, p, sms, stream) : launch_gemm<256, false, T>(tmA, tmB, p, sms, stream);
+  if (bn == 128) return launch_gemm<128, false, T>(tmA, tmB, p, sms, stream);
+  if (bn == 32) return launch_gemm<32, false, T>(tmA, tmB, p, sms, stream);
+  return launch_gemm<64, false, T>(tmA, tmB, p, sms, stream);
 }

@@ -12,6 +12,7 @@
 
 #include <math.h>
 
+template <typename T>
 int vsb_flash_attn_tc(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs, long long k_rs,
                       long long v_bs, long long v_rs, long long o_bs, long long o_rs, int B, int H, int Sq, int Sk, int D, int causal,
                       float scale, cudaStream_t stream);
@@ -29,10 +30,40 @@ extern "C" int vsb_llama_set_fuse_rope(int on) {
     if (_r != VSB_OK) return _r; \
   } while (0)
 
-extern "C" int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
-                                int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
-                                const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,
-                                void* scratch, void* stream) {
+// the entry points of one element type: the same layer sequence runs on bf16 (VSM, default VQA engine) or f16 weights
+template <typename T>
+struct LayerOps;
+template <>
+struct LayerOps<bf16> {
+  static constexpr auto gemm = vsb_gemm_bf16;
+  static constexpr auto gemm_rowscale = vsb_gemm_rowscale_bf16;
+  static constexpr auto gemm_qkv_rope = vsb_gemm_qkv_rope_bf16;
+  static constexpr auto rowsq = vsb_rowsq_bf16;
+  static constexpr auto rmsnorm = vsb_rmsnorm_bf16;
+  static constexpr auto rope = vsb_rope_bf16;
+  static constexpr auto flash_attn = vsb_flash_attn_bf16;
+  static constexpr auto flash_attn_seg = vsb_flash_attn_seg_bf16;
+  static constexpr auto attn_decode = vsb_attn_decode_bf16;
+};
+template <>
+struct LayerOps<half> {
+  static constexpr auto gemm = vsb_gemm_f16;
+  static constexpr auto gemm_rowscale = vsb_gemm_rowscale_f16;
+  static constexpr auto gemm_qkv_rope = vsb_gemm_qkv_rope_f16;
+  static constexpr auto rowsq = vsb_rowsq_f16;
+  static constexpr auto rmsnorm = vsb_rmsnorm_f16;
+  static constexpr auto rope = vsb_rope_f16;
+  static constexpr auto flash_attn = vsb_flash_attn_f16;
+  static constexpr auto flash_attn_seg = vsb_flash_attn_seg_f16;
+  static constexpr auto attn_decode = vsb_attn_decode_f16;
+};
+
+template <typename T>
+static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
+                        int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
+                        const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,
+                        void* scratch, void* stream) {
+  using K = LayerOps<T>;
   VSB_CHECK_ARG(layers && x && cache && rope_cos && rope_sin && scratch, "vsb_llama_layers: null pointer");
   VSB_CHECK_ARG(n_layers > 0 && B > 0 && Tn > 0 && past >= 0 && d > 0 && H > 0 && inter > 0, "vsb_llama_layers: bad shape");
   VSB_CHECK_ARG(B <= Bc && past + Tn <= Tmax, "vsb_llama_layers: B=%d Tn=%d past=%d exceed the cache [%d, %d]", B, Tn, past, Bc, Tmax);
@@ -42,10 +73,10 @@ extern "C" int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, v
   const long long rows = (long long)B * Tn;
   const long long ld = 3LL * d;
   const float scale = 1.0f / sqrtf((float)hd);
-  bf16* xb = reinterpret_cast<bf16*>(x);
-  bf16* h = reinterpret_cast<bf16*>(scratch);          // [rows, d]
-  bf16* attn = h + rows * d;                            // [rows, d]
-  bf16* gu = attn + rows * d;                           // [rows, inter]
+  T* xb = reinterpret_cast<T*>(x);
+  T* h = reinterpret_cast<T*>(scratch);                 // [rows, d]
+  T* attn = h + rows * d;                               // [rows, d]
+  T* gu = attn + rows * d;                              // [rows, inter]
   // tail mode: the caller consumes only the last `tail_rows` rows of every sequence (answer-predicting rows and the [LOC]
   // row of the guided search).  K/V of the last layer are needed by nobody else, so that layer runs its attention,
   // o-projection and MLP over B*tail rows only (same kernels, same per-row arithmetic => same values on those rows).
@@ -61,77 +92,92 @@ extern "C" int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, v
   float* sq_b = sq_a + (long long)sqc * rows;             // [sqc][rows]  input of the gate|up GEMM
   if (fused) {
     VSB_CHECK_ARG((long long)2 * sqc * rows * 4 <= rows * d * 2, "vsb_llama_layers: scratch too small for the row statistics");
-    VSB_TRY(vsb_rowsq_bf16(xb, d, sq_a, (int)rows, d, stream));
+    VSB_TRY(K::rowsq(xb, d, sq_a, (int)rows, d, stream));
   }
   // RoPE in the QKV epilogue (head_dim 128, wgmma tile path): q / k reach the cache already rotated
   const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && (rows > 16 || vsb_batch_invariant());
   int sq_a_chunks = 1;                                     // layer 0: one full-row sum from vsb_rowsq_bf16
   for (int li = 0; li < n_layers; ++li) {
     const vsb_llama_layer_t& L = layers[li];
-    bf16* cl = reinterpret_cast<bf16*>(cache) + (long long)li * Bc * Tmax * ld;       // [Bc*Tmax, 3d]
+    T* cl = reinterpret_cast<T*>(cache) + (long long)li * Bc * Tmax * ld;       // [Bc*Tmax, 3d]
     if (fused) {
       if (rope_fused)
-        VSB_TRY(vsb_gemm_qkv_rope_bf16(xb, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, sq_a, sq_a_chunks, rms_eps, rows, rope_cos,
+        VSB_TRY(K::gemm_qkv_rope(xb, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, sq_a, sq_a_chunks, rms_eps, rows, rope_cos,
                                        rope_sin, positions, Tn, past, hd, stream));
       else
-        VSB_TRY(vsb_gemm_rowscale_bf16(xb, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, nullptr, nullptr, 0, VSB_EPI_NONE, Tn, Tmax, past, sq_a,
+        VSB_TRY(K::gemm_rowscale(xb, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, nullptr, nullptr, 0, VSB_EPI_NONE, Tn, Tmax, past, sq_a,
                                        sq_a_chunks, rms_eps, nullptr, rows, stream));
     } else {
-      VSB_TRY(vsb_rmsnorm_bf16(xb, d, L.ln1, h, d, (int)rows, d, rms_eps, stream));
+      VSB_TRY(K::rmsnorm(xb, d, L.ln1, h, d, (int)rows, d, rms_eps, stream));
       if (rope_fused)
-        VSB_TRY(vsb_gemm_qkv_rope_bf16(h, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, nullptr, 0, rms_eps, rows, rope_cos, rope_sin,
+        VSB_TRY(K::gemm_qkv_rope(h, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, nullptr, 0, rms_eps, rows, rope_cos, rope_sin,
                                        positions, Tn, past, hd, stream));
       else
-        VSB_TRY(vsb_gemm_bf16(h, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, nullptr, nullptr, 0, VSB_EPI_NONE, 0, Tn, Tmax, past, stream));
+        VSB_TRY(K::gemm(h, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, nullptr, nullptr, 0, VSB_EPI_NONE, 0, Tn, Tmax, past, stream));
     }
-    if (!rope_fused) VSB_TRY(vsb_rope_bf16(cl, ld, (int)rows, Tn, H, hd, past, rope_cos, rope_sin, positions, Tmax, past, stream));
+    if (!rope_fused) VSB_TRY(K::rope(cl, ld, (int)rows, Tn, H, hd, past, rope_cos, rope_sin, positions, Tmax, past, stream));
     if (tail && li == n_layers - 1) {
       const long long trows = (long long)B * tail_rows;
-      bf16* xt = attn + trows * d;                                                     // compact copy of the tail rows of x
+      T* xt = attn + trows * d;                                                     // compact copy of the tail rows of x
       const int q0 = past + Tn - tail_rows;
-      VSB_TRY(vsb_flash_attn_tc(cl + (long long)q0 * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
+      VSB_TRY(vsb_flash_attn_tc<T>(cl + (long long)q0 * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
                                 (long long)Tmax * ld, ld, (long long)tail_rows * d, d, B, H, tail_rows, past + Tn, hd, 1, scale,
                                 reinterpret_cast<cudaStream_t>(stream)));
       VSB_TRY(vsb_copy2d_b16(xb + (long long)(Tn - tail_rows) * d, (long long)Tn * d, xt, (long long)tail_rows * d, B, tail_rows * d, stream));
       if (fused) {
         // compact tail rows: same fused kernels on trows rows (sq_b is indexed by compact row, leading dimension trows)
-        VSB_TRY(vsb_gemm_rowscale_bf16(attn, d, L.wo, d, xt, d, (int)trows, d, d, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0, rms_eps,
+        VSB_TRY(K::gemm_rowscale(attn, d, L.wo, d, xt, d, (int)trows, d, d, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0, rms_eps,
                                        sq_b, trows, stream));
-        VSB_TRY(vsb_gemm_rowscale_bf16(xt, d, L.wgu, d, gu, inter, (int)trows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, sq_b,
+        VSB_TRY(K::gemm_rowscale(xt, d, L.wgu, d, gu, inter, (int)trows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, sq_b,
                                        sqc, rms_eps, nullptr, trows, stream));
       } else {
-        VSB_TRY(vsb_gemm_bf16(attn, d, L.wo, d, xt, d, (int)trows, d, d, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
-        VSB_TRY(vsb_rmsnorm_bf16(xt, d, L.ln2, h, d, (int)trows, d, rms_eps, stream));
-        VSB_TRY(vsb_gemm_bf16(h, d, L.wgu, d, gu, inter, (int)trows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, 0, stream));
+        VSB_TRY(K::gemm(attn, d, L.wo, d, xt, d, (int)trows, d, d, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
+        VSB_TRY(K::rmsnorm(xt, d, L.ln2, h, d, (int)trows, d, rms_eps, stream));
+        VSB_TRY(K::gemm(h, d, L.wgu, d, gu, inter, (int)trows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, 0, stream));
       }
-      VSB_TRY(vsb_gemm_bf16(gu, inter, L.wdown, inter, xt, d, (int)trows, d, inter, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
+      VSB_TRY(K::gemm(gu, inter, L.wdown, inter, xt, d, (int)trows, d, inter, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
       VSB_TRY(vsb_copy2d_b16(xt, (long long)tail_rows * d, xb + (long long)(Tn - tail_rows) * d, (long long)Tn * d, B, tail_rows * d, stream));
       break;
     }
     if (q_seg != nullptr)
-      VSB_TRY(vsb_flash_attn_seg_bf16(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
+      VSB_TRY(K::flash_attn_seg(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
                                       (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, scale, q_seg, seg_lo, stream));
     else if (k_start != nullptr)
-      VSB_TRY(vsb_attn_decode_bf16(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
+      VSB_TRY(K::attn_decode(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
                                    (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, 1, scale, k_start, stream));
     else
-      VSB_TRY(vsb_flash_attn_bf16(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
+      VSB_TRY(K::flash_attn(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
                                   (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, 1, scale, stream));
     if (fused) {
-      VSB_TRY(vsb_gemm_rowscale_bf16(attn, d, L.wo, d, xb, d, (int)rows, d, d, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0, rms_eps, sq_b,
+      VSB_TRY(K::gemm_rowscale(attn, d, L.wo, d, xb, d, (int)rows, d, d, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0, rms_eps, sq_b,
                                      rows, stream));
-      VSB_TRY(vsb_gemm_rowscale_bf16(xb, d, L.wgu, d, gu, inter, (int)rows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, sq_b, sqc,
+      VSB_TRY(K::gemm_rowscale(xb, d, L.wgu, d, gu, inter, (int)rows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, sq_b, sqc,
                                      rms_eps, nullptr, rows, stream));
       // the down projection leaves the row statistics the NEXT layer's QKV GEMM needs (nobody reads them after the last layer)
-      VSB_TRY(vsb_gemm_rowscale_bf16(gu, inter, L.wdown, inter, xb, d, (int)rows, d, inter, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0,
+      VSB_TRY(K::gemm_rowscale(gu, inter, L.wdown, inter, xb, d, (int)rows, d, inter, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0,
                                      rms_eps, sq_a, rows, stream));
       sq_a_chunks = sqc;
     } else {
-      VSB_TRY(vsb_gemm_bf16(attn, d, L.wo, d, xb, d, (int)rows, d, d, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
-      VSB_TRY(vsb_rmsnorm_bf16(xb, d, L.ln2, h, d, (int)rows, d, rms_eps, stream));
-      VSB_TRY(vsb_gemm_bf16(h, d, L.wgu, d, gu, inter, (int)rows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, 0, stream));
-      VSB_TRY(vsb_gemm_bf16(gu, inter, L.wdown, inter, xb, d, (int)rows, d, inter, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
+      VSB_TRY(K::gemm(attn, d, L.wo, d, xb, d, (int)rows, d, d, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
+      VSB_TRY(K::rmsnorm(xb, d, L.ln2, h, d, (int)rows, d, rms_eps, stream));
+      VSB_TRY(K::gemm(h, d, L.wgu, d, gu, inter, (int)rows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, 0, stream));
+      VSB_TRY(K::gemm(gu, inter, L.wdown, inter, xb, d, (int)rows, d, inter, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
     }
   }
   return VSB_OK;
+}
+
+extern "C" int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
+                                int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
+                                const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,
+                                void* scratch, void* stream) {
+  return llama_layers<bf16>(layers, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, positions, k_start,
+                            tail_rows, q_seg, seg_lo, norm_folded, scratch, stream);
+}
+extern "C" int vsb_llama_layers_f16(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
+                                    int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
+                                    const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,
+                                    void* scratch, void* stream) {
+  return llama_layers<half>(layers, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, positions, k_start,
+                            tail_rows, q_seg, seg_lo, norm_folded, scratch, stream);
 }

@@ -35,16 +35,21 @@ def _pad8(n):
 
 class CoreWeights:
     """Llama-7B + CLIP ViT-L/14 + mm_projector: shared by the VSM (visual search model) and the SEAL VQA LLM.
-    Device-resident bf16 weights re-laid-out for the kernels (fused QKV, interleaved gate/up).  Source = any callable
-    name -> CPU/GPU tensor in the reference's state_dict key layout (SURVEY.md §8f-3)."""
+    Device-resident weights re-laid-out for the kernels (fused QKV, interleaved gate/up).  Source = any callable
+    name -> CPU/GPU tensor in the reference's state_dict key layout (SURVEY.md §8f-3).
+    dtype: torch.bfloat16 (default; the VSM) or torch.float16 (the SEAL VQA LLM as the reference runs it); the engine built on
+    these weights computes in that dtype."""
 
-    def __init__(self, cfg: VSMConfig, get, device="cuda"):
+    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF):
+        if dtype not in (torch.bfloat16, torch.float16):
+            raise ValueError(f"weights dtype must be torch.bfloat16 or torch.float16, got {dtype}")
         self.cfg = cfg
         self.device = device
+        self.dtype = dtype
         dev = device
 
         def g(name):
-            return get(name).to(device=dev, dtype=BF).contiguous()
+            return get(name).to(device=dev, dtype=dtype).contiguous()
 
         self._g = g
         c = cfg
@@ -66,27 +71,27 @@ class CoreWeights:
                 # LlamaRMSNorm's weight folded into the consuming projections: w * (x * rstd) @ W^T == rstd * (x @ (W * w)^T).  The
                 # kernels then apply 1/rms in the GEMM epilogue (vsb_gemm_rowscale_bf16) and no norm kernel runs; ln1 / ln2 become
                 # ones so that the unfused decode path (skinny GEMMs) computes the same function from the same folded weights.
-                wqkv = (wqkv.float() * ln1.float()[None, :]).to(BF)
-                wgu = (wgu.float() * ln2.float()[None, :]).to(BF)
+                wqkv = (wqkv.float() * ln1.float()[None, :]).to(dtype)
+                wgu = (wgu.float() * ln2.float()[None, :]).to(dtype)
                 if ones is None:
                     ones = torch.ones_like(ln1)
                 ln1 = ln2 = ones
             self.layers.append(dict(wqkv=wqkv.contiguous(), wo=g(p + "self_attn.o_proj.weight"), wgu=wgu.contiguous(),
                                     wdown=g(p + "mlp.down_proj.weight"), ln1=ln1, ln2=ln2))
-        # RoPE tables exactly as HF builds them (fp32 outer product -> cos/sin -> bf16)
+        # RoPE tables exactly as HF builds them (fp32 outer product -> cos/sin -> the model dtype)
         hd = c.head_dim
         inv = 1.0 / (c.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.float32) / hd))
         fr = torch.outer(torch.arange(2048, dtype=torch.float32), inv)
-        self.rope_cos = fr.cos().to(BF).to(dev).contiguous()
-        self.rope_sin = fr.sin().to(BF).to(dev).contiguous()
+        self.rope_cos = fr.cos().to(dtype).to(dev).contiguous()
+        self.rope_sin = fr.sin().to(dtype).to(dev).contiguous()
         # ---- ViTs
         self.clip = self._vit(g, "model.vision_tower.vision_tower.vision_model.", c.clip_layers + 1 + c.clip_select_layer
                               if c.clip_select_layer < 0 else c.clip_select_layer, c.clip_patch, "pre_layrnorm")
         self.mm_w, self.mm_b = g("model.mm_projector.weight"), g("model.mm_projector.bias")
 
     @classmethod
-    def from_state_dict(cls, cfg, sd, device="cuda"):
-        return cls(cfg, lambda n: sd[n], device)
+    def from_state_dict(cls, cfg, sd, device="cuda", dtype=BF):
+        return cls(cfg, lambda n: sd[n], device, dtype=dtype)
 
     @staticmethod
     def _vit(g, p, n_layers, patch, pre_name):
@@ -94,7 +99,7 @@ class CoreWeights:
         C = pw.shape[0]
         K = 3 * patch * patch
         Kp = _pad8(K)
-        w = torch.zeros((C, Kp), dtype=BF, device=pw.device)
+        w = torch.zeros((C, Kp), dtype=pw.dtype, device=pw.device)
         w[:, :K] = pw.reshape(C, K)
         layers = []
         for i in range(n_layers):
@@ -113,7 +118,9 @@ class VSMWeights(CoreWeights):
     """+ OWL-ViT-B/16, OWL heads, [LOC] query MLPs, SAM prompt encoder / mask decoder (stacked class-head rows,
     permuted conv taps)."""
 
-    def __init__(self, cfg: VSMConfig, get, device="cuda"):
+    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF):
+        if dtype != BF:
+            raise ValueError("the VSM runs in bf16 only, as in the reference (visual_search.py:145)")
         super().__init__(cfg, get, device)
         g, c, dev = self._g, cfg, device
         self.owl = self._vit(g, "model.owlvit.vision_model.", c.owl_layers, c.owl_patch, "pre_layernorm")
@@ -201,7 +208,8 @@ class CropResult:
 
 
 class LlamaClipCore:
-    """CLIP tower + Llama decoder on the sm_90a kernels with the fused-QKV cache; base of VSMEngine and VQAEngine."""
+    """CLIP tower + Llama decoder on the sm_90a kernels with the fused-QKV cache; base of VSMEngine and VQAEngine.
+    Computes in the weights' dtype (bf16, or fp16 for the VQA engine): cache, scratch and activations follow it."""
 
     MAX_POSITIONS = 2048          # rows of the RoPE tables (Llama-1 / Vicuna max_position_embeddings)
 
@@ -209,6 +217,7 @@ class LlamaClipCore:
         self.w = weights
         self.cfg = weights.cfg
         self.dev = weights.device
+        self.dtype = weights.dtype
         # rows per KV-cache slot allocated up front; the cache GROWS (up to MAX_POSITIONS) when a prompt or a generation
         # needs more - nothing is truncated silently, and a sequence beyond the RoPE tables raises VsbError
         self.max_tokens = min(int(max_tokens), self.MAX_POSITIONS)
@@ -256,7 +265,7 @@ class LlamaClipCore:
         S = g * g + 1
         C = vw["C"]
         A = ops.patchify(pixels, patch, vw["Kpad"])
-        x = torch.empty((B * S, C), dtype=BF, device=self.dev)
+        x = torch.empty((B * S, C), dtype=self.dtype, device=self.dev)
         ops.gemm(A, vw["patch_w"], out=x, rows_per_group=g * g, group_stride=S, group_offset=1)
         ops.vit_add_pos_(x, vw["cls"], vw["pos"], B, S)
         x = ops.layernorm(x, vw["pre"][0], vw["pre"][1], eps)
@@ -302,7 +311,7 @@ class LlamaClipCore:
         shape = (c.n_layers, B, Tmax, 3 * c.hidden)
         old = self._cache if keep else None
         self._cache = None                                # release before allocating the replacement (unless kept)
-        self._cache = torch.empty(shape, dtype=BF, device=self.dev)
+        self._cache = torch.empty(shape, dtype=self.dtype, device=self.dev)
         if old is not None:
             self._cache[:, :cur[1], :cur[2]].copy_(old)
         self._cache_shape = shape
@@ -320,7 +329,7 @@ class LlamaClipCore:
         if self._layer_table is None:
             self._layer_table = ops.llama_layer_table(self.w.layers)
         Bc, Tm = self._cache_shape[1], self._cache_shape[2]
-        scratch = torch.empty((B * Tn * (2 * c.hidden + c.intermediate),), dtype=BF, device=self.dev)
+        scratch = torch.empty((B * Tn * (2 * c.hidden + c.intermediate),), dtype=self.dtype, device=self.dev)
         return ops.llama_layers(self._layer_table, len(self.w.layers), x, B, Tn, past, self._cache, Bc, Tm, c.hidden, c.n_heads,
                                 c.intermediate, c.rms_eps, self.w.rope_cos, self.w.rope_sin, scratch, positions=positions,
                                 k_start=k_start, cache_row_offset=cache_row_offset, tail_rows=tail_rows, q_seg=q_seg, seg_lo=seg_lo,
@@ -377,7 +386,7 @@ class LlamaClipCore:
                     self._prefix_ids, self._prefix_kv, self._prefix_slots = None, None, 0
         Tn = T - P
         ct, S = self.clip_tokens(images_clip)                       # [B*257, Cc]
-        x = torch.empty((B * Tn, c.hidden), dtype=BF, device=self.dev)
+        x = torch.empty((B * Tn, c.hidden), dtype=self.dtype, device=self.dev)
         # mm_projector over all B*257 rows in ONE GEMM whose epilogue scatters each crop's rows straight into the LLM
         # input buffer: patch row i of crop b -> x[b*Tn + img_pos - P + i].  The CLS row lands on the <im_start> slot
         # (img_pos - 1 >= P) and is overwritten by the embedding splice below.

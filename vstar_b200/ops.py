@@ -1,8 +1,11 @@
 """Tensor-level wrappers over the C-ABI (torch is only the owner of device memory and streams here).
 
-Every function launches hand-written sm_100a kernels from libvstar_b200.so on the current torch CUDA
+Every function launches hand-written sm_90a kernels from libvstar_b200.so on the current torch CUDA
 stream.  No function has a PyTorch fallback: on a box without the built library, or on CPU tensors,
 they raise.
+
+The ops of the SEAL VQA LLM's path dispatch on the operand dtype: bf16 tensors run the _bf16 kernels, fp16 tensors their _f16
+twins.  Operands of one call must share that dtype (VsbError otherwise); the VSM-only ops are bf16-only.
 """
 import torch
 
@@ -11,6 +14,8 @@ from ._lib import call
 
 EPI_NONE, EPI_QUICK_GELU, EPI_GELU, EPI_RELU, EPI_SWIGLU = 0, 1, 2, 3, 4
 BF16 = torch.bfloat16
+F16 = torch.float16
+_SUFFIX = {BF16: "bf16", F16: "f16"}
 
 
 def _stream():
@@ -27,6 +32,22 @@ def _chk(t, dtype=None):
     if dtype is not None and t.dtype != dtype:
         raise _lib.VsbError(f"expected {dtype}, got {t.dtype}")
     return t
+
+
+def _sfx(*ts):
+    """kernel variant ("bf16" / "f16") for the dtype shared by all given tensors (None entries are skipped)"""
+    dt = None
+    for t in ts:
+        if t is None:
+            continue
+        _chk(t)
+        if dt is None:
+            dt = t.dtype
+        elif t.dtype != dt:
+            raise _lib.VsbError(f"mixed operand dtypes {dt} and {t.dtype} (one call runs on bf16 or on fp16 operands)")
+    if dt not in _SUFFIX:
+        raise _lib.VsbError(f"unsupported dtype {dt}: the kernels take bf16 or fp16")
+    return _SUFFIX[dt]
 
 
 def _rows2d(t):
@@ -73,13 +94,18 @@ def profile_end():
 
 
 def llama_layer_table(layers):
-    """layers: list of dicts with ln1, wqkv, wo, ln2, wgu, wdown tensors (kept alive by the caller) -> ctypes array"""
+    """layers: list of dicts with ln1, wqkv, wo, ln2, wgu, wdown tensors (kept alive by the caller), all bf16 or all fp16
+    -> ctypes array"""
     arr = (_lib.LlamaLayer * len(layers))()
+    dtypes = set()
     for i, L in enumerate(layers):
         for k in ("ln1", "wqkv", "wo", "ln2", "wgu", "wdown"):
             t = L[k]
-            assert t.dtype == BF16 and t.is_contiguous() and t.is_cuda, k
+            dtypes.add(t.dtype)
+            assert t.dtype in _SUFFIX and t.is_contiguous() and t.is_cuda, k
             setattr(arr[i], k, t.data_ptr())
+    if len(dtypes) > 1:
+        raise _lib.VsbError(f"mixed layer weight dtypes {sorted(map(str, dtypes))}")
     return arr
 
 
@@ -91,8 +117,9 @@ def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, 
     tail_rows > 0: only the last tail_rows rows of every sequence are valid on return (the last layer skips the others);
     q_seg int32 [B*Tn] + seg_lo: the new rows are several continuations of the cached prefix [0, seg_lo) appended back to back;
     row r attends the prefix and its own continuation from key q_seg[r] on;
-    norm_folded: ln1 / ln2 are already multiplied into wqkv / wgu (fused RMSNorm path, see vsb_llama_layers)."""
-    _chk(x, BF16), _chk(cache, BF16), _chk(scratch, BF16)
+    norm_folded: ln1 / ln2 are already multiplied into wqkv / wgu (fused RMSNorm path, see vsb_llama_layers).
+    x, cache, scratch, the RoPE tables and the table's weights are all bf16 or all fp16 (vsb_llama_layers_f16)."""
+    fn = "vsb_llama_layers" if _sfx(x, cache, scratch, rope_cos, rope_sin) == "bf16" else "vsb_llama_layers_f16"
     assert x.is_contiguous() and cache.is_contiguous() and x.shape == (B * Tn, d)
     assert scratch.numel() >= B * Tn * (2 * d + inter)
     for t in (positions, k_start, q_seg):
@@ -102,32 +129,35 @@ def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, 
     assert k_start is None or k_start.numel() == B
     _lib.launches += (6 if (norm_folded and k_start is None and (B * Tn > 16 or batch_invariant.depth > 0)) else 8) * n_layers + \
         (2 if (tail_rows > 0 and 2 * tail_rows <= Tn and k_start is None) else 0)
-    call("vsb_llama_layers", table, n_layers, x.data_ptr(), B, Tn, past, cache.data_ptr() + cache_row_offset * 3 * d * 2, Bc, Tmax, d, H,
+    call(fn, table, n_layers, x.data_ptr(), B, Tn, past, cache.data_ptr() + cache_row_offset * 3 * d * 2, Bc, Tmax, d, H,
          inter, float(eps), rope_cos.data_ptr(), rope_sin.data_ptr(), _p(positions), _p(k_start), int(tail_rows), _p(q_seg), int(seg_lo),
          1 if norm_folded else 0, scratch.data_ptr(), _stream())
     return x
 
 
-def gemm(a, w, out=None, bias=None, residual=None, epilogue=EPI_NONE, out_dtype=BF16, rows_per_group=0,
+def gemm(a, w, out=None, bias=None, residual=None, epilogue=EPI_NONE, out_dtype=None, rows_per_group=0,
          group_stride=0, group_offset=0, out_rows=None):
-    """out = epi(a @ w.T + bias) (+ residual).  a [M,K], w [N,K] bf16 (row stride arbitrary, inner stride 1)."""
-    _chk(a, BF16), _chk(w, BF16)
+    """out = epi(a @ w.T + bias) (+ residual).  a [M,K], w [N,K] bf16 or fp16 (row stride arbitrary, inner stride 1); out is
+    fp32 or the operands' dtype (default)."""
+    sfx = _sfx(a, w, bias)
     pa, M, K, lda = _rows2d(a)
     pw, N, K2, ldw = _rows2d(w)
     assert K == K2, (a.shape, w.shape)
     n_out = N // 2 if epilogue == EPI_SWIGLU else N
     if out is None:
-        out = torch.empty((out_rows if out_rows is not None else M, n_out), dtype=out_dtype, device=a.device)
+        out = torch.empty((out_rows if out_rows is not None else M, n_out), dtype=out_dtype or a.dtype, device=a.device)
     _chk(out)
     assert out.dim() == 2 and out.stride(1) == 1 and out.shape[1] >= n_out
     out_fp32 = 1 if out.dtype == torch.float32 else 0
+    if not out_fp32:
+        _sfx(a, out)
     if residual is not None:
-        assert residual.dtype == out.dtype and residual.stride(1) == 1
+        _chk(residual, out.dtype)
+        assert residual.stride(1) == 1
     if bias is not None:
-        _chk(bias, BF16)
         assert bias.numel() == N and bias.is_contiguous()
     _lib.launches += 1
-    call("vsb_gemm_bf16", pa, lda, pw, ldw, out.data_ptr(), out.stride(0), M, N, K, _p(bias), _p(residual),
+    call("vsb_gemm_" + sfx, pa, lda, pw, ldw, out.data_ptr(), out.stride(0), M, N, K, _p(bias), _p(residual),
          residual.stride(0) if residual is not None else 0, epilogue, out_fp32, rows_per_group, group_stride, group_offset,
          _stream())
     return out
@@ -136,53 +166,53 @@ def gemm(a, w, out=None, bias=None, residual=None, epilogue=EPI_NONE, out_dtype=
 def gemm_rowscale(a, w, out, rowsq_in=None, rowsq_out=None, eps=1e-6, residual=None, epilogue=EPI_NONE):
     """out = epi(rstd[m] * (a @ w.T)) (+ residual) with the RMSNorm weight already folded into w; rowsq_in fp32 [chunks, M] partial
     sums of squares of a's rows, rowsq_out fp32 [N/32, M] receives those of the stored output (see vsb_gemm_rowscale_bf16)"""
-    _chk(a, BF16), _chk(w, BF16), _chk(out, BF16)
+    sfx = _sfx(a, w, out, residual)
     pa, M, K, lda = _rows2d(a)
     pw, N, K2, ldw = _rows2d(w)
     assert K == K2 and out.stride(1) == 1
     for t in (rowsq_in, rowsq_out):
         assert t is None or (t.dtype == torch.float32 and t.is_cuda and t.is_contiguous() and t.shape[1] == M)
     _lib.launches += 1
-    call("vsb_gemm_rowscale_bf16", pa, lda, pw, ldw, out.data_ptr(), out.stride(0), M, N, K, 0, _p(residual),
+    call("vsb_gemm_rowscale_" + sfx, pa, lda, pw, ldw, out.data_ptr(), out.stride(0), M, N, K, 0, _p(residual),
          residual.stride(0) if residual is not None else 0, epilogue, 0, 0, 0, _p(rowsq_in), rowsq_in.shape[0] if rowsq_in is not None else 0,
          float(eps), _p(rowsq_out), M, _stream())
     return out
 
 
 def rowsq(x):
-    """fp32 [1, rows] sums of squares of the rows of x (bf16)"""
-    _chk(x, BF16)
+    """fp32 [1, rows] sums of squares of the rows of x (bf16 / fp16)"""
+    sfx = _sfx(x)
     px, rows, cols, ldx = _rows2d(x)
     out = torch.empty((1, rows), dtype=torch.float32, device=x.device)
     _lib.launches += 1
-    call("vsb_rowsq_bf16", px, ldx, out.data_ptr(), rows, cols, _stream())
+    call("vsb_rowsq_" + sfx, px, ldx, out.data_ptr(), rows, cols, _stream())
     return out
 
 
 def layernorm(x, w, b, eps, out=None, act=EPI_NONE):
-    _chk(x, BF16)
+    sfx = _sfx(x, w, b, out)
     px, rows, cols, ldx = _rows2d(x)
     if out is None:
-        out = torch.empty((rows, cols), dtype=BF16, device=x.device)
+        out = torch.empty((rows, cols), dtype=x.dtype, device=x.device)
     _lib.launches += 1
-    call("vsb_layernorm_bf16", px, ldx, w.data_ptr(), b.data_ptr(), out.data_ptr(), out.stride(0), rows, cols, float(eps), act, _stream())
+    call("vsb_layernorm_" + sfx, px, ldx, w.data_ptr(), b.data_ptr(), out.data_ptr(), out.stride(0), rows, cols, float(eps), act, _stream())
     return out
 
 
 def rmsnorm(x, w, eps, out=None):
-    _chk(x, BF16)
+    sfx = _sfx(x, w, out)
     px, rows, cols, ldx = _rows2d(x)
     if out is None:
-        out = torch.empty((rows, cols), dtype=BF16, device=x.device)
+        out = torch.empty((rows, cols), dtype=x.dtype, device=x.device)
     _lib.launches += 1
-    call("vsb_rmsnorm_bf16", px, ldx, w.data_ptr(), out.data_ptr(), out.stride(0), rows, cols, float(eps), _stream())
+    call("vsb_rmsnorm_" + sfx, px, ldx, w.data_ptr(), out.data_ptr(), out.stride(0), rows, cols, float(eps), _stream())
     return out
 
 
 def rope_(qkv, T, H, D, cos_t, sin_t, pos0=0, positions=None, rows=None, group_stride=None, group_offset=0):
     """In place on the q|k thirds of qkv [.., 3*H*D].  Default: `rows` = all rows, contiguous groups of T.
     KV-cache layout: logical row r -> physical row (r // T) * group_stride + group_offset + r % T."""
-    _chk(qkv, BF16)
+    sfx = _sfx(qkv, cos_t, sin_t)
     p, nrows, cols, ld = _rows2d(qkv)
     assert cols == 3 * H * D
     if rows is None:
@@ -190,7 +220,7 @@ def rope_(qkv, T, H, D, cos_t, sin_t, pos0=0, positions=None, rows=None, group_s
     if group_stride is None:
         group_stride = T
     _lib.launches += 1
-    call("vsb_rope_bf16", p, ld, rows, T, H, D, pos0, cos_t.data_ptr(), sin_t.data_ptr(), _p(positions), group_stride, group_offset,
+    call("vsb_rope_" + sfx, p, ld, rows, T, H, D, pos0, cos_t.data_ptr(), sin_t.data_ptr(), _p(positions), group_stride, group_offset,
          _stream())
     return qkv
 
@@ -204,32 +234,35 @@ def embed_splice(ids, table, out, img_pos, n_img):
 
 
 def gather_rows(idx, table, out=None):
+    """out[i] = table[idx[i]] (2-byte elements: bf16 or fp16)"""
     assert idx.dtype == torch.int64 and idx.is_contiguous()
     pt, nrows, d, ldt = _rows2d(table)
     n = idx.numel()
     if out is None:
-        out = torch.empty((n, d), dtype=BF16, device=table.device)
+        out = torch.empty((n, d), dtype=table.dtype, device=table.device)
+    assert table.element_size() == 2 and out.element_size() == 2
     _lib.launches += 1
     call("vsb_gather_rows_bf16", idx.data_ptr(), pt, ldt, out.data_ptr(), out.stride(0), n, d, nrows, _stream())
     return out
 
 
 def patchify(pixels, P, Kpad):
-    """pixels [B,3,S,S] bf16 -> [B*g*g, Kpad]"""
-    _chk(pixels, BF16)
+    """pixels [B,3,S,S] bf16 / fp16 -> [B*g*g, Kpad] of the same dtype (a 2-byte copy)"""
+    _sfx(pixels)
     B, C, S, S2 = pixels.shape
     assert C == 3 and S == S2 and pixels.is_contiguous()
     g = S // P
-    out = torch.empty((B * g * g, Kpad), dtype=BF16, device=pixels.device)
+    out = torch.empty((B * g * g, Kpad), dtype=pixels.dtype, device=pixels.device)
     _lib.launches += 1
     call("vsb_patchify_bf16", pixels.data_ptr(), out.data_ptr(), B, S, P, Kpad, _stream())
     return out
 
 
 def vit_add_pos_(x, cls, pos, B, S):
+    sfx = _sfx(x, cls, pos)
     assert x.is_contiguous()
     _lib.launches += 1
-    call("vsb_vit_add_pos_bf16", x.data_ptr(), cls.data_ptr(), pos.data_ptr(), B, S, x.shape[-1], _stream())
+    call("vsb_vit_add_pos_" + sfx, x.data_ptr(), cls.data_ptr(), pos.data_ptr(), B, S, x.shape[-1], _stream())
     return x
 
 
@@ -243,22 +276,33 @@ def owl_merge(x, w1, b1, w2, b2, B, S, eps):
 
 
 def add_rows(a, b, out=None):
-    """out[r] = a[r] + b[r % b.rows] (bf16)."""
+    """out[r] = a[r] + b[r % b.rows] (bf16 / fp16)."""
+    sfx = _sfx(a, b, out)
     assert a.is_contiguous() and b.is_contiguous() and a.shape[-1] == b.shape[-1]
     a2, b2 = a.view(-1, a.shape[-1]), b.view(-1, b.shape[-1])
     if out is None:
         out = torch.empty_like(a)
     _lib.launches += 1
-    call("vsb_add_rows_bf16", a2.data_ptr(), b2.data_ptr(), out.data_ptr(), a2.shape[0], a2.shape[1], b2.shape[0], _stream())
+    call("vsb_add_rows_" + sfx, a2.data_ptr(), b2.data_ptr(), out.data_ptr(), a2.shape[0], a2.shape[1], b2.shape[0], _stream())
     return out
 
 
 def cast_f32_bf16(x):
+    return cast_f32(x, BF16)
+
+
+def cast_f32(x, dtype, out=None):
+    """fp32 -> bf16 / fp16 copy of x (round to nearest even), into `out` (contiguous, same shape) if given"""
     _chk(x, torch.float32)
     assert x.is_contiguous()
-    out = torch.empty(x.shape, dtype=BF16, device=x.device)
+    if dtype not in _SUFFIX:
+        raise _lib.VsbError(f"unsupported dtype {dtype}: the kernels take bf16 or fp16")
+    if out is None:
+        out = torch.empty(x.shape, dtype=dtype, device=x.device)
+    _chk(out, dtype)
+    assert out.is_contiguous() and out.shape == x.shape
     _lib.launches += 1
-    call("vsb_cast_f32_bf16", x.data_ptr(), out.data_ptr(), x.numel(), _stream())
+    call("vsb_cast_f32_" + _SUFFIX[dtype], x.data_ptr(), out.data_ptr(), x.numel(), _stream())
     return out
 
 
@@ -295,8 +339,9 @@ def copy2d(src, dst):
 
 def flash_attn(q, k, v, out, B, H, Sq, Sk, D, causal, scale, q_bs, q_rs, k_bs, k_rs, v_bs, v_rs, o_bs, o_rs):
     """Strided attention: element (b,s,h,d) of q at q.data_ptr() + (b*q_bs + s*q_rs + h*D + d) elements, etc."""
+    sfx = _sfx(q, k, v, out)
     _lib.launches += 1
-    call("vsb_flash_attn_bf16", q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), q_bs, q_rs, k_bs, k_rs, v_bs, v_rs,
+    call("vsb_flash_attn_" + sfx, q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), q_bs, q_rs, k_bs, k_rs, v_bs, v_rs,
          o_bs, o_rs, B, H, Sq, Sk, D, 1 if causal else 0, float(scale), _stream())
     return out
 
@@ -305,7 +350,7 @@ def attn_fused_qkv(qkv, B, S, H, D, causal, scale, out=None):
     """qkv [B*S, 3*H*D] (q|k|v) -> out [B*S, H*D]"""
     ld = qkv.stride(0)
     if out is None:
-        out = torch.empty((B * S, H * D), dtype=BF16, device=qkv.device)
+        out = torch.empty((B * S, H * D), dtype=qkv.dtype, device=qkv.device)
     q = qkv
     k = qkv[:, H * D:]
     v = qkv[:, 2 * H * D:]
@@ -313,13 +358,14 @@ def attn_fused_qkv(qkv, B, S, H, D, causal, scale, out=None):
 
 
 def attn_small(q, k, v, B, H, Nq, Nk, D, scale, out=None):
+    sfx = _sfx(q, k, v, out)
     pq, rq, cq, ldq = _rows2d(q)
     pk, rk, ck, ldk = _rows2d(k)
     pv, rv, cv, ldv = _rows2d(v)
     if out is None:
-        out = torch.empty((B * Nq, H * D), dtype=BF16, device=q.device)
+        out = torch.empty((B * Nq, H * D), dtype=q.dtype, device=q.device)
     _lib.launches += 1
-    call("vsb_attn_small_bf16", pq, ldq, pk, ldk, pv, ldv, out.data_ptr(), out.stride(0), B, H, Nq, Nk, D, float(scale), _stream())
+    call("vsb_attn_small_" + sfx, pq, ldq, pk, ldk, pv, ldv, out.data_ptr(), out.stride(0), B, H, Nq, Nk, D, float(scale), _stream())
     return out
 
 

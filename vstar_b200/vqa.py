@@ -9,8 +9,11 @@
   VQA_LLM                : drop-in mirror of `vstar_bench_eval.VQA_LLM` (free_form_inference, multiple_choices_inference,
                            get_patch, get_object_crop).
 
-The reference runs this model in fp16 (LLaVA/llava/model/builder.py:43); the kernels here are bf16 with fp32
-accumulation — the tolerance is stated in tests/test_vqa_gpu.py.
+The reference runs this model in fp16 (LLaVA/llava/model/builder.py:43).  The engine runs in bf16 by default (fp32
+accumulation; tolerance stated in tests/test_vqa_gpu.py) or, opt-in, in fp16 like the reference on the _f16 variants of the
+same kernels: VQAWeights(..., dtype=torch.float16), load_pretrained_model(..., torch_dtype=torch.float16) or
+VQA_LLM(args) with args.vqa_dtype = "fp16".  fp16 brings the option NLLs and logits close to the reference's own
+numbers (tests/test_vqa_fp16_gpu.py; DESIGN.md §7b).  The VSM stays bf16, as in the reference.
 """
 from __future__ import annotations
 
@@ -23,6 +26,7 @@ from .engine import CoreWeights, LlamaClipCore
 from .vsm import CLIP_MEAN, SyntheticTokenizer, _normalize_into
 
 BF = torch.bfloat16
+VQA_DTYPES = {"bf16": torch.bfloat16, "fp16": torch.float16}
 IMAGE_TOKEN_INDEX = -200
 OBJECT_TOKEN_INDEX = -300
 DEFAULT_IMAGE_TOKEN = "<image>"
@@ -64,10 +68,11 @@ def tokenizer_image_object_token(prompt, tokenizer, image_token_index=IMAGE_TOKE
 
 
 class VQAWeights(CoreWeights):
-    """CoreWeights + the object projector `model.mm_projector_object.{0,1,2}` (multimodal_projector/builder.py:54-68)"""
+    """CoreWeights + the object projector `model.mm_projector_object.{0,1,2}` (multimodal_projector/builder.py:54-68).
+    dtype: torch.bfloat16 (default) or torch.float16 (the reference's dtype for this model)."""
 
-    def __init__(self, cfg: VSMConfig, get, device="cuda"):
-        super().__init__(cfg, get, device)
+    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF):
+        super().__init__(cfg, get, device, dtype=dtype)
         g = self._g
         p = "model.mm_projector_object."
         self.pj_ln = (g(p + "0.weight"), g(p + "0.bias"))
@@ -92,7 +97,7 @@ class VQAEngine(LlamaClipCore):
 
     # ------------------------------------------------------------------ projectors
     def project_both(self, pixels):
-        """encode_images / project_features (llava_search_arch.py:83-93): pixels [n,3,224,224] bf16 ->
+        """encode_images / project_features (llava_search_arch.py:83-93): pixels [n,3,224,224] in the engine dtype ->
         (long [n*256, d], short [n*32, d])"""
         c, w = self.cfg, self.w
         n = pixels.shape[0]
@@ -107,7 +112,7 @@ class VQAEngine(LlamaClipCore):
         x = ops.add_rows(x, w.media_pos)                                   # + media_pos_emb[:1]
         lat = w.latents.repeat(n, 1).contiguous()                          # [n*32, C]
         NK = P + self.NLAT
-        kv = torch.empty((n * NK, 2 * inner), dtype=BF, device=self.dev)
+        kv = torch.empty((n * NK, 2 * inner), dtype=self.dtype, device=self.dev)
         for L in w.pj_layers:
             xm = ops.layernorm(x, L["nm"][0], L["nm"][1], 1e-5)
             lt = ops.layernorm(lat, L["nl"][0], L["nl"][1], 1e-5)
@@ -147,7 +152,7 @@ class VQAEngine(LlamaClipCore):
         if cur:
             segs.append(("ids", cur))
         T = sum(len(v) if k == "ids" else v.shape[0] for k, v in segs)
-        x = torch.empty((T, c.hidden), dtype=BF, device=self.dev)
+        x = torch.empty((T, c.hidden), dtype=self.dtype, device=self.dev)
         t = 0
         for k, v in segs:
             n = len(v) if k == "ids" else v.shape[0]
@@ -423,7 +428,7 @@ class LlavaSearchModel:
     def _px(self, t):
         if t is None or len(t) == 0:
             return None
-        return ops.cast_f32_bf16(torch.as_tensor(t).float().to(self.engine.dev).contiguous())
+        return ops.cast_f32(torch.as_tensor(t).float().to(self.engine.dev).contiguous(), self.engine.dtype)
 
     @torch.inference_mode()
     def generate(self, input_ids, images=None, object_features=None, images_long=None, objects_long=None, do_sample=False, num_beams=1,
@@ -458,10 +463,11 @@ class LlavaSearchModel:
 
 
 def load_pretrained_model(model_path, model_base=None, model_name=None, load_8bit=False, load_4bit=False, device_map="auto",
-                          device="cuda"):
+                          device="cuda", torch_dtype=None):
     """Drop-in for /root/reference/LLaVA/llava/model/builder.py:26-151 (the SEAL VQA LLM branch):
     -> (tokenizer, model, image_processor, context_len).  model_path: local `seal_vqa_7b` checkpoint directory (HF
-    safetensors / .bin shards in the reference's key layout).  bitsandbytes paths are out of scope."""
+    safetensors / .bin shards in the reference's key layout).  bitsandbytes paths are out of scope.
+    torch_dtype: None / torch.bfloat16 (default) or torch.float16 (the reference's dtype, builder.py:43) for the engine."""
     import os
     if load_8bit or load_4bit:
         raise NotImplementedError("load_8bit / load_4bit (bitsandbytes) are outside the hot-path scope (SURVEY.md §2)")
@@ -471,16 +477,21 @@ def load_pretrained_model(model_path, model_base=None, model_name=None, load_8bi
     from .vsm import config_from_hf, open_checkpoint
     tokenizer = AutoTokenizer.from_pretrained(model_path, use_fast=False)
     cfg = config_from_hf(model_path)
-    engine = VQAEngine(VQAWeights(cfg, open_checkpoint(model_path, device=device), device=device))
+    dtype = BF if torch_dtype is None else torch_dtype
+    engine = VQAEngine(VQAWeights(cfg, open_checkpoint(model_path, device=device), device=device, dtype=dtype))
     return tokenizer, LlavaSearchModel(engine, getattr(tokenizer, "eos_token_id", 2)), _Proc(), 2048
 
 
 class VQA_LLM:
-    """Same surface as /root/reference/vstar_bench_eval.py:38-165."""
+    """Same surface as /root/reference/vstar_bench_eval.py:38-165.  args.vqa_dtype (optional): "bf16" (default) or "fp16"."""
 
     def __init__(self, args=None, engine: VQAEngine = None, tokenizer=None, conv_type="v1"):
         if engine is None:
-            self.tokenizer, self.model, self.image_processor, self.context_len = load_pretrained_model(args.vqa_model_path, None, None)
+            name = getattr(args, "vqa_dtype", None) or "bf16"
+            if name not in VQA_DTYPES:
+                raise ValueError(f"vqa_dtype must be one of {sorted(VQA_DTYPES)}, got {name!r}")
+            self.tokenizer, self.model, self.image_processor, self.context_len = load_pretrained_model(
+                args.vqa_model_path, None, None, torch_dtype=VQA_DTYPES[name])
             self.engine = self.model.engine
             self.conv_type = getattr(args, "conv_type", "v1")
             self.eos = getattr(self.tokenizer, "eos_token_id", 2)
@@ -519,10 +530,10 @@ class VQA_LLM:
         if torch.is_tensor(image) and image.is_cuda:            # already preprocessed on the device (device_pixels)
             return image, object_crops
         img = _clip_preprocess(image).unsqueeze(0).to(self.engine.dev)
-        img = ops.cast_f32_bf16(img.contiguous())
+        img = ops.cast_f32(img.contiguous(), self.engine.dtype)
         crops = None
         if object_crops is not None and len(object_crops) > 0:
-            crops = ops.cast_f32_bf16(torch.as_tensor(object_crops).float().to(self.engine.dev).contiguous())
+            crops = ops.cast_f32(torch.as_tensor(object_crops).float().to(self.engine.dev).contiguous(), self.engine.dtype)
         return img, crops
 
     def use_device_images(self, vsm):
@@ -532,15 +543,26 @@ class VQA_LLM:
         self._img_src = vsm
 
     def device_pixels(self, image, boxes, patch_scale=1.2):
-        """== (_clip_preprocess(expand2square_center(image)), [get_object_crop(image, b, patch_scale) for b in boxes]) as bf16
-        device tensors ([1,3,224,224], [k,3,224,224] or None), computed by the GPU image pipeline"""
+        """== (_clip_preprocess(expand2square_center(image)), [get_object_crop(image, b, patch_scale) for b in boxes]) as device
+        tensors of the engine dtype ([1,3,224,224], [k,3,224,224] or None), computed by the GPU image pipeline.  fp16: the
+        pipeline's fp32 normalised pixels cast to fp16, i.e. the reference's .half() of its fp32 pixel tensor"""
         vsm = self._img_src
         pipe = vsm.pipeline
         res = vsm.resident(image)                                   # uint8 [H, W, 3] in HBM
         H, W = int(res.shape[0]), int(res.shape[1])
         side = max(W, H)
         dev = self.engine.dev
-        img = torch.empty((1, 3, 224, 224), dtype=BF, device=dev)
+        f16 = self.engine.dtype == torch.float16
+
+        def resize(src_, l, t, w, h, iw, ih, out):
+            if f16:
+                f32 = torch.empty(out.shape, dtype=torch.float32, device=dev)
+                pipe._resize(src_, l, t, w, h, iw, ih, 224, 224, out_f32=f32)
+                ops.cast_f32(f32, torch.float16, out=out)
+            else:
+                pipe._resize(src_, l, t, w, h, iw, ih, 224, 224, out_bf16=out)
+
+        img = torch.empty((1, 3, 224, 224), dtype=self.engine.dtype, device=dev)
         if W == H:
             src = res
         else:                                                       # centred padding (vstar_bench_eval.py:25-36)
@@ -548,13 +570,13 @@ class VQA_LLM:
             src = bg.view(1, 1, 3).expand(side, side, 3).contiguous()
             left, top = (side - W) // 2, (side - H) // 2
             src[top:top + H, left:left + W] = res
-        pipe._resize(src, 0, 0, side, side, side, side, 224, 224, out_bf16=img[0])
+        resize(src, 0, 0, side, side, side, side, img[0])
         crops = None
         if boxes is not None and len(boxes) > 0:
-            crops = torch.empty((len(boxes), 3, 224, 224), dtype=BF, device=dev)
+            crops = torch.empty((len(boxes), 3, 224, 224), dtype=self.engine.dtype, device=dev)
             for i, b in enumerate(boxes):
                 l, t, r, btm = self.get_patch(b, W, H, patch_scale=patch_scale)
-                pipe._resize(res, l, t, r - l, btm - t, r - l, btm - t, 224, 224, out_bf16=crops[i])
+                resize(res, l, t, r - l, btm - t, r - l, btm - t, crops[i])
         return img, crops
 
     @torch.inference_mode()
