@@ -172,6 +172,43 @@ int vsb_llama_layers_f16(const vsb_llama_layer_t* layers, int n_layers, void* x,
                          int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin, const void* positions,
                          const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded, void* scratch, void* stream);
 
+/* NF4 weights: the SEAL VQA LLM's 4-bit mode (the reference's load_4bit: bitsandbytes NF4, double-quantised scales, fp16 compute,
+ * LLaVA/llava/model/builder.py:26-43).  Format of W [N, K], K % 64 == 0 (csrc/nf4.cu, oracle/nf4_oracle.py): codes u8 [N, K/2], two
+ * 4-bit codes per byte with the first element in the high nibble, one fp32 scale per 64-value block [N, K/64]; a weight is
+ * f16(nf4[code] * scale).
+ * vsb_nf4_quantize: f16 W -> codes and the first-level fp32 absmax of every block (code = NF4 entry nearest to w * (1/absmax),
+ * ties to the lower code).  vsb_nf4_double_quant: absmax [n] -> scales [n] = map[q8] * absmax2 + offset, with offset = *offset (fp32
+ * on the device, the mean of absmax), groups of 256, map = the signed 8-bit dynamic map dmap [256] (fp32, sorted). */
+int vsb_nf4_quantize(const void* w, int N, int K, void* codes, void* absmax, void* stream);
+int vsb_nf4_double_quant(const void* absmax, long long n, const void* offset, const void* dmap, void* scales, void* stream);
+/* out [N, K] (row stride ldo) = f16 dequantisation of (codes, scales) */
+int vsb_nf4_dequant(const void* codes, const void* scales, int N, int K, void* out, long long ldo, void* stream);
+/* vsb_gemm_f16 with W = deq(codes, scales): same arguments, epilogues and semantics.  Small M: weight-streaming kernels that
+ * dequantise in registers (vsb_gemm_set_tuning 1 = CUDA-core kernel, M <= 8; 2 = mma.sync kernel, M <= 32); otherwise deq(W) is
+ * written to deq_scratch (f16, N*K elements) and vsb_gemm_f16 runs on it (a forced tile width selects this path). */
+int vsb_gemm_nf4(const void* A, long long lda, const void* codes, const void* scales, void* C, long long ldc, int M, int N, int K,
+                     const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
+                     long long group_stride, long long group_offset, void* deq_scratch, void* stream);
+/* vsb_llama_layers_f16 on NF4 projections: ln1 / ln2 f16 [d] (not folded), codes and scales of wqkv, wo, wgu, wdown in the layouts
+ * of vsb_llama_layer_t.  RMSNorm kernel then GEMM (norm_folded = 0 only); tail_rows must be 0.  deq_scratch: f16, 2*inter*d
+ * elements (the largest weight), used by the row counts that take the dequant + tile path. */
+typedef struct {
+  const void* ln1;
+  const void* wqkv_codes;
+  const void* wqkv_scales;
+  const void* wo_codes;
+  const void* wo_scales;
+  const void* ln2;
+  const void* wgu_codes;
+  const void* wgu_scales;
+  const void* wdown_codes;
+  const void* wdown_scales;
+} vsb_llama_layer_nf4_t;
+int vsb_llama_layers_nf4(const vsb_llama_layer_nf4_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
+                             int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
+                             const void* positions, const void* k_start, const void* q_seg, int seg_lo, void* scratch, void* deq_scratch,
+                             void* stream);
+
 /* softmax(QK^T*scale [+causal]) V, head_dim 64/128; element (b,s,h,d) at base + b*bs + s*rs + h*D + d.
  * HF CLIP/OWL attention (modeling_clip.py:261-329) and Llama attention (modeling_llama.py:199-221). */
 int vsb_flash_attn_bf16(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,

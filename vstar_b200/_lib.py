@@ -65,10 +65,25 @@ for _name in ("vsb_gemm", "vsb_gemm_rowscale", "vsb_gemm_qkv_rope", "vsb_rowsq",
     SIGNATURES[_name + "_f16"] = SIGNATURES[_name + "_bf16"]
 SIGNATURES["vsb_llama_layers_f16"] = SIGNATURES["vsb_llama_layers"]
 
+# NF4 weights (the SEAL VQA LLM's 4-bit mode)
+SIGNATURES.update({
+    "vsb_nf4_quantize": [c_p, c_i, c_i, c_p, c_p, c_p],
+    "vsb_nf4_double_quant": [c_p, c_ll, c_p, c_p, c_p, c_p],
+    "vsb_nf4_dequant": [c_p, c_p, c_i, c_i, c_p, c_ll, c_p],
+    "vsb_gemm_nf4": [c_p, c_ll, c_p, c_p, c_p, c_ll, c_i, c_i, c_i, c_p, c_p, c_ll, c_i, c_i, c_i, c_ll, c_ll, c_p, c_p],
+    "vsb_llama_layers_nf4": [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p],
+})
+
 
 class LlamaLayer(ctypes.Structure):
     """vsb_llama_layer_t"""
     _fields_ = [("ln1", c_p), ("wqkv", c_p), ("wo", c_p), ("ln2", c_p), ("wgu", c_p), ("wdown", c_p)]
+
+
+class LlamaLayerNF4(ctypes.Structure):
+    """vsb_llama_layer_nf4_t"""
+    _fields_ = [("ln1", c_p), ("wqkv_codes", c_p), ("wqkv_scales", c_p), ("wo_codes", c_p), ("wo_scales", c_p), ("ln2", c_p),
+                ("wgu_codes", c_p), ("wgu_scales", c_p), ("wdown_codes", c_p), ("wdown_scales", c_p)]
 
 
 _lib = None

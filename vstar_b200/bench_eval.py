@@ -44,6 +44,8 @@ def build_parser():
     p.add_argument("--search-batch", default=64, type=int, help="frontier crops per VSM call")
     p.add_argument("--vqa-dtype", default="bf16", choices=("bf16", "fp16"),
                    help="compute dtype of the SEAL VQA LLM: fp16 is the reference's (LLaVA/llava/model/builder.py:43); the VSM stays bf16")
+    p.add_argument("--vqa-load-4bit", action="store_true",
+                   help="load the SEAL VQA LLM's Linear weights in NF4 (the reference's load_4bit); computes in fp16 whatever --vqa-dtype says")
     return p
 
 

@@ -14,6 +14,7 @@
 
 void vsb_set_error(const char* fmt, ...);
 int vsb_batch_invariant();   // see api.cu
+int vsb_gemm_forced_bn();    // force_bn of vsb_gemm_set_tuning (gemm_tcgen05.cu)
 
 #define VSB_CHECK_ARG(cond, ...)                 \
   do {                                           \

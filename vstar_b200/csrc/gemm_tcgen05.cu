@@ -489,6 +489,7 @@ extern "C" int vsb_gemm_set_tuning(int force_bn, int max_ctas) {
   g_max_ctas = max_ctas;
   return VSB_OK;
 }
+int vsb_gemm_forced_bn() { return g_force_bn; }
 extern "C" int vsb_gemm_set_l2_hints(int on) {
   g_l2_hints = on;
   return VSB_OK;

@@ -167,6 +167,64 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
   return VSB_OK;
 }
 
+int vsb_nf4_variant(int M);   // nf4.cu: 0 = the NF4 GEMM of M rows dequantises W and runs the tile kernels
+
+// NF4 projections (the SEAL VQA LLM's 4-bit mode): the unfused sequence above on vsb_gemm_nf4.  Where an M-row NF4 GEMM takes
+// the dequant + tile path, the QKV projection dequantises wqkv itself and uses the fused-RoPE tile epilogue like the f16 runner.
+extern "C" int vsb_llama_layers_nf4(const vsb_llama_layer_nf4_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache,
+                                        int Bc, int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
+                                        const void* positions, const void* k_start, const void* q_seg, int seg_lo, void* scratch,
+                                        void* deq_scratch, void* stream) {
+  using K = LayerOps<half>;
+  VSB_CHECK_ARG(layers && x && cache && rope_cos && rope_sin && scratch && deq_scratch, "vsb_llama_layers_nf4: null pointer");
+  VSB_CHECK_ARG(n_layers > 0 && B > 0 && Tn > 0 && past >= 0 && d > 0 && H > 0 && inter > 0, "vsb_llama_layers_nf4: bad shape");
+  VSB_CHECK_ARG(B <= Bc && past + Tn <= Tmax, "vsb_llama_layers_nf4: B=%d Tn=%d past=%d exceed the cache [%d, %d]", B, Tn, past, Bc, Tmax);
+  VSB_CHECK_ARG(d % H == 0, "vsb_llama_layers_nf4: hidden %d not divisible by heads %d", d, H);
+  VSB_CHECK_ARG(k_start == nullptr || Tn <= 4, "vsb_llama_layers_nf4: ragged batches (k_start) need Tn <= 4, got %d", Tn);
+  VSB_CHECK_ARG(q_seg == nullptr || k_start == nullptr, "vsb_llama_layers_nf4: q_seg excludes k_start");
+  const int hd = d / H;
+  const long long rows = (long long)B * Tn;
+  const long long ld = 3LL * d;
+  const float scale = 1.0f / sqrtf((float)hd);
+  half* xb = reinterpret_cast<half*>(x);
+  half* h = reinterpret_cast<half*>(scratch);           // [rows, d]
+  half* attn = h + rows * d;                            // [rows, d]
+  half* gu = attn + rows * d;                           // [rows, inter]
+  const bool tiles = vsb_nf4_variant((int)rows) == 0;
+  const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && tiles;
+  for (int li = 0; li < n_layers; ++li) {
+    const vsb_llama_layer_nf4_t& L = layers[li];
+    half* cl = reinterpret_cast<half*>(cache) + (long long)li * Bc * Tmax * ld;
+    VSB_TRY(K::rmsnorm(xb, d, L.ln1, h, d, (int)rows, d, rms_eps, stream));
+    if (rope_fused) {
+      VSB_TRY(vsb_nf4_dequant(L.wqkv_codes, L.wqkv_scales, 3 * d, d, deq_scratch, d, stream));
+      VSB_TRY(K::gemm_qkv_rope(h, d, deq_scratch, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, nullptr, 0, rms_eps, rows, rope_cos,
+                               rope_sin, positions, Tn, past, hd, stream));
+    } else {
+      VSB_TRY(vsb_gemm_nf4(h, d, L.wqkv_codes, L.wqkv_scales, cl, ld, (int)rows, 3 * d, d, nullptr, nullptr, 0, VSB_EPI_NONE, 0, Tn,
+                               Tmax, past, deq_scratch, stream));
+      VSB_TRY(K::rope(cl, ld, (int)rows, Tn, H, hd, past, rope_cos, rope_sin, positions, Tmax, past, stream));
+    }
+    if (q_seg != nullptr)
+      VSB_TRY(K::flash_attn_seg(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
+                                (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, scale, q_seg, seg_lo, stream));
+    else if (k_start != nullptr)
+      VSB_TRY(K::attn_decode(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
+                             (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, 1, scale, k_start, stream));
+    else
+      VSB_TRY(K::flash_attn(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
+                            (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, 1, scale, stream));
+    VSB_TRY(vsb_gemm_nf4(attn, d, L.wo_codes, L.wo_scales, xb, d, (int)rows, d, d, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0, deq_scratch,
+                             stream));
+    VSB_TRY(K::rmsnorm(xb, d, L.ln2, h, d, (int)rows, d, rms_eps, stream));
+    VSB_TRY(vsb_gemm_nf4(h, d, L.wgu_codes, L.wgu_scales, gu, inter, (int)rows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0,
+                             0, 0, deq_scratch, stream));
+    VSB_TRY(vsb_gemm_nf4(gu, inter, L.wdown_codes, L.wdown_scales, xb, d, (int)rows, d, inter, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0,
+                             deq_scratch, stream));
+  }
+  return VSB_OK;
+}
+
 extern "C" int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
                                 int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
                                 const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,

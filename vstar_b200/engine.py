@@ -40,28 +40,46 @@ class CoreWeights:
     dtype: torch.bfloat16 (default; the VSM) or torch.float16 (the SEAL VQA LLM as the reference runs it); the engine built on
     these weights computes in that dtype."""
 
-    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF):
+    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF, quant=None):
         if dtype not in (torch.bfloat16, torch.float16):
             raise ValueError(f"weights dtype must be torch.bfloat16 or torch.float16, got {dtype}")
+        if quant not in (None, "nf4") or (quant == "nf4" and dtype != torch.float16):
+            raise ValueError(f"quant must be None or 'nf4' (fp16 weights only), got {quant!r} with {dtype}")
         self.cfg = cfg
         self.device = device
         self.dtype = dtype
+        self.quant = quant
         dev = device
 
         def g(name):
             return get(name).to(device=dev, dtype=dtype).contiguous()
 
+        def lin(name):
+            """a Linear weight: NF4 when quantised, straight from the fp16 copy so that only one fp16 tensor is resident"""
+            return ops.nf4_quantize(g(name)) if quant else g(name)
+
         self._g = g
+        self._lin = lin
         c = cfg
         # ---- Llama
         self.embed = g("model.embed_tokens.weight")
         self.lm_head = g("lm_head.weight")
         self.final_norm = g("model.norm.weight")
         self.layers = []
-        self.fold_norms = os.environ.get("VSB_FOLD_NORMS", "1") != "0"
+        # NF4 quantises each HF tensor on its own, so the norms cannot be folded into the weights first
+        self.fold_norms = os.environ.get("VSB_FOLD_NORMS", "1") != "0" and not quant
         ones = None
         for i in range(c.n_layers):
             p = f"model.layers.{i}."
+            if quant:
+                self.layers.append(dict(
+                    wqkv=ops.NF4Weight.cat_rows([lin(p + "self_attn.q_proj.weight"), lin(p + "self_attn.k_proj.weight"),
+                                                 lin(p + "self_attn.v_proj.weight")]),
+                    wo=lin(p + "self_attn.o_proj.weight"),
+                    wgu=ops.NF4Weight.interleave_rows(lin(p + "mlp.gate_proj.weight"), lin(p + "mlp.up_proj.weight")),
+                    wdown=lin(p + "mlp.down_proj.weight"),
+                    ln1=g(p + "input_layernorm.weight"), ln2=g(p + "post_attention_layernorm.weight")))
+                continue
             wqkv = torch.cat([g(p + "self_attn.q_proj.weight"), g(p + "self_attn.k_proj.weight"), g(p + "self_attn.v_proj.weight")], 0)
             gate, up = g(p + "mlp.gate_proj.weight"), g(p + "mlp.up_proj.weight")
             wgu = torch.stack([gate, up], dim=1).reshape(2 * c.intermediate, c.hidden).contiguous()   # row 2j = gate_j, 2j+1 = up_j
@@ -87,11 +105,16 @@ class CoreWeights:
         # ---- ViTs
         self.clip = self._vit(g, "model.vision_tower.vision_tower.vision_model.", c.clip_layers + 1 + c.clip_select_layer
                               if c.clip_select_layer < 0 else c.clip_select_layer, c.clip_patch, "pre_layrnorm")
-        self.mm_w, self.mm_b = g("model.mm_projector.weight"), g("model.mm_projector.bias")
+        self.mm_w, self.mm_b = lin("model.mm_projector.weight"), g("model.mm_projector.bias")
 
     @classmethod
-    def from_state_dict(cls, cfg, sd, device="cuda", dtype=BF):
-        return cls(cfg, lambda n: sd[n], device, dtype=dtype)
+    def from_state_dict(cls, cfg, sd, device="cuda", dtype=BF, **kw):
+        return cls(cfg, lambda n: sd[n], device, dtype=dtype, **kw)
+
+    def linear_bytes(self):
+        """device bytes of the Llama and projector Linear weights (the ones NF4 quantises)"""
+        nb = ops.weight_nbytes
+        return sum(nb(L[k]) for L in self.layers for k in ops.NF4_LINEARS) + nb(self.mm_w)
 
     @staticmethod
     def _vit(g, p, n_layers, patch, pre_name):
@@ -118,9 +141,11 @@ class VSMWeights(CoreWeights):
     """+ OWL-ViT-B/16, OWL heads, [LOC] query MLPs, SAM prompt encoder / mask decoder (stacked class-head rows,
     permuted conv taps)."""
 
-    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF):
+    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF, quant=None):
         if dtype != BF:
             raise ValueError("the VSM runs in bf16 only, as in the reference (visual_search.py:145)")
+        if quant is not None:
+            raise ValueError("the VSM is not quantised: the reference loads it in bf16 only")
         super().__init__(cfg, get, device)
         g, c, dev = self._g, cfg, device
         self.owl = self._vit(g, "model.owlvit.vision_model.", c.owl_layers, c.owl_patch, "pre_layernorm")
@@ -330,10 +355,14 @@ class LlamaClipCore:
             self._layer_table = ops.llama_layer_table(self.w.layers)
         Bc, Tm = self._cache_shape[1], self._cache_shape[2]
         scratch = torch.empty((B * Tn * (2 * c.hidden + c.intermediate),), dtype=self.dtype, device=self.dev)
+        deq = None
+        if getattr(self.w, "quant", None):
+            # NF4 projections dequantise into this buffer on the row counts that take the tile kernels
+            deq = torch.empty((2 * c.intermediate * c.hidden,), dtype=self.dtype, device=self.dev)
         return ops.llama_layers(self._layer_table, len(self.w.layers), x, B, Tn, past, self._cache, Bc, Tm, c.hidden, c.n_heads,
                                 c.intermediate, c.rms_eps, self.w.rope_cos, self.w.rope_sin, scratch, positions=positions,
                                 k_start=k_start, cache_row_offset=cache_row_offset, tail_rows=tail_rows, q_seg=q_seg, seg_lo=seg_lo,
-                                norm_folded=getattr(self.w, "fold_norms", False))
+                                norm_folded=getattr(self.w, "fold_norms", False), deq_scratch=deq)
 
     def _logits_rows(self, x, rows):
         """final RMSNorm + lm_head on selected rows of the residual stream -> (hidden [n,d], argmax [n], logits fp32 [n,V])"""

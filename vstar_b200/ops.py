@@ -93,9 +93,115 @@ def profile_end():
     return f.value, t.value, n.value
 
 
+NF4_LINEARS = ("wqkv", "wo", "wgu", "wdown")
+
+
+class NF4Weight:
+    """A weight W [N, K] in NF4 (the SEAL VQA LLM's 4-bit mode, see include/vstar_b200.h): codes uint8 [N, K/2] (first element of
+    a pair in the high nibble) and fp32 scales [N, K/64], one per 64-value block.  W dequantises to f16(nf4[code] * scale)."""
+
+    def __init__(self, codes, scales, N, K):
+        assert codes.dtype == torch.uint8 and codes.shape == (N, K // 2) and codes.is_contiguous()
+        assert scales.dtype == torch.float32 and scales.shape == (N, K // 64) and scales.is_contiguous()
+        self.codes, self.scales, self.N, self.K = codes, scales, N, K
+
+    @property
+    def shape(self):
+        return (self.N, self.K)
+
+    @property
+    def nbytes(self):
+        return self.codes.numel() + 4 * self.scales.numel()
+
+    @staticmethod
+    def cat_rows(ws):
+        """rows of several NF4 weights of the same K stacked (wqkv = q | k | v)"""
+        assert len({w.K for w in ws}) == 1
+        return NF4Weight(torch.cat([w.codes for w in ws], 0), torch.cat([w.scales for w in ws], 0), sum(w.N for w in ws), ws[0].K)
+
+    @staticmethod
+    def interleave_rows(a, b):
+        """row 2j = a_j, row 2j+1 = b_j (wgu: gate / up)"""
+        assert a.shape == b.shape
+        return NF4Weight(torch.stack([a.codes, b.codes], 1).reshape(2 * a.N, -1).contiguous(),
+                         torch.stack([a.scales, b.scales], 1).reshape(2 * a.N, -1).contiguous(), 2 * a.N, a.K)
+
+
+def weight_nbytes(w):
+    """device bytes of a dense or NF4 weight"""
+    return w.nbytes if isinstance(w, NF4Weight) else w.numel() * w.element_size()
+
+
+def nf4_dynamic_map(device):
+    """bitsandbytes' create_dynamic_map(signed=True, max_exponent_bits=7, total_bits=8): 256 sorted fp32 values"""
+    data = []
+    for i in range(7):
+        b = torch.linspace(0.1, 1, 2 ** i + 1)
+        means = (b[:-1] + b[1:]) / 2.0
+        data += ((10 ** (-6 + i)) * means).tolist()
+        data += (-(10 ** (-6 + i)) * means).tolist()
+    data += [0.0, 1.0]
+    data.sort()
+    return torch.tensor(data, dtype=torch.float32).to(device)
+
+
+_DMAP = {}
+
+
+def nf4_quantize(w):
+    """fp16 [N, K] CUDA tensor (K % 64 == 0) -> NF4Weight, with bitsandbytes' double quant of the block scales (offset = mean of
+    the block absmax, taken on the device)"""
+    _chk(w, F16)
+    assert w.dim() == 2 and w.is_contiguous()
+    N, K = w.shape
+    if K % 64:
+        raise _lib.VsbError(f"NF4 needs K % 64 == 0 (64-value blocks inside one row), got K = {K}")
+    codes = torch.empty((N, K // 2), dtype=torch.uint8, device=w.device)
+    absmax = torch.empty((N, K // 64), dtype=torch.float32, device=w.device)
+    _lib.launches += 2
+    call("vsb_nf4_quantize", w.data_ptr(), N, K, codes.data_ptr(), absmax.data_ptr(), _stream())
+    offset = absmax.mean()
+    dmap = _DMAP.get(w.device)
+    if dmap is None:
+        dmap = _DMAP[w.device] = nf4_dynamic_map(w.device)
+    scales = torch.empty_like(absmax)
+    call("vsb_nf4_double_quant", absmax.data_ptr(), absmax.numel(), offset.data_ptr(), dmap.data_ptr(), scales.data_ptr(), _stream())
+    return NF4Weight(codes, scales, N, K)
+
+
+def nf4_dequant(w, out=None):
+    """NF4Weight -> fp16 [N, K] (into `out`, a view with unit inner stride, if given)"""
+    if out is None:
+        out = torch.empty((w.N, w.K), dtype=F16, device=w.codes.device)
+    _chk(out, F16)
+    assert out.shape == (w.N, w.K) and out.stride(1) == 1
+    _lib.launches += 1
+    call("vsb_nf4_dequant", w.codes.data_ptr(), w.scales.data_ptr(), w.N, w.K, out.data_ptr(), out.stride(0), _stream())
+    return out
+
+
+def _layer_nf4(L):
+    return isinstance(L["wqkv"], NF4Weight)
+
+
 def llama_layer_table(layers):
     """layers: list of dicts with ln1, wqkv, wo, ln2, wgu, wdown tensors (kept alive by the caller), all bf16 or all fp16
-    -> ctypes array"""
+    -> ctypes array.  NF4 layers (wqkv, wo, wgu, wdown NF4Weight, fp16 ln1 / ln2) -> the vsb_llama_layer_nf4_t array; a table
+    cannot mix NF4 and dense layers."""
+    kinds = {_layer_nf4(L) for L in layers}
+    if len(kinds) > 1 or any(isinstance(L[k], NF4Weight) != _layer_nf4(L) for L in layers for k in NF4_LINEARS):
+        raise _lib.VsbError("a layer table cannot mix NF4 and fp16 / bf16 projections")
+    if kinds == {True}:
+        arr = (_lib.LlamaLayerNF4 * len(layers))()
+        for i, L in enumerate(layers):
+            for k in ("ln1", "ln2"):
+                _chk(L[k], F16)
+                assert L[k].is_contiguous(), k
+                setattr(arr[i], k, L[k].data_ptr())
+            for k in NF4_LINEARS:
+                setattr(arr[i], k + "_codes", L[k].codes.data_ptr())
+                setattr(arr[i], k + "_scales", L[k].scales.data_ptr())
+        return arr
     arr = (_lib.LlamaLayer * len(layers))()
     dtypes = set()
     for i, L in enumerate(layers):
@@ -110,7 +216,7 @@ def llama_layer_table(layers):
 
 
 def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, eps, rope_cos, rope_sin, scratch, positions=None,
-                 k_start=None, cache_row_offset=0, tail_rows=0, q_seg=None, seg_lo=0, norm_folded=False):
+                 k_start=None, cache_row_offset=0, tail_rows=0, q_seg=None, seg_lo=0, norm_folded=False, deq_scratch=None):
     """whole decoder stack in ONE native call (csrc/llama_layers.cu): in place on x [B*Tn, d].
     cache_row_offset shifts the cache origin by that many [3d] rows (a sequence placed at batch slot b, first row s:
     b*Tmax + s) so a single sequence can be prefilled anywhere in a shared cache; positions / k_start: ragged decode;
@@ -118,8 +224,11 @@ def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, 
     q_seg int32 [B*Tn] + seg_lo: the new rows are several continuations of the cached prefix [0, seg_lo) appended back to back;
     row r attends the prefix and its own continuation from key q_seg[r] on;
     norm_folded: ln1 / ln2 are already multiplied into wqkv / wgu (fused RMSNorm path, see vsb_llama_layers).
-    x, cache, scratch, the RoPE tables and the table's weights are all bf16 or all fp16 (vsb_llama_layers_f16)."""
-    fn = "vsb_llama_layers" if _sfx(x, cache, scratch, rope_cos, rope_sin) == "bf16" else "vsb_llama_layers_f16"
+    x, cache, scratch, the RoPE tables and the table's weights are all bf16 or all fp16 (vsb_llama_layers_f16).
+    An NF4 table (fp16 only, norms not folded, tail_rows 0) runs vsb_llama_layers_nf4 and needs deq_scratch, fp16 with
+    2 * inter * d elements."""
+    sfx = _sfx(x, cache, scratch, rope_cos, rope_sin)
+    fn = "vsb_llama_layers" if sfx == "bf16" else "vsb_llama_layers_f16"
     assert x.is_contiguous() and cache.is_contiguous() and x.shape == (B * Tn, d)
     assert scratch.numel() >= B * Tn * (2 * d + inter)
     for t in (positions, k_start, q_seg):
@@ -127,6 +236,16 @@ def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, 
     assert q_seg is None or (q_seg.numel() == B * Tn and positions is not None)
     assert positions is None or positions.numel() == B * Tn
     assert k_start is None or k_start.numel() == B
+    if isinstance(table[0], _lib.LlamaLayerNF4):
+        if sfx != "f16" or norm_folded or tail_rows:
+            raise _lib.VsbError("NF4 layers run in fp16 with unfolded norms and tail_rows = 0")
+        _chk(deq_scratch, F16)
+        assert deq_scratch.is_contiguous() and deq_scratch.numel() >= 2 * inter * d
+        _lib.launches += 9 * n_layers
+        call("vsb_llama_layers_nf4", table, n_layers, x.data_ptr(), B, Tn, past, cache.data_ptr() + cache_row_offset * 3 * d * 2, Bc,
+             Tmax, d, H, inter, float(eps), rope_cos.data_ptr(), rope_sin.data_ptr(), _p(positions), _p(k_start), _p(q_seg), int(seg_lo),
+             scratch.data_ptr(), deq_scratch.data_ptr(), _stream())
+        return x
     _lib.launches += (6 if (norm_folded and k_start is None and (B * Tn > 16 or batch_invariant.depth > 0)) else 8) * n_layers + \
         (2 if (tail_rows > 0 and 2 * tail_rows <= Tn and k_start is None) else 0)
     call(fn, table, n_layers, x.data_ptr(), B, Tn, past, cache.data_ptr() + cache_row_offset * 3 * d * 2, Bc, Tmax, d, H,
@@ -135,10 +254,46 @@ def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, 
     return x
 
 
+def _gemm_out(a, M, n_out, out, out_dtype, out_rows, residual):
+    if out is None:
+        out = torch.empty((out_rows if out_rows is not None else M, n_out), dtype=out_dtype or a.dtype, device=a.device)
+    _chk(out)
+    assert out.dim() == 2 and out.stride(1) == 1 and out.shape[1] >= n_out
+    if out.dtype != torch.float32:
+        _sfx(a, out)
+    if residual is not None:
+        _chk(residual, out.dtype)
+        assert residual.stride(1) == 1
+    return out
+
+
+def _gemm_nf4(a, w, out, bias, residual, epilogue, out_dtype, rows_per_group, group_stride, group_offset, out_rows, deq_scratch):
+    _sfx(a, bias)
+    _chk(a, F16)
+    pa, M, K, lda = _rows2d(a)
+    assert K == w.K, (a.shape, w.shape)
+    N = w.N
+    out = _gemm_out(a, M, N // 2 if epilogue == EPI_SWIGLU else N, out, out_dtype, out_rows, residual)
+    if bias is not None:
+        assert bias.numel() == N and bias.is_contiguous()
+    if deq_scratch is None:
+        deq_scratch = torch.empty((N * K,), dtype=F16, device=a.device)
+    _chk(deq_scratch, F16)
+    assert deq_scratch.is_contiguous() and deq_scratch.numel() >= N * K
+    _lib.launches += 1
+    call("vsb_gemm_nf4", pa, lda, w.codes.data_ptr(), w.scales.data_ptr(), out.data_ptr(), out.stride(0), M, N, K, _p(bias), _p(residual),
+         residual.stride(0) if residual is not None else 0, epilogue, 1 if out.dtype == torch.float32 else 0, rows_per_group, group_stride,
+         group_offset, deq_scratch.data_ptr(), _stream())
+    return out
+
+
 def gemm(a, w, out=None, bias=None, residual=None, epilogue=EPI_NONE, out_dtype=None, rows_per_group=0,
-         group_stride=0, group_offset=0, out_rows=None):
+         group_stride=0, group_offset=0, out_rows=None, deq_scratch=None):
     """out = epi(a @ w.T + bias) (+ residual).  a [M,K], w [N,K] bf16 or fp16 (row stride arbitrary, inner stride 1); out is
-    fp32 or the operands' dtype (default)."""
+    fp32 or the operands' dtype (default).  w may be an NF4Weight (fp16 a): vsb_gemm_nf4, with deq_scratch (fp16, N*K
+    elements) allocated here unless given."""
+    if isinstance(w, NF4Weight):
+        return _gemm_nf4(a, w, out, bias, residual, epilogue, out_dtype, rows_per_group, group_stride, group_offset, out_rows, deq_scratch)
     sfx = _sfx(a, w, bias)
     pa, M, K, lda = _rows2d(a)
     pw, N, K2, ldw = _rows2d(w)

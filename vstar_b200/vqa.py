@@ -71,9 +71,9 @@ class VQAWeights(CoreWeights):
     """CoreWeights + the object projector `model.mm_projector_object.{0,1,2}` (multimodal_projector/builder.py:54-68).
     dtype: torch.bfloat16 (default) or torch.float16 (the reference's dtype for this model)."""
 
-    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF):
-        super().__init__(cfg, get, device, dtype=dtype)
-        g = self._g
+    def __init__(self, cfg: VSMConfig, get, device="cuda", dtype=BF, quant=None):
+        super().__init__(cfg, get, device, dtype=dtype, quant=quant)
+        g, lin = self._g, self._lin
         p = "model.mm_projector_object."
         self.pj_ln = (g(p + "0.weight"), g(p + "0.bias"))
         self.latents = g(p + "1.latents")
@@ -83,10 +83,14 @@ class VQAWeights(CoreWeights):
             a, f = f"{p}1.layers.{i}.0.", f"{p}1.layers.{i}.1."
             self.pj_layers.append(dict(
                 nm=(g(a + "norm_media.weight"), g(a + "norm_media.bias")), nl=(g(a + "norm_latents.weight"), g(a + "norm_latents.bias")),
-                wq=g(a + "to_q.weight"), wkv=g(a + "to_kv.weight"), wo=g(a + "to_out.weight"),
-                ffn=(g(f + "0.weight"), g(f + "0.bias")), w1=g(f + "1.weight"), w2=g(f + "3.weight")))
+                wq=lin(a + "to_q.weight"), wkv=lin(a + "to_kv.weight"), wo=lin(a + "to_out.weight"),
+                ffn=(g(f + "0.weight"), g(f + "0.bias")), w1=lin(f + "1.weight"), w2=lin(f + "3.weight")))
         self.pj_norm = (g(p + "1.norm.weight"), g(p + "1.norm.bias"))
-        self.pj_out = (g(p + "2.weight"), g(p + "2.bias"))
+        self.pj_out = (lin(p + "2.weight"), g(p + "2.bias"))
+
+    def linear_bytes(self):
+        nb = ops.weight_nbytes
+        return super().linear_bytes() + sum(nb(L[k]) for L in self.pj_layers for k in ("wq", "wkv", "wo", "w1", "w2")) + nb(self.pj_out[0])
 
 
 class VQAEngine(LlamaClipCore):
@@ -466,32 +470,40 @@ def load_pretrained_model(model_path, model_base=None, model_name=None, load_8bi
                           device="cuda", torch_dtype=None):
     """Drop-in for /root/reference/LLaVA/llava/model/builder.py:26-151 (the SEAL VQA LLM branch):
     -> (tokenizer, model, image_processor, context_len).  model_path: local `seal_vqa_7b` checkpoint directory (HF
-    safetensors / .bin shards in the reference's key layout).  bitsandbytes paths are out of scope.
-    torch_dtype: None / torch.bfloat16 (default) or torch.float16 (the reference's dtype, builder.py:43) for the engine."""
+    safetensors / .bin shards in the reference's key layout).
+    torch_dtype: None / torch.bfloat16 (default) or torch.float16 (the reference's dtype, builder.py:43) for the engine.
+    load_4bit: the reference's bitsandbytes NF4 mode (builder.py:33-40): every Llama and projector Linear in NF4 with
+    double-quantised scales, CLIP / embeddings / lm_head / norms / biases in fp16, compute in fp16 (torch_dtype None or fp16).
+    load_8bit (LLM.int8 with outlier decomposition) is not implemented."""
     import os
-    if load_8bit or load_4bit:
-        raise NotImplementedError("load_8bit / load_4bit (bitsandbytes) are outside the hot-path scope (SURVEY.md §2)")
+    if load_8bit:
+        raise NotImplementedError("load_8bit (bitsandbytes LLM.int8) is not implemented; load_4bit (NF4) is")
+    if load_4bit and torch_dtype not in (None, torch.float16):
+        raise ValueError(f"load_4bit computes in fp16 (the reference's bnb_4bit_compute_dtype), got torch_dtype={torch_dtype}")
     if not os.path.isdir(str(model_path)):
         raise FileNotFoundError("load_pretrained_model: model_path must be a local checkpoint directory (no network here)")
     from transformers import AutoTokenizer
     from .vsm import config_from_hf, open_checkpoint
     tokenizer = AutoTokenizer.from_pretrained(model_path, use_fast=False)
     cfg = config_from_hf(model_path)
-    dtype = BF if torch_dtype is None else torch_dtype
-    engine = VQAEngine(VQAWeights(cfg, open_checkpoint(model_path, device=device), device=device, dtype=dtype))
+    dtype = torch.float16 if load_4bit else (BF if torch_dtype is None else torch_dtype)
+    engine = VQAEngine(VQAWeights(cfg, open_checkpoint(model_path, device=device), device=device, dtype=dtype,
+                                  quant="nf4" if load_4bit else None))
     return tokenizer, LlavaSearchModel(engine, getattr(tokenizer, "eos_token_id", 2)), _Proc(), 2048
 
 
 class VQA_LLM:
-    """Same surface as /root/reference/vstar_bench_eval.py:38-165.  args.vqa_dtype (optional): "bf16" (default) or "fp16"."""
+    """Same surface as /root/reference/vstar_bench_eval.py:38-165.  args.vqa_dtype (optional): "bf16" (default) or "fp16";
+    args.vqa_load_4bit (optional): NF4 Linear weights, fp16 compute (load_pretrained_model(load_4bit=True))."""
 
     def __init__(self, args=None, engine: VQAEngine = None, tokenizer=None, conv_type="v1"):
         if engine is None:
             name = getattr(args, "vqa_dtype", None) or "bf16"
             if name not in VQA_DTYPES:
                 raise ValueError(f"vqa_dtype must be one of {sorted(VQA_DTYPES)}, got {name!r}")
+            load_4bit = bool(getattr(args, "vqa_load_4bit", False))      # NF4 computes in fp16 whatever vqa_dtype says
             self.tokenizer, self.model, self.image_processor, self.context_len = load_pretrained_model(
-                args.vqa_model_path, None, None, torch_dtype=VQA_DTYPES[name])
+                args.vqa_model_path, None, None, load_4bit=load_4bit, torch_dtype=None if load_4bit else VQA_DTYPES[name])
             self.engine = self.model.engine
             self.conv_type = getattr(args, "conv_type", "v1")
             self.eos = getattr(self.tokenizer, "eos_token_id", 2)
