@@ -14,10 +14,10 @@
 // lm_head, the [LOC]-row MLPs, OWL class/box heads and the SAM decoder linears
 // and 3x3 convs (im2col).
 //
-// Warp groups (384 threads): warpgroup 0 = TMA producer (1 thread issues, the
-// rest idle with a minimal register budget), warpgroups 1 and 2 = consumers:
-// consumer c issues m64nBNk16 wgmma on rows [64c, 64c + 64) of the tile and
-// stores them.
+// Warp groups (384 threads): warpgroup 0 = producer, minimal register budget: thread 0 issues the TMA loads, warps 1-3
+// compute the folded-RMSNorm row scales of the tile the consumers finish next; warpgroups 1 and 2 = consumers: consumer c
+// issues m64nBNk16 wgmma on rows [64c, 64c + 64) of the tile and stores them, reading each 32-column chunk's bias / residual
+// before the previous chunk's stores.
 #include "common.cuh"
 #include "vstar_b200.h"
 #include "wgmma.cuh"
@@ -125,6 +125,9 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   return d;
 }
 
+constexpr int RSTD_THREADS = 96;    // warps 1-3 of the producer warpgroup: folded-RMSNorm row scales (tile_rstd)
+constexpr int RSTD_PIECE = 16;      // rowsq_in chunks staged per round trip
+
 template <int BN>
 struct SmemLayout {
   static constexpr int A_BYTES = BM * BK * 2;
@@ -132,7 +135,10 @@ struct SmemLayout {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : (BN == 64 ? 8 : 10));
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;  // barriers + alignment slack
+  static constexpr int RSTD_OFFSET = BAR_OFFSET + 256;   // float [2][BM]: folded-RMSNorm row scales, two tiles in flight
+  static constexpr int PART_OFFSET = RSTD_OFFSET + 2 * BM * 4;   // float [RSTD_PIECE][BM]: staged partial sums (tile_rstd)
+  static constexpr int TOTAL = PART_OFFSET + RSTD_PIECE * BM * 4 + 1024;  // + alignment slack
+  static_assert((2 * STAGES + 4) * 8 <= 256, "barriers overflow their 256-byte slot");
 };
 
 __device__ __forceinline__ float apply_act(float x, int epi) {
@@ -161,25 +167,91 @@ __device__ __forceinline__ long long remap_row(const GemmParams<T>& p, int m) {
   return (long long)(m / p.rows_per_group) * p.group_stride + p.group_offset + (m % p.rows_per_group);
 }
 
-// 1 / rms of A row m from the partial sums a producer GEMM (or vsb_rowsq_bf16) left behind; fixed summation order
+__device__ __forceinline__ void cp_async4(float* smem_dst, const float* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// 1 / rms of the BM rows of m-block m_blk from the partial sums a producer GEMM (or vsb_rowsq_bf16) left behind:
+// out[r] = rsqrt(sum_c rowsq_in[c][m] * sq_inv_cols + sq_eps), summed in fp32 from 0 over c = 0 .. sq_in_chunks - 1 in order;
+// 1 for rows >= M.  Run by the producer warpgroup's warps 1-3, thread r0 taking rows r0 and r0 + RSTD_THREADS.  The partials
+// are staged through `part` by cp.async, RSTD_PIECE chunks per round trip: under the producer's 40-register budget plain loads
+// keep only 2-3 in flight, and the sum of 128 chunks then outlasts a tile's main loop.  Each thread reads back only what it copied.
 template <typename T>
-__device__ __forceinline__ float row_rstd(const GemmParams<T>& p, int m) {
-  if (p.rowsq_in == nullptr || m >= p.M) return 1.f;
-  float s = 0.f;
-  for (int c = 0; c < p.sq_in_chunks; ++c) s += p.rowsq_in[(long long)c * p.sq_ld + m];
-  return rsqrtf(s * p.sq_inv_cols + p.sq_eps);
+__device__ __forceinline__ void tile_rstd(const GemmParams<T>& p, int m_blk, int r0, float* part, float* out) {
+  const int r[2] = {r0, r0 + RSTD_THREADS};
+  const bool ok[2] = {m_blk * BM + r[0] < p.M, r[1] < BM && m_blk * BM + r[1] < p.M};
+  float s[2] = {0.f, 0.f};
+  for (int c0 = 0; c0 < p.sq_in_chunks; c0 += RSTD_PIECE) {
+    const int nc = min(RSTD_PIECE, p.sq_in_chunks - c0);
+    for (int i = 0; i < nc; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (ok[h]) cp_async4(part + i * BM + r[h], p.rowsq_in + (long long)(c0 + i) * p.sq_ld + m_blk * BM + r[h]);
+    cp_async_wait_all();
+    for (int i = 0; i < nc; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (ok[h]) s[h] += part[i * BM + r[h]];
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+    if (r[h] < BM) out[r[h]] = ok[h] ? rsqrtf(s[h] * p.sq_inv_cols + p.sq_eps) : 1.f;
 }
 
 // ---------------------------------------------------------------- epilogue of one accumulator pair
-// row orow (already remapped), columns n, n+1 (n even, n < N): bias -> activation / SwiGLU -> (+residual) -> T / fp32 store.
-// Returns the sum of squares of the T values stored (the folded-RMSNorm row statistics).
+// Bias and residual of one accumulator pair (row orow, columns n, n+1), as fp32.  The epilogue reads them a 32-column chunk
+// ahead of its stores: C, bias and residual may alias (the o-proj and down-proj GEMMs add in place, residual == C), so a load
+// written after a store is issued after it, and a chain of load -> add -> store per pair would expose one memory round trip
+// per pair.  Each element is still read before it is written, by the same thread.
+struct PairIn {
+  float b0, b1, r0, r1;
+};
+
 template <typename T>
-__device__ __forceinline__ float epilogue_pair(const GemmParams<T>& p, long long orow, int n, float x0, float x1, bool swiglu) {
+__device__ __forceinline__ PairIn load_pair(const GemmParams<T>& p, long long orow, int n) {
+  using E = ElemT<T>;
+  const bool has1 = n + 1 < p.N;
+  PairIn in{0.f, 0.f, 0.f, 0.f};
+  if (p.bias != nullptr) {
+    in.b0 = E::to_f(p.bias[n]);
+    if (has1) in.b1 = E::to_f(p.bias[n + 1]);
+  }
+  if (p.residual == nullptr) return in;
+  if (p.out_fp32) {
+    const float* r = reinterpret_cast<const float*>(p.residual) + orow * p.ldr + n;
+    if (has1 && p.vec2) {
+      const float2 rv = *reinterpret_cast<const float2*>(r);
+      in.r0 = rv.x;
+      in.r1 = rv.y;
+    } else {
+      in.r0 = r[0];
+      if (has1) in.r1 = r[1];
+    }
+  } else {
+    const T* r = reinterpret_cast<const T*>(p.residual) + orow * p.ldr + n;
+    if (has1 && p.vec2) {
+      const float2 rv = E::unpack2(*reinterpret_cast<const uint32_t*>(r));
+      in.r0 = rv.x;
+      in.r1 = rv.y;
+    } else {
+      in.r0 = E::to_f(r[0]);
+      if (has1) in.r1 = E::to_f(r[1]);
+    }
+  }
+  return in;
+}
+
+// row orow (already remapped), columns n, n+1 (n even, n < N): bias -> activation / SwiGLU -> (+residual) -> T / fp32 store,
+// with bias and residual from load_pair.  Returns the sum of squares of the T values stored (the folded-RMSNorm row statistics).
+template <typename T>
+__device__ __forceinline__ float epilogue_pair(const GemmParams<T>& p, long long orow, int n, float x0, float x1, bool swiglu,
+                                               const PairIn& in) {
   using E = ElemT<T>;
   const bool has1 = n + 1 < p.N;
   if (p.bias != nullptr) {
-    x0 += E::to_f(p.bias[n]);
-    if (has1) x1 += E::to_f(p.bias[n + 1]);
+    x0 += in.b0;
+    if (has1) x1 += in.b1;
   }
   if (swiglu) {
     // interleaved weight rows: even column = gate_j, odd column = up_j -> out column n/2 (N is even)
@@ -188,27 +260,25 @@ __device__ __forceinline__ float epilogue_pair(const GemmParams<T>& p, long long
   }
   x0 = apply_act(x0, p.epilogue);
   x1 = apply_act(x1, p.epilogue);
+  if (p.residual != nullptr) {
+    x0 += in.r0;
+    if (has1) x1 += in.r1;
+  }
   if (p.out_fp32) {
     float* c = reinterpret_cast<float*>(p.C) + orow * p.ldc + n;
-    const float* r = p.residual ? reinterpret_cast<const float*>(p.residual) + orow * p.ldr + n : nullptr;
     if (has1 && p.vec2) {
-      if (r) { const float2 rv = *reinterpret_cast<const float2*>(r); x0 += rv.x; x1 += rv.y; }
       *reinterpret_cast<float2*>(c) = make_float2(x0, x1);
     } else {
-      if (r) { x0 += r[0]; if (has1) x1 += r[1]; }
       c[0] = x0;
       if (has1) c[1] = x1;
     }
     return 0.f;
   }
   T* c = reinterpret_cast<T*>(p.C) + orow * p.ldc + n;
-  const T* r = p.residual ? reinterpret_cast<const T*>(p.residual) + orow * p.ldr + n : nullptr;
   if (has1 && p.vec2) {
-    if (r) { const float2 rv = E::unpack2(*reinterpret_cast<const uint32_t*>(r)); x0 += rv.x; x1 += rv.y; }
     const uint32_t w = E::pack2(x0, x1);
     if (p.stream_out) __stcs(reinterpret_cast<unsigned int*>(c), w); else *reinterpret_cast<uint32_t*>(c) = w;
   } else {
-    if (r) { x0 += E::to_f(r[0]); if (has1) x1 += E::to_f(r[1]); }
     c[0] = E::from_f(x0);
     if (has1) c[1] = E::from_f(x1);
   }
@@ -249,11 +319,25 @@ __device__ __forceinline__ void rope_tile(const GemmParams<T>& p, float* acc, co
   }
 }
 
-// Epilogue of one consumer thread: rows m[0], m[1] of the tile, fragment columns 8j + 2t (see wgmma.cuh)
+// load_pair for the 8 accumulator pairs of one thread in the 32-column chunk starting at n0
+template <typename T>
+__device__ __forceinline__ void load_chunk(const GemmParams<T>& p, const bool* ok, const long long* orow, int n0, int t, PairIn (&in)[4][2]) {
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int n = n0 + 8 * jj + 2 * t;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (ok[h] && n < p.N) in[jj][h] = load_pair<T>(p, orow[h], n);
+  }
+}
+
+// Epilogue of one consumer thread: rows m[0], m[1] of the tile, fragment columns 8j + 2t (see wgmma.cuh); rs = their
+// folded-RMSNorm scales (1 without a folded norm)
 template <int BN, bool ROPE, typename T>
-__device__ __forceinline__ void epilogue_tile(const GemmParams<T>& p, float* acc, int m0, int n_blk, int t) {
+__device__ __forceinline__ void epilogue_tile(const GemmParams<T>& p, float* acc, int m0, int n_blk, int t, float rs0, float rs1) {
+  static_assert(BN % 32 == 0, "the epilogue works in whole 32-column chunks");
   const int m[2] = {m0, m0 + 8};
-  float rs[2] = {row_rstd(p, m[0]), row_rstd(p, m[1])};
+  float rs[2] = {rs0, rs1};
   const bool ok[2] = {m[0] < p.M, m[1] < p.M};
   const long long orow[2] = {ok[0] ? remap_row(p, m[0]) : 0, ok[1] ? remap_row(p, m[1]) : 0};
   const bool swiglu = (p.epilogue == VSB_EPI_SWIGLU);
@@ -264,18 +348,24 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams<T>& p, float* acc
       rs[0] = rs[1] = 1.f;
     }
   }
+  // fused QKV + RoPE has neither bias nor residual (gemm_qkv_rope): no input registers beside its 128 accumulators
+  const bool has_in = !ROPE && (p.bias != nullptr || p.residual != nullptr);
+  PairIn in[2][4][2];                              // chunk c uses in[c & 1] while chunk c + 1 loads into the other half
+  if (has_in) load_chunk<T>(p, ok, orow, n_tile0, t, in[0]);
 #pragma unroll
-  for (int c = 0; c < (BN + 31) / 32; ++c) {      // 32-column chunks (the granularity of the row statistics)
+  for (int c = 0; c < BN / 32; ++c) {              // 32-column chunks (the granularity of the row statistics)
     const int n0 = n_tile0 + 32 * c;
     if (n0 >= p.N) break;                          // warp-uniform
+    if (has_in && c + 1 < BN / 32 && n0 + 32 < p.N) load_chunk<T>(p, ok, orow, n0 + 32, t, in[(c + 1) & 1]);
     float sq[2] = {0.f, 0.f};
 #pragma unroll
-    for (int jj = 0; jj < 4 && 8 * (4 * c + jj) < BN; ++jj) {
+    for (int jj = 0; jj < 4; ++jj) {
       const int j = 4 * c + jj;
       const int n = n0 + 8 * jj + 2 * t;
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        if (ok[h] && n < p.N) sq[h] += epilogue_pair<T>(p, orow[h], n, acc[4 * j + 2 * h] * rs[h], acc[4 * j + 2 * h + 1] * rs[h], swiglu);
+        if (ok[h] && n < p.N)
+          sq[h] += epilogue_pair<T>(p, orow[h], n, acc[4 * j + 2 * h] * rs[h], acc[4 * j + 2 * h + 1] * rs[h], swiglu, in[c & 1][jj][h]);
     }
     if (p.rowsq_out != nullptr) {                  // N % 32 == 0: every chunk is complete
 #pragma unroll
@@ -306,6 +396,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* rstd_full = empty_bar + STAGES;     // [2]: the row scales of slot s are written
+  uint64_t* rstd_empty = rstd_full + 2;         // [2]: every consumer thread has read them
+  float* rstd_s = reinterpret_cast<float*>(smem + L::RSTD_OFFSET);   // [2][BM]
 
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
@@ -318,6 +411,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);   // one arrive per consumer warp
+    }
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&rstd_full[s], RSTD_THREADS);
+      mbar_init(&rstd_empty[s], 256);
     }
     fence_barrier_init();
   }
@@ -342,6 +439,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
+    } else if (threadIdx.x >= 32 && p.rowsq_in != nullptr) {
+      // warps 1-3: the folded-RMSNorm scale of each row of the tiles this CTA runs, one tile ahead of the consumers' epilogue
+      // (each row sum reads sq_in_chunks scattered floats; in the epilogue that latency would stall the tensor cores)
+      float* part = reinterpret_cast<float*>(smem + L::PART_OFFSET);
+      int it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        int m_blk, n_blk;
+        tile_coords(tile, p.tiles_m, p.tiles_n, p.group_m, m_blk, n_blk);
+        const int slot = it & 1;
+        mbar_wait(&rstd_empty[slot], ((it >> 1) & 1) ^ 1);
+        tile_rstd(p, m_blk, threadIdx.x - 32, part, rstd_s + slot * BM);
+        mbar_arrive(&rstd_full[slot]);
+      }
     }
     return;
   }
@@ -353,7 +463,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   float acc[BN / 2];
   int stage = 0;
   uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  int it = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
     int m_blk, n_blk;
     tile_coords(tile, p.tiles_m, p.tiles_n, p.group_m, m_blk, n_blk);
     int prev = -1;
@@ -378,7 +489,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     wgmma_wait<0>();
     fence_acc<BN / 2>(acc);
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
-    epilogue_tile<BN, ROPE, T>(p, acc, m_blk * BM + cw * 64 + wq * 16 + (lane >> 2), n_blk, lane & 3);
+    const int r = cw * 64 + wq * 16 + (lane >> 2);   // tile row of the thread's first accumulator row
+    float rs0 = 1.f, rs1 = 1.f;
+    if (p.rowsq_in != nullptr) {
+      const int slot = it & 1;
+      mbar_wait(&rstd_full[slot], (it >> 1) & 1);
+      rs0 = rstd_s[slot * BM + r];
+      rs1 = rstd_s[slot * BM + r + 8];
+      mbar_arrive(&rstd_empty[slot]);
+    }
+    epilogue_tile<BN, ROPE, T>(p, acc, m_blk * BM + r, n_blk, lane & 3, rs0, rs1);
   }
 }
 
