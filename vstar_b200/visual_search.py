@@ -9,7 +9,8 @@ What is different underneath (H100-first):
     expansion order (including heapq tie behaviour) is the reference's;
   * frontier nodes are evaluated SPECULATIVELY in batches (each node's outputs are a pure function of its crop) and
     committed strictly in pop order; speculative work is simply dropped when the search ends early;
-  * several searches can run in lock-step (`visual_search_many`) so their frontiers share one GPU batch;
+  * several searches can run in lock-step (`visual_search_many`) so their frontiers share one GPU batch, or be admitted
+    continuously into one controller (`SearchController.stream`, used by the search-only evaluation `main`);
   * every crop evaluation comes back as ONE fixed-size record (records.py): best score/box, the boxes above 0.5, the
     heat-map statistics and the sums of the normalised map over the crop's quad-tree descendants — computed on the GPU
     straight from the 192 x 192 low-res mask.  Committing a node is then pure host arithmetic on records of the node
@@ -22,6 +23,9 @@ from __future__ import annotations
 
 import argparse
 import functools
+import json
+import os
+import sys
 from queue import PriorityQueue
 
 import numpy as np
@@ -60,6 +64,12 @@ def parse_args(args):
     parser.add_argument("--vision-tower", default="openai/clip-vit-large-patch14", type=str)
     parser.add_argument("--use_mm_start_end", action="store_true", default=True)
     parser.add_argument("--conv_type", default="llava_v1", type=str, choices=["llava_v1", "llava_llama_2"])
+    # scheduling of `main` (not in the reference, which runs one search at a time); none of these changes a result
+    parser.add_argument("--searches-in-flight", default=32, type=int,
+                        help="searches kept active at once; the next target is admitted when one ends (1 = the reference's order)")
+    parser.add_argument("--search-batch", default=64, type=int, help="frontier crops per VSM call")
+    parser.add_argument("--trajectory-json", default=None, type=str,
+                        help="write one record per target (expanded boxes and scores, final box, IoU, latency) to this file")
     return parser.parse_args(args)
 
 
@@ -575,14 +585,41 @@ class SearchController:
         return reqs
 
     def run(self, states):
+        """run a fixed list of searches together until the last one ends; results in the order of `states`"""
+        results = {id(st): res for st, res in self.stream(states)}
+        return [results[id(st)] for st in states]
+
+    def stream(self, states, window=None):
+        """Continuous admission: take searches from the iterable `states` as they are needed, keep at most `window` of them
+        active (None = all at once), and yield (state, result) for each search as soon as it ends.  A finished search frees its
+        slot for the next one before the next frontier batch is selected, so batches mix searches at different depths.  The
+        controller holds no reference to a yielded state; speculative crops of it that are still in flight are dropped with
+        their batch.  Sets `t_admit` / `t_done` (time.perf_counter) on every state."""
+        import time
         from collections import deque
+        feed = iter(states)
+        more = True
+        active = []
         inflight = deque()
         while True:
-            for st in states:
+            for st in active:
                 self._advance(st)
-            if self._serve_cues(states):
+            if any(st.done for st in active):
+                finished = [st for st in active if st.done]
+                active = [st for st in active if not st.done]
+                for st in finished:
+                    st.t_done = time.perf_counter()
+                    yield st, self._finish(st)
+                del finished, st
+            while more and (window is None or len(active) < window):
+                st = next(feed, None)
+                if st is None:
+                    more = False
+                    break
+                st.t_admit = time.perf_counter()
+                active.append(st)
+            if self._serve_cues(active):
                 continue               # replies are in: let the parked commits run on before evaluating more crops
-            active = [st for st in states if not st.done]
             if not active:
                 break                  # speculative batches still in flight are simply dropped
             if not self.pipelined:
@@ -603,7 +640,6 @@ class SearchController:
             if not inflight:
                 raise RuntimeError("search controller stalled: active searches but nothing to evaluate")
             self._collect(inflight.popleft())
-        return [self._finish(st) for st in states]
 
     @staticmethod
     def _finish(st: SearchState):
@@ -651,3 +687,127 @@ def visual_search_many(vsm, jobs, batch_size=8, scorer=None, extract_noun_chunks
     states = [SearchState(img, name, ss, **kw) for img, name, ss in jobs]
     ctl = SearchController(vsm, scorer, batch_size, extract_noun_chunks, depth=depth)
     return ctl.run(states), states
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# search-only V*Bench evaluation (visual_search.py:520-564)
+# ---------------------------------------------------------------------------------------------------------------
+def _decode(path):
+    from PIL import Image
+    with Image.open(path) as im:
+        return im.convert("RGB")
+
+
+def _benchmark_images(args, pool, lookahead):
+    """(test_type, image_file, [(gt_bbox, target_object)], PIL image) per image with at least one target, in the reference's
+    order: direct_attributes then relative_position, files in os.listdir order.  Images are decoded on `pool`, `lookahead`
+    images ahead of the caller.  The annotation is the image FILE name cut at its first '.' (bench_eval.list_samples); the
+    reference cuts the whole path there, which breaks under a directory whose name contains a dot."""
+    from collections import deque
+    from .bench_eval import TEST_TYPES, list_samples
+
+    def entries():
+        for test_type in TEST_TYPES:
+            if args.visualization:
+                os.makedirs(os.path.join(args.output_path, test_type), exist_ok=True)
+            for image_file, image_path, annotation_path in list_samples(os.path.join(args.benchmark_folder, test_type)):
+                with open(annotation_path) as f:
+                    ann = json.load(f)
+                targets = list(zip(ann["bbox"], ann["target_object"]))
+                if targets:
+                    yield test_type, image_file, targets, image_path
+
+    ahead = deque()
+    for entry in entries():
+        ahead.append((entry, pool.submit(_decode, entry[3])))
+        if len(ahead) > lookahead:
+            (test_type, image_file, targets, _), fut = ahead.popleft()
+            yield test_type, image_file, targets, fut.result()
+    while ahead:
+        (test_type, image_file, targets, _), fut = ahead.popleft()
+        yield test_type, image_file, targets, fut.result()
+
+
+def main(args, vsm=None, scorer=None, extract_noun_chunks=None):
+    """The reference's search-only benchmark: one visual_search() per annotated target of V*Bench, then the two lines it prints
+    (average search path length over the hits, Top-1 accuracy at IoU > 0.5).  Same arguments, thresholds, per-target logic
+    and visualisation files.  The schedule differs: up to --searches-in-flight searches run at once in one SearchController,
+    the next target is admitted as soon as one ends, and the frontier batches mix their crops.  Every search is
+    independent of the others, so the per-target results do not depend on the window.  `vsm` may be injected; otherwise it
+    is built from the arguments as the reference does.  Returns the per-target records (see --trajectory-json)."""
+    from concurrent.futures import ThreadPoolExecutor
+    from .seal import smallest_size_for
+    args = parse_args(args)
+    if vsm is None:
+        from .vsm import VSM
+        vsm = VSM(args)
+    window = max(1, int(args.searches_in_flight))
+    ctl = SearchController(vsm, scorer, args.search_batch, extract_noun_chunks)
+    release = getattr(vsm, "release", None)
+    held = {}                  # id(image) -> [image, targets not finished yet]
+    thresholds = dict(confidence_high=args.confidence_high, confidence_low=args.confidence_low,
+                      target_cue_threshold=args.target_cue_threshold, target_cue_threshold_decay=args.target_cue_threshold_decay,
+                      target_cue_threshold_minimum=args.target_cue_threshold_minimum)
+
+    def states(images):
+        n = 0
+        for test_type, image_file, targets, image in images:
+            smallest = smallest_size_for(image, args.minimum_size_scale, args.minimum_size)
+            held[id(image)] = [image, len(targets)]
+            for i, (gt_bbox, object_name) in enumerate(targets):
+                st = SearchState(image, object_name, smallest, **thresholds)
+                st.sample = dict(order=n, test_type=test_type, image=image_file, target_index=i, target=object_name, gt_bbox=gt_bbox)
+                n += 1
+                yield st
+
+    records = []
+    with ThreadPoolExecutor(max_workers=1) as pool:
+        feed = states(_benchmark_images(args, pool, lookahead=max(2, window)))
+        for st, (final_step, path_length, ok, _) in ctl.stream(feed, window):
+            smp = st.sample
+            if args.visualization:           # visual_search.py:512-514, before main shifts the box (:552-555)
+                from .visualize import visualize_search_path
+                vis_path = os.path.join(args.output_path, smp["test_type"], "{}_{}".format(smp["image"].split(".")[0], smp["target_index"]))
+                visualize_search_path(st.image, st.search_path, path_length if ok else len(st.search_path), smp["gt_bbox"],
+                                      smp["target"], vis_path)
+            box, patch = final_step["detection_result"], final_step["bbox"]
+            if ok:
+                box[0] += patch[0]           # in place, as the reference does
+                box[1] += patch[1]
+            else:
+                box = box.clone()
+                box[0] += patch[0]
+                box[1] += patch[1]
+            iou_i = float(iou(box, smp["gt_bbox"]))
+            smp.update(search_successful=bool(ok), path_length=int(path_length), final_box=[float(v) for v in box], iou=iou_i,
+                       accuracy=(1.0 if iou_i > 0.5 else 0.0) if ok else 0,
+                       expanded=[dict(bbox=[int(v) for v in node["bbox"]], score=None if node["score"] is None else float(node["score"]),
+                                      context_cue=node.get("context_cue")) for node in st.search_path],
+                       evaluations=st.n_evals, latency_s=st.t_done - st.t_admit)
+            records.append(smp)
+            entry = held[id(st.image)]
+            entry[1] -= 1
+            if entry[1] == 0:                # last target of the image: drop its resident device copy now
+                del held[id(st.image)]
+                if release is not None:
+                    release(st.image)
+    records.sort(key=lambda r: r.pop("order"))
+    acc_list = [r["accuracy"] for r in records]
+    search_path_length_list = [r["path_length"] if r["search_successful"] else 0 for r in records]
+    avg_len = np.mean([search_path_length_list[i] for i in range(len(search_path_length_list)) if acc_list[i]])
+    top1 = np.mean(acc_list)
+    print("Avg search path length:", avg_len)
+    print("Top 1 Acc:", top1)
+    if args.trajectory_json:
+        def num(x):
+            return None if np.isnan(x) else float(x)
+        with open(args.trajectory_json, "w") as f:
+            json.dump(dict(avg_search_path_length=num(avg_len), top1_acc=num(top1), searches_in_flight=window,
+                           search_batch=args.search_batch, samples=records), f, indent=1)
+    return records
+
+
+if __name__ == "__main__":
+    # run the package's copy of this module: vsm.py imports it, and the controller's isinstance checks need ONE set of classes
+    from vstar_b200.visual_search import main as _main
+    _main(sys.argv[1:])
