@@ -8,7 +8,7 @@ Rows (bf16, random data, one H100 per run):
       gu    folded-RMSNorm input, SwiGLU
       down  K = 11008, in-place residual, row statistics out
   * the CLIP-L (M = B*257) and OWL-B (M = B*2305) Linears with bias / QuickGELU / residual;
-  * a K sweep (256 ... 4096) at the o and gu shapes of 64 crops.  Time is linear in K: the slope is the main loop's rate, the
+  * a K sweep (256 ... 4096) at the qkv, o and gu shapes of 64 crops and the CLIP qkv shape (bias) of 64 crops.  Time is linear in K: the slope is the main loop's rate, the
     intercept the cost every tile pays whatever K is (mostly the epilogue), reported per wave of tiles as well.
 Every row also times torch.matmul (cuBLAS) on the same M, N, K without an epilogue, as a reference for the card; cuBLAS is not
 used by the product.
@@ -186,9 +186,22 @@ def k_sweep(bf, sms, which, B, ks):
 
 
 def _sweep_call(bf, which, B, K):
-    """the o (in-place residual + row statistics) or gu (folded norm + SwiGLU) GEMM of B crops with its K changed"""
+    """the qkv (folded norm + RoPE + cache remap), o (in-place residual + row statistics), gu (folded norm + SwiGLU) or CLIP
+    qkv (bias) GEMM of B crops with its K changed"""
     M = B * T_CROP
     x, y, w = bf.x, bf.y, bf.w
+    if which == "qkv":
+        def f():
+            _lib.call("vsb_gemm_qkv_rope_bf16", x.data_ptr(), K, w.data_ptr(), K, bf.cache.data_ptr(), 3 * D, M, 3 * D, K, T_CROP, T_MAX,
+                      PAST, bf.sq_in.data_ptr(), D // 32, 1e-6, M, bf.cos.data_ptr(), bf.sin.data_ptr(), None, T_CROP, PAST, 128,
+                      stream())
+        return "qkv", M, 3 * D, K, True, f
+    if which == "clip.qkv":
+        M, N = B * 257, 3 * 1024
+        def f():
+            _lib.call("vsb_gemm_bf16", x.data_ptr(), K, w.data_ptr(), K, y.data_ptr(), N, M, N, K, bf.bias.data_ptr(), None, 0, 0, 0, 0, 0,
+                      0, stream())
+        return "clip.qkv", M, N, K, False, f
     if which == "o":
         def f():
             _lib.call("vsb_gemm_rowscale_bf16", y.data_ptr(), K, w.data_ptr(), K, x.data_ptr(), D, M, D, K, None, x.data_ptr(), D, 0, 0, 0,
@@ -227,7 +240,7 @@ def main():
         vit = [c for B in sorted({batches[0], batches[-1]}) for c in vit_calls(bf, f"clip.B{B}", B * 257, 1024, 4096)]
         for name, M, N, K, rope, fn in vit + vit_calls(bf, "owl.B8", 8 * 2305, 768, 3072):
             rows.append(row(bf, sms, name, M, N, K, rope, fn))
-        sweeps = [k_sweep(bf, sms, w, max(batches), ks) for w in ("o", "gu")]
+        sweeps = [k_sweep(bf, sms, w, max(batches), ks) for w in ("qkv", "o", "gu", "clip.qkv")]
     res = dict(gpu=info, lib=_lib.LIB_PATH, rows=rows, k_sweep=sweeps)
     for s in sweeps:
         print(f"K sweep {s['shape']}: intercept {s['intercept_ms']:.3f} ms ({s['intercept_us_per_wave']:.2f} us per wave of "

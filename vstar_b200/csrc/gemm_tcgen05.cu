@@ -2,9 +2,10 @@
 //
 // Hand-written sm_90a GEMM: TMA (cp.async.bulk.tensor, 128B swizzle) -> shared
 // memory ring (mbarrier full / empty pairs) -> wgmma.mma_async (bf16 or f16 ->
-// fp32 in registers) -> epilogue straight from the accumulator registers
+// fp32 in registers) -> epilogue from the accumulator registers
 // (bias / activation / SwiGLU / residual / row remap / folded RMSNorm / RoPE) ->
-// global.  Persistent: one CTA per SM loops over 128 x BN output tiles; the
+// per-warp shared-memory slots -> global by bulk copies, one per row (T output
+// with 16-byte aligned rows; fp32 output and BN = 32 store directly).  Persistent: one CTA per SM loops over 128 x BN output tiles; the
 // producer keeps loading the next tile's k-blocks while the consumers run the
 // epilogue of the current one.
 //
@@ -41,6 +42,7 @@ struct GemmParams {
   int epilogue;        // VSB_EPI_*
   int out_fp32;        // C (and residual) element type: 0 T (bf16 / f16), 1 fp32
   int vec2;            // C (and residual) rows allow 2-element vector access at even columns
+  int staged;          // T output written through shared memory with bulk copies (16-byte aligned rows, see gemm_dispatch)
   int rows_per_group;  // output row remap: r = (m / rpg) * group_stride + group_offset + m % rpg
   long long group_stride, group_offset;
   int tiles_m, tiles_n;
@@ -113,6 +115,20 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
 }
 
+// bulk (non-tensor) shared -> global copies of the staged epilogue: `bytes` and both addresses multiples of 16
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void bulk_store(void* gdst, const void* ssrc, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(ssrc)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void sts_u16(uint32_t saddr, uint16_t v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(saddr), "h"(v) : "memory"); }
+__device__ __forceinline__ void sts_u32(uint32_t saddr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory"); }
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every bulk group of this thread but the newest N has finished reading its shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// every bulk group of this thread has completed (its global writes included)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
 // K-major, 128B-swizzled shared-memory operand descriptor (cute::GMMA::GmmaDescriptor):
 //   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (8 rows * 128 B = 1024)
 //   [62,64) layout = 1 (SWIZZLE_128B)
@@ -128,6 +144,13 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
 constexpr int RSTD_THREADS = 96;    // warps 1-3 of the producer warpgroup: folded-RMSNorm row scales (tile_rstd)
 constexpr int RSTD_PIECE = 16;      // rowsq_in chunks staged per round trip
 
+// Staged epilogue output: each consumer warp owns two slots of its 16 rows x one 32-column chunk (T), rows OUT_PITCH bytes
+// apart.  80 B = 20 banks: the 4-byte fragment writes of one instruction (8 rows x 4 lanes, banks 20r + 4jj + t mod 32) are
+// conflict-free, and every row starts 16-byte aligned for its bulk copy.
+constexpr int OUT_PITCH = 80;
+constexpr int OUT_SLOT = 16 * OUT_PITCH;
+constexpr int SMEM_OPTIN_MAX = 232448;   // H100 opt-in dynamic shared memory per block
+
 template <int BN>
 struct SmemLayout {
   static constexpr int A_BYTES = BM * BK * 2;
@@ -137,8 +160,12 @@ struct SmemLayout {
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
   static constexpr int RSTD_OFFSET = BAR_OFFSET + 256;   // float [2][BM]: folded-RMSNorm row scales, two tiles in flight
   static constexpr int PART_OFFSET = RSTD_OFFSET + 2 * BM * 4;   // float [RSTD_PIECE][BM]: staged partial sums (tile_rstd)
-  static constexpr int TOTAL = PART_OFFSET + RSTD_PIECE * BM * 4 + 1024;  // + alignment slack
+  static constexpr int OUT_OFFSET = PART_OFFSET + RSTD_PIECE * BM * 4;   // [8 consumer warps][2][OUT_SLOT]: staged output
+  // BN = 32 (batched decode, HBM-bound on W) has no room for the staging slots beside its 10 stages: it stores directly
+  static constexpr bool STAGED = BN != 32;
+  static constexpr int TOTAL = OUT_OFFSET + (STAGED ? 8 * 2 * OUT_SLOT : 0) + 1024;  // + alignment slack
   static_assert((2 * STAGES + 4) * 8 <= 256, "barriers overflow their 256-byte slot");
+  static_assert(TOTAL <= SMEM_OPTIN_MAX, "shared memory over the per-block limit");
 };
 
 __device__ __forceinline__ float apply_act(float x, int epi) {
@@ -244,9 +271,11 @@ __device__ __forceinline__ PairIn load_pair(const GemmParams<T>& p, long long or
 
 // row orow (already remapped), columns n, n+1 (n even, n < N): bias -> activation / SwiGLU -> (+residual) -> T / fp32 store,
 // with bias and residual from load_pair.  Returns the sum of squares of the T values stored (the folded-RMSNorm row statistics).
-template <typename T>
+// STAGED: the T values go to the shared-memory staging slot at shared address s (output column n, or n/2 for SwiGLU) instead
+// of C; there N % 8 == 0, so n + 1 < N.
+template <bool STAGED, typename T>
 __device__ __forceinline__ float epilogue_pair(const GemmParams<T>& p, long long orow, int n, float x0, float x1, bool swiglu,
-                                               const PairIn& in) {
+                                               const PairIn& in, uint32_t s) {
   using E = ElemT<T>;
   const bool has1 = n + 1 < p.N;
   if (p.bias != nullptr) {
@@ -255,7 +284,9 @@ __device__ __forceinline__ float epilogue_pair(const GemmParams<T>& p, long long
   }
   if (swiglu) {
     // interleaved weight rows: even column = gate_j, odd column = up_j -> out column n/2 (N is even)
-    reinterpret_cast<T*>(p.C)[orow * p.ldc + (n >> 1)] = E::from_f(silu_f(x0) * x1);
+    const T v = E::from_f(silu_f(x0) * x1);
+    if constexpr (STAGED) sts_u16(s, *reinterpret_cast<const uint16_t*>(&v));
+    else reinterpret_cast<T*>(p.C)[orow * p.ldc + (n >> 1)] = v;
     return 0.f;
   }
   x0 = apply_act(x0, p.epilogue);
@@ -263,6 +294,11 @@ __device__ __forceinline__ float epilogue_pair(const GemmParams<T>& p, long long
   if (p.residual != nullptr) {
     x0 += in.r0;
     if (has1) x1 += in.r1;
+  }
+  if constexpr (STAGED) {
+    sts_u32(s, E::pack2(x0, x1));
+    const float s0 = E::round(x0), s1 = E::round(x1);
+    return fmaf(s1, s1, s0 * s0);
   }
   if (p.out_fp32) {
     float* c = reinterpret_cast<float*>(p.C) + orow * p.ldc + n;
@@ -332,15 +368,26 @@ __device__ __forceinline__ void load_chunk(const GemmParams<T>& p, const bool* o
 }
 
 // Epilogue of one consumer thread: rows m[0], m[1] of the tile, fragment columns 8j + 2t (see wgmma.cuh); rs = their
-// folded-RMSNorm scales (1 without a folded norm)
-template <int BN, bool ROPE, typename T>
-__device__ __forceinline__ void epilogue_tile(const GemmParams<T>& p, float* acc, int m0, int n_blk, int t, float rs0, float rs1) {
+// folded-RMSNorm scales (1 without a folded norm).
+// STAGED: each 32-column chunk of the warp's 16 rows is written into one of the warp's two shared-memory slots (`stage`, slot
+// `oslot & 1`, oslot counting the warp's slot fills across tiles) and leaves as one bulk copy per row, issued by lanes 0-15.
+// SwiGLU halves the columns, so a slot takes the 16 output columns of two consecutive chunks and is copied after the second
+// (64-byte rows, half as many copies).  The warp waits only until the copies of the fill before last have read their slot,
+// never for a global write.  SW: the staged SwiGLU epilogue (a template parameter so the other epilogues keep a branch-free
+// chunk loop).  In-place residual
+// (C == residual) stays safe: every element's residual load completes before its value is written to the slot (the value depends
+// on it), so before the bulk copy that writes the same bytes is issued, and chunk c + 1's loads touch no column of chunk c.  Tiles
+// (and remapped rows) are disjoint, so no other thread reads what a copy writes.
+template <int BN, bool ROPE, bool STAGED, bool SW, typename T>
+__device__ __forceinline__ void epilogue_tile(const GemmParams<T>& p, float* acc, int m0, int n_blk, int t, float rs0, float rs1,
+                                              uint8_t* stage, int& oslot) {
   static_assert(BN % 32 == 0, "the epilogue works in whole 32-column chunks");
+  const int lane = threadIdx.x & 31;
   const int m[2] = {m0, m0 + 8};
   float rs[2] = {rs0, rs1};
   const bool ok[2] = {m[0] < p.M, m[1] < p.M};
   const long long orow[2] = {ok[0] ? remap_row(p, m[0]) : 0, ok[1] ? remap_row(p, m[1]) : 0};
-  const bool swiglu = (p.epilogue == VSB_EPI_SWIGLU);
+  const bool swiglu = STAGED ? SW : (p.epilogue == VSB_EPI_SWIGLU);
   const int n_tile0 = n_blk * BN;
   if constexpr (ROPE) {
     if (n_tile0 < p.rope_cols) {
@@ -357,15 +404,37 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams<T>& p, float* acc
     const int n0 = n_tile0 + 32 * c;
     if (n0 >= p.N) break;                          // warp-uniform
     if (has_in && c + 1 < BN / 32 && n0 + 32 < p.N) load_chunk<T>(p, ok, orow, n0 + 32, t, in[(c + 1) & 1]);
+    uint8_t* slot = stage + (oslot & 1) * OUT_SLOT;    // the warp's staging slot for this chunk
+    const int half = SW ? (c & 1) : 0;             // SwiGLU: second chunk of the slot's two
+    if (STAGED && half == 0) {
+      bulk_wait_read<1>();                         // the copies that last read this slot (fill before last) are done with it
+      __syncwarp();
+    }
     float sq[2] = {0.f, 0.f};
 #pragma unroll
     for (int jj = 0; jj < 4; ++jj) {
       const int j = 4 * c + jj;
       const int n = n0 + 8 * jj + 2 * t;
+      const int sc = swiglu ? 16 * half + 4 * jj + t : 8 * jj + 2 * t;   // column in the slot
 #pragma unroll
       for (int h = 0; h < 2; ++h)
         if (ok[h] && n < p.N)
-          sq[h] += epilogue_pair<T>(p, orow[h], n, acc[4 * j + 2 * h] * rs[h], acc[4 * j + 2 * h + 1] * rs[h], swiglu, in[c & 1][jj][h]);
+          sq[h] += epilogue_pair<STAGED, T>(p, orow[h], n, acc[4 * j + 2 * h] * rs[h], acc[4 * j + 2 * h + 1] * rs[h], swiglu,
+                                            in[c & 1][jj][h], smem_u32(slot) + (8 * h + (lane >> 2)) * OUT_PITCH + sc * (int)sizeof(T));
+    }
+    if (STAGED && (!SW || half == 1 || n0 + 32 >= p.N)) {
+      fence_proxy_async_smem();                    // this thread's slot writes -> visible to the bulk copies
+      __syncwarp();
+      const int mr = m0 - (lane >> 2) + lane;      // lane < 16: tile row of slot row `lane`
+      if (lane < 16 && mr < p.M) {
+        const int nb = n0 - 32 * half;             // first input column of the slot
+        // bytes: 2 per output column; the output width is a multiple of 8 on this path
+        const int bytes = swiglu ? min(64, p.N - nb) : 2 * min(32, p.N - nb);
+        T* dst = reinterpret_cast<T*>(p.C) + remap_row(p, mr) * p.ldc + (swiglu ? nb >> 1 : nb);
+        bulk_store(dst, slot + lane * OUT_PITCH, bytes);
+      }
+      bulk_commit();
+      ++oslot;
     }
     if (p.rowsq_out != nullptr) {                  // N % 32 == 0: every chunk is complete
 #pragma unroll
@@ -461,6 +530,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int cw = wg - 1;                        // rows [64 cw, 64 cw + 64) of the tile
   const int wq = (threadIdx.x >> 5) & 3;        // warp inside the warpgroup: 16 rows each
   float acc[BN / 2];
+  uint8_t* ostage = smem + L::OUT_OFFSET + (threadIdx.x / 32 - 4) * (2 * OUT_SLOT);   // this warp's two output slots
+  int oslot = 0;
   int stage = 0;
   uint32_t phase = 0;
   int it = 0;
@@ -498,8 +569,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       rs1 = rstd_s[slot * BM + r + 8];
       mbar_arrive(&rstd_empty[slot]);
     }
-    epilogue_tile<BN, ROPE, T>(p, acc, m_blk * BM + r, n_blk, lane & 3, rs0, rs1);
+    if (L::STAGED && p.staged && !ROPE && p.epilogue == VSB_EPI_SWIGLU)
+      epilogue_tile<BN, ROPE, L::STAGED, !ROPE, T>(p, acc, m_blk * BM + r, n_blk, lane & 3, rs0, rs1, ostage, oslot);
+    else if (L::STAGED && p.staged)
+      epilogue_tile<BN, ROPE, L::STAGED, false, T>(p, acc, m_blk * BM + r, n_blk, lane & 3, rs0, rs1, ostage, oslot);
+    else
+      epilogue_tile<BN, ROPE, false, false, T>(p, acc, m_blk * BM + r, n_blk, lane & 3, rs0, rs1, ostage, oslot);
   }
+  bulk_wait_all();   // the staging slots must outlive the copies that read them
 }
 
 // ---------------------------------------------------------------- host side
@@ -896,6 +973,12 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
   p.vec2 = (ldc % 2 == 0) && (reinterpret_cast<uintptr_t>(C) % (2 * esz) == 0) &&
            (residual == nullptr || ((ldr % 2 == 0) && (reinterpret_cast<uintptr_t>(residual) % (2 * esz) == 0)));
   if (p.rope_cos != nullptr) bn = 256;        // the fused-RoPE epilogue pairs columns inside one 128-wide head: 256-wide tiles only
+  // staged epilogue (T output through shared memory, one bulk copy per row and 32-column chunk): needs 16-byte aligned rows and
+  // chunks.  fp32 output (its rows would need twice the staging), the BN = 32 tiles (no room beside their stages) and the
+  // streaming-store switch (.cs stores, vsb_gemm_set_l2_hints bit 2) store straight from the registers.
+  const int out_cols = epilogue == VSB_EPI_SWIGLU ? N / 2 : N;
+  p.staged = !out_fp32 && bn != 32 && !p.stream_out && (ldc * esz) % 16 == 0 && reinterpret_cast<uintptr_t>(C) % 16 == 0 &&
+             out_cols % 8 == 0;
   r = make_tensor_map(&tmB, W, N, K, ldw, bn, ElemT<T>::tma);
   if (r) return r;
   if (bn == 256)
