@@ -27,6 +27,9 @@ extern "C" {
 #define VSB_EPI_RELU 3       /* SAM transformer MLP, text_hidden_fcs, hyper-network MLPs */
 #define VSB_EPI_SWIGLU 4     /* silu(gate)*up with gate/up rows interleaved in W (Llama MLP) */
 
+#define VSB_DTYPE_BF16 0 /* logit_dtype of vsb_sample_rows_f32: the engine dtype the logits are rounded to */
+#define VSB_DTYPE_F16 1
+
 #define VSB_HEATMAP_MAX_BLOCKS 1184 /* blocks of the heat-map reduction (fixed: its summation order does not depend on the GPU) */
 
 const char* vsb_last_error(void);
@@ -137,6 +140,16 @@ int vsb_cast_f32_bf16(const void* x, void* y, long long n, void* stream);
 /* f16 twin of vsb_cast_f32_bf16 (the reference's .half() of fp32 pixels) */
 int vsb_cast_f32_f16(const void* x, void* y, long long n, void* stream);
 int vsb_argmax_rows_f32(const void* x, long long ld, int rows, int n, void* idx_i32, void* val_f32, void* stream);
+/* Sampled next token of every row of fp32 logits [rows, n] (HF `sample()` with TemperatureLogitsWarper, TopKLogitsWarper,
+ * TopPLogitsWarper and multinomial(softmax), as transformers 4.31 runs them for free_form_inference(temperature > 0)).  Per row:
+ * v = dtype(float(dtype(x)) / temperature) with dtype = logit_dtype (VSB_DTYPE_BF16 / VSB_DTYPE_F16: the reference's logits
+ * are the lm_head output in the model dtype); top_k > 0 keeps every v >= the k-th largest (ties kept), 0 disables it;
+ * top_p < 1 keeps, in descending order, each position whose probability mass at or after it exceeds 1 - top_p (the largest
+ * always kept), 1 disables it; probabilities in fp64 from exp(v - max).  The token is drawn by inverse CDF over the kept tokens
+ * (descending v, ties by ascending id) at u = Philox4x32-10(key = seeds_i64[row], counter = (step, 0, 0, 0)), 53 bits, so it
+ * depends only on the row's logits, its seed and step.  seeds_i64: device int64 [rows]; idx_i32: device int32 [rows]. */
+int vsb_sample_rows_f32(const void* logits, long long ld, int rows, int n, float temperature, int top_k, float top_p, int logit_dtype,
+                        const void* seeds_i64, int step, void* idx_i32, void* stream);
 /* per-row negative log-likelihood of labels under softmax(logits) — option scoring of the SEAL VQA LLM
  * (CrossEntropyLoss, /root/reference/vstar_bench_eval.py:154-159) */
 int vsb_nll_rows_f32(const void* logits, long long ld, int rows, int n, const void* labels_i64, void* out_f32, void* stream);

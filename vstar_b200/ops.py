@@ -471,6 +471,23 @@ def argmax_rows(x):
     return idx, val
 
 
+def sample_rows(x, temperature, top_k, top_p, dtype, seeds, step):
+    """one sampled token per row of fp32 logits x [rows, n] (vsb_sample_rows_f32): the logits rounded to `dtype` (bf16 / fp16)
+    and divided by `temperature` (> 0), top_k (0 = off, ties at the k-th value kept), top_p (None or 1 = off), then an
+    inverse-CDF draw keyed by seeds (int64 [rows] on the device) and `step` -> idx int32 [rows]"""
+    _chk(x, torch.float32)
+    p, rows, n, ld = _rows2d(x)
+    _chk(seeds, torch.int64)
+    assert seeds.numel() == rows and seeds.is_contiguous()
+    if dtype not in _SUFFIX:
+        raise _lib.VsbError(f"unsupported dtype {dtype}: the logits are rounded to bf16 or fp16")
+    idx = torch.empty((rows,), dtype=torch.int32, device=x.device)
+    _lib.launches += 1
+    call("vsb_sample_rows_f32", p, ld, rows, n, float(temperature), int(top_k), 1.0 if top_p is None else float(top_p),
+         1 if dtype == F16 else 0, seeds.data_ptr(), int(step), idx.data_ptr(), _stream())
+    return idx
+
+
 def nll_rows(logits, labels):
     """logits fp32 [rows, V], labels int64 [rows] -> nll fp32 [rows]"""
     _chk(logits, torch.float32)

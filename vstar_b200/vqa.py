@@ -14,6 +14,8 @@ accumulation; tolerance stated in tests/test_vqa_gpu.py) or, opt-in, in fp16 lik
 same kernels: VQAWeights(..., dtype=torch.float16), load_pretrained_model(..., torch_dtype=torch.float16) or
 VQA_LLM(args) with args.vqa_dtype = "fp16".  fp16 brings the option NLLs and logits close to the reference's own
 numbers (tests/test_vqa_fp16_gpu.py; DESIGN.md §7b).  The VSM stays bf16, as in the reference.
+free_form_inference(temperature > 0, top_p) samples like the reference's `generate(do_sample=True)`: one vsb_sample_rows_f32
+launch per decode step in place of the greedy argmax (oracle/sampling_oracle.py; DESIGN.md §7b).
 """
 from __future__ import annotations
 
@@ -31,6 +33,8 @@ IMAGE_TOKEN_INDEX = -200
 OBJECT_TOKEN_INDEX = -300
 DEFAULT_IMAGE_TOKEN = "<image>"
 DEFAULT_OBJECT_TOKEN = "<object>"
+
+DEFAULT_TOP_K = 50        # transformers 4.31 GenerationConfig.top_k, used unless the checkpoint's generation_config.json sets it
 
 VICUNA_V1_SYSTEM = ("A chat between a curious user and an artificial intelligence assistant. "
                     "The assistant gives helpful, detailed, and polite answers to the user's questions.")
@@ -65,6 +69,38 @@ def tokenizer_image_object_token(prompt, tokenizer, image_token_index=IMAGE_TOKE
     for x in insert_separator(prompt_chunks, sep):
         input_ids.extend(x[offset:])
     return input_ids
+
+
+def check_sampling(top_k, top_p):
+    """the arguments the reference's warpers validate (TopKLogitsWarper / TopPLogitsWarper) -> (top_k, top_p) for the sampler:
+    top_k None or 0 = no top-k filter, top_p None = no nucleus filter"""
+    top_k = 0 if top_k is None else top_k
+    if isinstance(top_k, bool) or not isinstance(top_k, int) or top_k < 0:
+        raise ValueError(f"`top_k` has to be a non-negative integer, but is {top_k!r}")
+    if top_p is not None:
+        top_p = float(top_p)
+        if not (0.0 <= top_p <= 1.0):
+            raise ValueError(f"`top_p` has to be a float >= 0 and <= 1, but is {top_p}")
+    return top_k, top_p
+
+
+def draw_seeds(n):
+    """n sampler seeds from torch's default generator, one int64 draw per request in request order (where HF's `sample()`
+    takes its randomness for torch.multinomial), so torch.manual_seed(s) reproduces a sampled call"""
+    return torch.empty(n, dtype=torch.int64).random_().tolist()
+
+
+def generation_top_k(model_path):
+    """top_k of the checkpoint's generation_config.json, else the transformers 4.31 default (50)"""
+    import json
+    import os
+    path = os.path.join(str(model_path), "generation_config.json")
+    if os.path.isfile(path):
+        with open(path) as f:
+            k = json.load(f).get("top_k")
+        if k is not None:
+            return int(k)
+    return DEFAULT_TOP_K
 
 
 class VQAWeights(CoreWeights):
@@ -195,18 +231,32 @@ class VQAEngine(LlamaClipCore):
         hn, am, logits = self._logits_rows(x, rows)
         return logits
 
+    def _sampler(self, temperature, top_k, top_p, seeds):
+        """None for greedy decoding (temperature None or <= 0); else fn(logits [B, V], step) -> int32 [B] tokens drawn by
+        vsb_sample_rows_f32 with one seed per row (uploaded once per call; None: one default-generator draw for a single row)"""
+        if temperature is None or not temperature > 0:
+            return None
+        top_k, top_p = check_sampling(top_k, top_p)
+        seeds = draw_seeds(1) if seeds is None else seeds
+        sd = torch.tensor([(int(s) + (1 << 63)) % (1 << 64) - (1 << 63) for s in seeds], dtype=torch.int64, device=self.dev)   # any 64 bits
+        T, dtype = float(temperature), self.dtype
+        return lambda logits, step: ops.sample_rows(logits, T, top_k, top_p, dtype, sd, step)
+
     def generate(self, input_ids, image, object_crops=None, images_long=None, objects_long=None, max_new_tokens=200, eos_token_id=2,
-                 stop_ids=None, stop_fn=None):
+                 stop_ids=None, stop_fn=None, temperature=0, top_k=DEFAULT_TOP_K, top_p=None, seed=None):
         """greedy `model.generate(use_cache=True, do_sample=False)` (vstar_bench_eval.py:91-103) -> list of new token ids.
-        stop_ids: stop once the output ends with these ids; stop_fn(new_ids) -> bool: HF-style stopping criterion."""
+        stop_ids: stop once the output ends with these ids; stop_fn(new_ids) -> bool: HF-style stopping criterion.
+        temperature > 0: sampled decoding instead (`do_sample=True` with top_k / top_p, ops.sample_rows); token t is drawn with
+        (seed, step t), seed None = one draw from torch's default generator."""
+        sampler = self._sampler(temperature, top_k, top_p, None if seed is None else [seed])
         x = self.build_embeds(input_ids, image, object_crops, images_long, objects_long)
         T = x.shape[0]
         self.prefill_embeds(x, reserve=max(0, min(max_new_tokens, self.MAX_POSITIONS - T)))
         logits = self.last_logits(x)
         out = []
         past = T
-        for _ in range(max_new_tokens):
-            nxt = int(ops.argmax_rows(logits)[0][0])
+        for step in range(max_new_tokens):
+            nxt = int(ops.argmax_rows(logits)[0][0] if sampler is None else sampler(logits, step)[0])
             out.append(nxt)
             if nxt == eos_token_id or (stop_ids and out[-len(stop_ids):] == list(stop_ids)) or \
                     (stop_fn is not None and stop_fn(out)):
@@ -256,20 +306,25 @@ class VQAEngine(LlamaClipCore):
         hn = ops.rmsnorm(x, self.w.final_norm, self.cfg.rms_eps)
         return ops.gemm(hn, self.w.lm_head, out_dtype=torch.float32)
 
-    def generate_batch(self, requests, max_new_tokens=200, eos_token_id=2, stop_ids=None):
+    def generate_batch(self, requests, max_new_tokens=200, eos_token_id=2, stop_ids=None, temperature=0, top_k=DEFAULT_TOP_K, top_p=None,
+                       seeds=None):
         """greedy generation for several (input_ids, image, object_crops, images_long, objects_long) requests at once.
         Same per-sequence semantics as generate(); finished sequences idle (their slots keep stepping, results ignored).
-        -> list of new-token lists"""
+        temperature > 0: sampled decoding as in generate(), request i with seeds[i] (None = one default-generator draw per
+        request, in request order).  -> list of new-token lists"""
+        if temperature is not None and temperature > 0 and seeds is None:
+            seeds = draw_seeds(len(requests))
         xs = self.build_embeds_batch(list(requests))           # one CLIP + projector pass for every image of the batch
         perm = sorted(range(len(xs)), key=lambda i: int(xs[i].shape[0]))       # equal lengths next to each other (stable)
         xs = [xs[i] for i in perm]
+        sampler = self._sampler(temperature, top_k, top_p, None if seeds is None else [seeds[i] for i in perm])
         longest = max(int(x.shape[0]) for x in xs)
         logits, Tpad, lens = self.prefill_ragged(xs, reserve=max(0, min(max_new_tokens, self.MAX_POSITIONS - longest)))
         B = len(xs)
         outs = [[] for _ in range(B)]
         done = [False] * B
         for step in range(max_new_tokens):
-            nxt = ops.argmax_rows(logits)[0].tolist()              # one D2H per step for the whole batch
+            nxt = (ops.argmax_rows(logits)[0] if sampler is None else sampler(logits, step)).tolist()   # one D2H per step
             for b in range(B):
                 if done[b]:
                     continue
@@ -422,6 +477,7 @@ class LlavaSearchModel:
         self.config.vocab_size = engine.cfg.vocab
         self.eos_token_id = eos_token_id
         self.device = torch.device(engine.dev)
+        self.top_k = DEFAULT_TOP_K                      # the top_k VQA_LLM samples with (generation_config.json's, if any)
 
     def eval(self):
         return self
@@ -489,7 +545,9 @@ def load_pretrained_model(model_path, model_base=None, model_name=None, load_8bi
     dtype = torch.float16 if load_4bit else (BF if torch_dtype is None else torch_dtype)
     engine = VQAEngine(VQAWeights(cfg, open_checkpoint(model_path, device=device), device=device, dtype=dtype,
                                   quant="nf4" if load_4bit else None))
-    return tokenizer, LlavaSearchModel(engine, getattr(tokenizer, "eos_token_id", 2)), _Proc(), 2048
+    model = LlavaSearchModel(engine, getattr(tokenizer, "eos_token_id", 2))
+    model.top_k = generation_top_k(model_path)
+    return tokenizer, model, _Proc(), 2048
 
 
 class VQA_LLM:
@@ -505,6 +563,7 @@ class VQA_LLM:
             self.tokenizer, self.model, self.image_processor, self.context_len = load_pretrained_model(
                 args.vqa_model_path, None, None, load_4bit=load_4bit, torch_dtype=None if load_4bit else VQA_DTYPES[name])
             self.engine = self.model.engine
+            self.top_k = self.model.top_k
             self.conv_type = getattr(args, "conv_type", "v1")
             self.eos = getattr(self.tokenizer, "eos_token_id", 2)
             return
@@ -513,6 +572,7 @@ class VQA_LLM:
         self.tokenizer = tokenizer if tokenizer is not None else SyntheticTokenizer(engine.cfg)
         self.image_processor = _Proc()
         self.context_len = 2048
+        self.top_k = DEFAULT_TOP_K
         self.conv_type = conv_type
         self.eos = getattr(self.tokenizer, "eos_token_id", 2)
 
@@ -594,8 +654,11 @@ class VQA_LLM:
     @torch.inference_mode()
     def free_form_inference(self, image, question, temperature=0, top_p=None, num_beams=1, max_new_tokens=200, object_crops=None,
                             images_long=None, objects_long=None):
-        if temperature and temperature > 0:
-            raise NotImplementedError("sampling is not on the V*Bench path (temperature=0, vstar_bench_eval.py:196)")
+        """temperature > 0 samples (the reference's do_sample = temperature > 0, vstar_bench_eval.py:97) with top_k = self.top_k
+        and top_p; the request takes one seed from torch's default generator"""
+        sample = temperature is not None and temperature > 0
+        if sample:
+            check_sampling(self.top_k, top_p)
         prompt = build_prompt_v1(DEFAULT_IMAGE_TOKEN + "\n" + question)
         stop_str = "</s>"
         ids = tokenizer_image_object_token(prompt, self.tokenizer)
@@ -603,18 +666,24 @@ class VQA_LLM:
         if len(kw) > 1 and kw[0] == self.tokenizer.bos_token_id:
             kw = kw[1:]
         img, crops = self._pixels(image, object_crops)
-        out = self.engine.generate(ids, img, crops, images_long, objects_long, max_new_tokens, self.eos, stop_ids=kw)
+        out = self.engine.generate(ids, img, crops, images_long, objects_long, max_new_tokens, self.eos, stop_ids=kw,
+                                   temperature=temperature if sample else 0, top_k=self.top_k, top_p=top_p,
+                                   seed=draw_seeds(1)[0] if sample else None)
         text = self.tokenizer.batch_decode([out], skip_special_tokens=True)[0].strip()
         if text.endswith(stop_str):
             text = text[:-len(stop_str)]
         return text.strip()
 
     @torch.inference_mode()
-    def free_form_inference_batch(self, images, questions, max_new_tokens=200, originals=None):
+    def free_form_inference_batch(self, images, questions, max_new_tokens=200, originals=None, temperature=0, top_p=None):
         """free_form_inference for several (image, question) pairs in ONE continuous-batched decode (not in the reference,
         which answers one image at a time, vstar_bench_eval.py:196): same prompt, stop string and post-processing per
         sample; each decode step reads the 7B weights once for the whole batch.  originals: the un-padded images the padded
-        `images` were made from; with `use_device_images` the pixels are then produced on the GPU (bit-identical)."""
+        `images` were made from; with `use_device_images` the pixels are then produced on the GPU (bit-identical).
+        temperature / top_p as in free_form_inference; each request takes one seed from torch's default generator, in order."""
+        sample = temperature is not None and temperature > 0
+        if sample:
+            check_sampling(self.top_k, top_p)
         stop_str = "</s>"
         kw = self.tokenizer(stop_str).input_ids
         if len(kw) > 1 and kw[0] == self.tokenizer.bos_token_id:
@@ -627,7 +696,8 @@ class VQA_LLM:
             else:
                 img, _ = self._pixels(image, None)
             reqs.append((ids, img, None, None, None))
-        outs = self.engine.generate_batch(reqs, max_new_tokens, self.eos, stop_ids=kw)
+        outs = self.engine.generate_batch(reqs, max_new_tokens, self.eos, stop_ids=kw, temperature=temperature if sample else 0,
+                                          top_k=self.top_k, top_p=top_p, seeds=draw_seeds(len(reqs)) if sample else None)
         texts = []
         for out in outs:
             text = self.tokenizer.batch_decode([out], skip_special_tokens=True)[0].strip()
