@@ -168,7 +168,11 @@ int vsb_copy2d_b16(const void* src, long long lds, void* dst, long long ldd, lon
  * prefix keys [0, seg_lo) and its own continuation from key q_seg[r] on (vsb_flash_attn_seg_bf16).  norm_folded != 0: the caller
  * has multiplied ln1 into wqkv's columns and ln2 into wgu's (ln1 / ln2 then hold ones): the QKV and gate|up GEMMs take the
  * un-normalised residual stream and apply 1/rms in their epilogue, fed by the row statistics the o-proj / down-proj GEMMs leave
- * (vsb_gemm_rowscale_bf16) - 6 kernel launches per layer instead of 8. */
+ * (vsb_gemm_rowscale_bf16) - 6 kernel launches per layer instead of 8.
+ * Weight format: the w*_scales fields are NULL for dense weights.  Set, they make the matching w* field hold NF4 codes and
+ * themselves the codes' fp32 block scales (layout below), and that projection runs on vsb_gemm_nf4; a table is all dense or
+ * all NF4.  NF4 tables need vsb_llama_layers_f16, norm_folded = 0 and tail_rows = 0, and deq_scratch: f16, 2*inter*d elements
+ * (the largest weight), which the row counts that take the dequant + tile path use; dense tables leave it unused (NULL). */
 typedef struct {
   const void* ln1;
   const void* wqkv;
@@ -176,14 +180,20 @@ typedef struct {
   const void* ln2;
   const void* wgu;
   const void* wdown;
+  const void* wqkv_scales;
+  const void* wo_scales;
+  const void* wgu_scales;
+  const void* wdown_scales;
 } vsb_llama_layer_t;
 int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc, int Tmax,
                      int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin, const void* positions,
-                     const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded, void* scratch, void* stream);
+                     const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded, void* scratch,
+                     void* deq_scratch, void* stream);
 /* f16 twin of vsb_llama_layers: f16 weights, residual stream, cache, RoPE tables and scratch, dispatching to the _f16 kernels */
 int vsb_llama_layers_f16(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc, int Tmax,
                          int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin, const void* positions,
-                         const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded, void* scratch, void* stream);
+                         const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded, void* scratch,
+                         void* deq_scratch, void* stream);
 
 /* NF4 weights: the SEAL VQA LLM's 4-bit mode (the reference's load_4bit: bitsandbytes NF4, double-quantised scales, fp16 compute,
  * LLaVA/llava/model/builder.py:26-43).  Format of W [N, K], K % 64 == 0 (csrc/nf4.cu, oracle/nf4_oracle.py): codes u8 [N, K/2], two
@@ -202,25 +212,6 @@ int vsb_nf4_dequant(const void* codes, const void* scales, int N, int K, void* o
 int vsb_gemm_nf4(const void* A, long long lda, const void* codes, const void* scales, void* C, long long ldc, int M, int N, int K,
                      const void* bias, const void* residual, long long ldr, int epilogue, int out_fp32, int rows_per_group,
                      long long group_stride, long long group_offset, void* deq_scratch, void* stream);
-/* vsb_llama_layers_f16 on NF4 projections: ln1 / ln2 f16 [d] (not folded), codes and scales of wqkv, wo, wgu, wdown in the layouts
- * of vsb_llama_layer_t.  RMSNorm kernel then GEMM (norm_folded = 0 only); tail_rows must be 0.  deq_scratch: f16, 2*inter*d
- * elements (the largest weight), used by the row counts that take the dequant + tile path. */
-typedef struct {
-  const void* ln1;
-  const void* wqkv_codes;
-  const void* wqkv_scales;
-  const void* wo_codes;
-  const void* wo_scales;
-  const void* ln2;
-  const void* wgu_codes;
-  const void* wgu_scales;
-  const void* wdown_codes;
-  const void* wdown_scales;
-} vsb_llama_layer_nf4_t;
-int vsb_llama_layers_nf4(const vsb_llama_layer_nf4_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
-                             int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
-                             const void* positions, const void* k_start, const void* q_seg, int seg_lo, void* scratch, void* deq_scratch,
-                             void* stream);
 
 /* softmax(QK^T*scale [+causal]) V, head_dim 64/128; element (b,s,h,d) at base + b*bs + s*rs + h*D + d.
  * HF CLIP/OWL attention (modeling_clip.py:261-329) and Llama attention (modeling_llama.py:199-221). */

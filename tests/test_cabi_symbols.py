@@ -73,3 +73,16 @@ def test_ctypes_table_matches_the_header_prototypes():
         c_ints = [("long long" in " ".join(p.split())) for p in protos[name].split(",") if kind_c(p) == "i"]
         py_ints = [t is ctypes.c_longlong for t in argtypes if kind_py(t) == "i"]
         assert c_ints == py_ints, (name, c_ints, py_ints)
+
+
+def test_layer_struct_matches_the_header():
+    """member names of vsb_llama_layer_t in include/vstar_b200.h, in order, against the ctypes struct the layer table is built
+    from - the runner reads the table by field offset"""
+    from vstar_b200 import _lib
+    src = open(os.path.join(ROOT, "include", "vstar_b200.h")).read()
+    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+    body = re.search(r"typedef struct \{([^}]*)\} vsb_llama_layer_t;", src).group(1)
+    members = re.findall(r"const void\* (\w+);", body)
+    assert len(members) == len(body.split(";")) - 1, body
+    assert members == [name for name, _ in _lib.LlamaLayer._fields_]
+    assert all(t is ctypes.c_void_p for _, t in _lib.LlamaLayer._fields_)

@@ -4,7 +4,7 @@
     oracle's dequantisation (random tensors at Llama-7B shapes and edge blocks);
 (2) GEMM: vsb_gemm_nf4 against fp32 x @ deq(W)^T with every variant forced, every epilogue and the row remap; criterion
     err <= 2 * err(torch fp16 matmul on deq(W)) + ATOL; the dequant + tile path is bit-identical to vsb_gemm_f16 on deq(W);
-(3) the native NF4 layer runner == the same kernels sequenced from Python, bit for bit (prefill, ragged decode, option pass);
+(3) the native layer runner on an NF4 table == the same kernels sequenced from Python, bit for bit (prefill, ragged decode, option pass);
 (4) the NF4 engine against vqa_oracle in fp32 on the dequantised state dict (the reference's 4-bit math) on the goldens;
 (5) the rest of the VQA surface on the NF4 engine, and the memory footprint of the load."""
 import json
@@ -194,8 +194,9 @@ def _rope_tables(maxpos, D, theta=10000.0):
 
 @pytest.mark.parametrize("d,H,inter", [(256, 2, 512), (1024, 8, 2048)])
 def test_llama_layers_nf4_native_runner(ops, d, H, inter):
-    """vsb_llama_layers_nf4 == the same kernels from Python, bit for bit: prefill Tn = 70, a ragged decode step (k_start), an
-    option pass (q_seg); head_dim 128 takes the fused-RoPE QKV GEMM on the prefill"""
+    """vsb_llama_layers_f16 on an NF4 table == the same kernels from Python, bit for bit: prefill Tn = 70, a ragged decode step
+    (k_start), an option pass (q_seg); head_dim 128 takes the fused-RoPE QKV GEMM on the prefill.  The bf16 entry point and a
+    table that mixes NF4 and dense projections are refused."""
     nl, B, Tmax = 2, 2, 128
     hd = d // H
     layers = [dict(ln1=(1 + 0.1 * torch.randn(d)).to(F16).cuda(), wqkv=ops.nf4_quantize(rnd(3 * d, d, scale=d ** -0.5, seed=70 + i)),
@@ -258,6 +259,19 @@ def test_llama_layers_nf4_native_runner(ops, d, H, inter):
     assert torch.isfinite(outs[0][0].float()).all() and float(outs[0][0].float().abs().max()) > 0
     with pytest.raises(Exception):
         ops.llama_layer_table([dict(layers[0]), dict(layers[1], wo=ops.nf4_dequant(layers[1]["wo"]))])
+
+    def raw_call(fn, tab):
+        x, cache = rnd(B, d, seed=113).clone(), torch.zeros(nl, B, Tmax, 3 * d, dtype=F16, device="cuda")
+        scratch = torch.empty(B * (2 * d + inter), dtype=F16, device="cuda")
+        ops.call(fn, tab, nl, x.data_ptr(), B, 1, 0, cache.data_ptr(), B, Tmax, d, H, inter, 1e-6, cos_t.data_ptr(), sin_t.data_ptr(),
+                 None, None, 0, None, 0, 0, scratch.data_ptr(), deq.data_ptr(), ops._stream())
+
+    with pytest.raises(ops._lib.VsbError):
+        raw_call("vsb_llama_layers", table)
+    mixed = (type(table[0]) * nl)(*table)
+    mixed[1].wo_scales = None
+    with pytest.raises(ops._lib.VsbError):
+        raw_call("vsb_llama_layers_f16", mixed)
 
 
 # ------------------------------------------------------------------------------------------------ (4) engine parity

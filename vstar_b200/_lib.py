@@ -37,7 +37,8 @@ SIGNATURES = {
     "vsb_argmax_rows_f32": [c_p, c_ll, c_i, c_i, c_p, c_p, c_p],
     "vsb_sample_rows_f32": [c_p, c_ll, c_i, c_i, c_f, c_i, c_f, c_i, c_p, c_i, c_p, c_p],
     "vsb_copy2d_b16": [c_p, c_ll, c_p, c_ll, c_ll, c_i, c_p],
-    "vsb_llama_layers": [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_i, c_p, c_i, c_i, c_p, c_p],
+    "vsb_llama_layers": [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_i, c_p, c_i, c_i, c_p, c_p,
+                         c_p],
     "vsb_gemm_rowscale_bf16": [c_p, c_ll, c_p, c_ll, c_p, c_ll, c_i, c_i, c_i, c_p, c_p, c_ll, c_i, c_i, c_ll, c_ll, c_p, c_i, c_f, c_p, c_ll, c_p],
     "vsb_rowsq_bf16": [c_p, c_ll, c_p, c_i, c_i, c_p],
     "vsb_gemm_qkv_rope_bf16": [c_p, c_ll, c_p, c_ll, c_p, c_ll, c_i, c_i, c_i, c_i, c_ll, c_ll, c_p, c_i, c_f, c_ll, c_p, c_p, c_p, c_i, c_i, c_i, c_p],
@@ -72,19 +73,13 @@ SIGNATURES.update({
     "vsb_nf4_double_quant": [c_p, c_ll, c_p, c_p, c_p, c_p],
     "vsb_nf4_dequant": [c_p, c_p, c_i, c_i, c_p, c_ll, c_p],
     "vsb_gemm_nf4": [c_p, c_ll, c_p, c_p, c_p, c_ll, c_i, c_i, c_i, c_p, c_p, c_ll, c_i, c_i, c_i, c_ll, c_ll, c_p, c_p],
-    "vsb_llama_layers_nf4": [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p],
 })
 
 
 class LlamaLayer(ctypes.Structure):
     """vsb_llama_layer_t"""
-    _fields_ = [("ln1", c_p), ("wqkv", c_p), ("wo", c_p), ("ln2", c_p), ("wgu", c_p), ("wdown", c_p)]
-
-
-class LlamaLayerNF4(ctypes.Structure):
-    """vsb_llama_layer_nf4_t"""
-    _fields_ = [("ln1", c_p), ("wqkv_codes", c_p), ("wqkv_scales", c_p), ("wo_codes", c_p), ("wo_scales", c_p), ("ln2", c_p),
-                ("wgu_codes", c_p), ("wgu_scales", c_p), ("wdown_codes", c_p), ("wdown_scales", c_p)]
+    _fields_ = [("ln1", c_p), ("wqkv", c_p), ("wo", c_p), ("ln2", c_p), ("wgu", c_p), ("wdown", c_p),
+                ("wqkv_scales", c_p), ("wo_scales", c_p), ("wgu_scales", c_p), ("wdown_scales", c_p)]
 
 
 _lib = None

@@ -58,17 +58,32 @@ struct LayerOps<half> {
   static constexpr auto attn_decode = vsb_attn_decode_f16;
 };
 
+int vsb_nf4_variant(int M);   // nf4.cu: 0 = the NF4 GEMM of M rows dequantises W and runs the tile kernels
+
 template <typename T>
 static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
                         int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
                         const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,
-                        void* scratch, void* stream) {
+                        void* scratch, void* deq_scratch, void* stream) {
   using K = LayerOps<T>;
   VSB_CHECK_ARG(layers && x && cache && rope_cos && rope_sin && scratch, "vsb_llama_layers: null pointer");
   VSB_CHECK_ARG(n_layers > 0 && B > 0 && Tn > 0 && past >= 0 && d > 0 && H > 0 && inter > 0, "vsb_llama_layers: bad shape");
   VSB_CHECK_ARG(B <= Bc && past + Tn <= Tmax, "vsb_llama_layers: B=%d Tn=%d past=%d exceed the cache [%d, %d]", B, Tn, past, Bc, Tmax);
   VSB_CHECK_ARG(d % H == 0, "vsb_llama_layers: hidden %d not divisible by heads %d", d, H);
   VSB_CHECK_ARG(k_start == nullptr || Tn <= 4, "vsb_llama_layers: ragged batches (k_start) need Tn <= 4, got %d", Tn);
+  VSB_CHECK_ARG(q_seg == nullptr || (k_start == nullptr && tail_rows == 0), "vsb_llama_layers: q_seg excludes k_start / tail_rows");
+  // weight format: NF4 codes where the block scales are set, dense weights where they are NULL
+  const bool nf4 = layers[0].wqkv_scales != nullptr;
+  for (int li = 0; li < n_layers; ++li) {
+    const vsb_llama_layer_t& L = layers[li];
+    const int n = !!L.wqkv_scales + !!L.wo_scales + !!L.wgu_scales + !!L.wdown_scales;
+    VSB_CHECK_ARG(n == (nf4 ? 4 : 0), "vsb_llama_layers: layer %d mixes NF4 and dense projections (a table is all one or the other)", li);
+  }
+  if (nf4) {
+    VSB_CHECK_ARG(ElemT<T>::is_f16, "vsb_llama_layers: NF4 projections compute in fp16 (vsb_llama_layers_f16)");
+    VSB_CHECK_ARG(!norm_folded && tail_rows == 0, "vsb_llama_layers: NF4 projections need norm_folded = 0 and tail_rows = 0");
+    VSB_CHECK_ARG(deq_scratch, "vsb_llama_layers: NF4 projections need deq_scratch");
+  }
   const int hd = d / H;
   const long long rows = (long long)B * Tn;
   const long long ld = 3LL * d;
@@ -80,13 +95,14 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
   // tail mode: the caller consumes only the last `tail_rows` rows of every sequence (answer-predicting rows and the [LOC]
   // row of the guided search).  K/V of the last layer are needed by nobody else, so that layer runs its attention,
   // o-projection and MLP over B*tail rows only (same kernels, same per-row arithmetic => same values on those rows).
-  VSB_CHECK_ARG(q_seg == nullptr || (k_start == nullptr && tail_rows == 0), "vsb_llama_layers: q_seg excludes k_start / tail_rows");
   const bool tail = tail_rows > 0 && 2 * tail_rows <= Tn && k_start == nullptr && (hd == 64 || hd == 128);
+  // the projections of this call run on the wgmma tile kernels, whose epilogues alone fold RMSNorm and RoPE in (row counts
+  // that take the skinny / weight-streaming decode kernels keep the separate RMSNorm and RoPE kernels)
+  const bool tiles = nf4 ? vsb_nf4_variant((int)rows) == 0 : (rows > 16 || vsb_batch_invariant());
   // Folded RMSNorm (norm_folded: the caller multiplied ln1 into wqkv's and ln2 into wgu's columns): the QKV and gate|up GEMMs
   // read the un-normalised residual stream and scale their output rows by 1/rms in the epilogue; the o-proj and down-proj GEMMs
   // leave the per-row partial sums of squares of what they store.  Two kernels and ~0.3 GB of traffic less per layer at 64 crops.
-  // Needs the wgmma tile epilogue (row counts that would take the skinny decode kernels keep the unfused form, where ln = 1).
-  const bool fused = norm_folded && k_start == nullptr && d % 32 == 0 && (rows > 16 || vsb_batch_invariant());
+  const bool fused = norm_folded && k_start == nullptr && d % 32 == 0 && tiles;
   const int sqc = d / 32;                                  // partial sums per row left by a d-wide producer GEMM
   float* sq_a = reinterpret_cast<float*>(h);              // [sqc][rows]  input of the next QKV GEMM   (h itself is unused when fused)
   float* sq_b = sq_a + (long long)sqc * rows;             // [sqc][rows]  input of the gate|up GEMM
@@ -94,28 +110,54 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
     VSB_CHECK_ARG((long long)2 * sqc * rows * 4 <= rows * d * 2, "vsb_llama_layers: scratch too small for the row statistics");
     VSB_TRY(K::rowsq(xb, d, sq_a, (int)rows, d, stream));
   }
-  // RoPE in the QKV epilogue (head_dim 128, wgmma tile path): q / k reach the cache already rotated
-  const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && (rows > 16 || vsb_batch_invariant());
-  int sq_a_chunks = 1;                                     // layer 0: one full-row sum from vsb_rowsq_bf16
+  // RoPE in the QKV epilogue (head_dim 128): q / k reach the cache already rotated
+  const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && tiles;
+
+  // C [M, N] (leading dimension ldc) = epi(A W^T), A [M, Kd] with leading dimension Kd, plus C itself when `accumulate` (the
+  // residual stream).  NF4 W (scales set): vsb_gemm_nf4.  Dense W: the tile / skinny GEMM, or its row-scale form when the folded
+  // norm's row statistics go in (sq_in, sq_chunks partial sums per row) or out (sq_out), both [chunks][M].
+  auto proj = [&](const void* A, const void* W, const void* scales, void* C, long long ldc, long long M, int N, int Kd, bool accumulate,
+                  int epi, int rows_per_group, long long group_stride, long long group_offset, const float* sq_in, int sq_chunks,
+                  float* sq_out) -> int {
+    const void* res = accumulate ? C : nullptr;
+    const long long ldr = accumulate ? ldc : 0;
+    if (scales)
+      return vsb_gemm_nf4(A, Kd, W, scales, C, ldc, (int)M, N, Kd, nullptr, res, ldr, epi, 0, rows_per_group, group_stride, group_offset,
+                          deq_scratch, stream);
+    if (sq_in || sq_out)
+      return K::gemm_rowscale(A, Kd, W, Kd, C, ldc, (int)M, N, Kd, nullptr, res, ldr, epi, rows_per_group, group_stride, group_offset, sq_in,
+                              sq_chunks, rms_eps, sq_out, M, stream);
+    return K::gemm(A, Kd, W, Kd, C, ldc, (int)M, N, Kd, nullptr, res, ldr, epi, 0, rows_per_group, group_stride, group_offset, stream);
+  };
+  // x += a Wo^T ; h = RMSNorm(x) ; g = SwiGLU(h Wgu^T) ; x += g Wdown^T over the R rows of X [R, d] whose attention output is in
+  // attn.  Folded norms: the o-proj leaves the row statistics gate|up reads, and down-proj leaves them in sq_out (NULL: nowhere).
+  auto post_attention = [&](const vsb_llama_layer_t& L, T* X, long long R, float* sq_out) -> int {
+    VSB_TRY(proj(attn, L.wo, L.wo_scales, X, d, R, d, d, true, VSB_EPI_NONE, 0, 0, 0, nullptr, 0, fused ? sq_b : nullptr));
+    if (!fused) VSB_TRY(K::rmsnorm(X, d, L.ln2, h, d, (int)R, d, rms_eps, stream));
+    VSB_TRY(proj(fused ? X : h, L.wgu, L.wgu_scales, gu, inter, R, 2 * inter, d, false, VSB_EPI_SWIGLU, 0, 0, 0, fused ? sq_b : nullptr,
+                 sqc, nullptr));
+    return proj(gu, L.wdown, L.wdown_scales, X, d, R, d, inter, true, VSB_EPI_NONE, 0, 0, 0, nullptr, 0, sq_out);
+  };
+
   for (int li = 0; li < n_layers; ++li) {
     const vsb_llama_layer_t& L = layers[li];
     T* cl = reinterpret_cast<T*>(cache) + (long long)li * Bc * Tmax * ld;       // [Bc*Tmax, 3d]
-    if (fused) {
-      if (rope_fused)
-        VSB_TRY(K::gemm_qkv_rope(xb, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, sq_a, sq_a_chunks, rms_eps, rows, rope_cos,
-                                       rope_sin, positions, Tn, past, hd, stream));
-      else
-        VSB_TRY(K::gemm_rowscale(xb, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, nullptr, nullptr, 0, VSB_EPI_NONE, Tn, Tmax, past, sq_a,
-                                       sq_a_chunks, rms_eps, nullptr, rows, stream));
+    if (!fused) VSB_TRY(K::rmsnorm(xb, d, L.ln1, h, d, (int)rows, d, rms_eps, stream));
+    const T* qkv_in = fused ? xb : h;
+    const float* sq_in = fused ? sq_a : nullptr;
+    const int sq_in_chunks = !fused ? 0 : li == 0 ? 1 : sqc;   // layer 0: one full-row sum from K::rowsq
+    if (rope_fused) {
+      const void* wqkv = L.wqkv;
+      if (nf4) {                                               // the RoPE epilogue has no NF4 form: it runs on deq(wqkv)
+        VSB_TRY(vsb_nf4_dequant(L.wqkv, L.wqkv_scales, 3 * d, d, deq_scratch, d, stream));
+        wqkv = deq_scratch;
+      }
+      VSB_TRY(K::gemm_qkv_rope(qkv_in, d, wqkv, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, sq_in, sq_in_chunks, rms_eps, rows, rope_cos,
+                               rope_sin, positions, Tn, past, hd, stream));
     } else {
-      VSB_TRY(K::rmsnorm(xb, d, L.ln1, h, d, (int)rows, d, rms_eps, stream));
-      if (rope_fused)
-        VSB_TRY(K::gemm_qkv_rope(h, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, nullptr, 0, rms_eps, rows, rope_cos, rope_sin,
-                                       positions, Tn, past, hd, stream));
-      else
-        VSB_TRY(K::gemm(h, d, L.wqkv, d, cl, ld, (int)rows, 3 * d, d, nullptr, nullptr, 0, VSB_EPI_NONE, 0, Tn, Tmax, past, stream));
+      VSB_TRY(proj(qkv_in, L.wqkv, L.wqkv_scales, cl, ld, rows, 3 * d, d, false, VSB_EPI_NONE, Tn, Tmax, past, sq_in, sq_in_chunks, nullptr));
+      VSB_TRY(K::rope(cl, ld, (int)rows, Tn, H, hd, past, rope_cos, rope_sin, positions, Tmax, past, stream));
     }
-    if (!rope_fused) VSB_TRY(K::rope(cl, ld, (int)rows, Tn, H, hd, past, rope_cos, rope_sin, positions, Tmax, past, stream));
     if (tail && li == n_layers - 1) {
       const long long trows = (long long)B * tail_rows;
       T* xt = attn + trows * d;                                                     // compact copy of the tail rows of x
@@ -124,18 +166,8 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
                                 (long long)Tmax * ld, ld, (long long)tail_rows * d, d, B, H, tail_rows, past + Tn, hd, 1, scale,
                                 reinterpret_cast<cudaStream_t>(stream)));
       VSB_TRY(vsb_copy2d_b16(xb + (long long)(Tn - tail_rows) * d, (long long)Tn * d, xt, (long long)tail_rows * d, B, tail_rows * d, stream));
-      if (fused) {
-        // compact tail rows: same fused kernels on trows rows (sq_b is indexed by compact row, leading dimension trows)
-        VSB_TRY(K::gemm_rowscale(attn, d, L.wo, d, xt, d, (int)trows, d, d, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0, rms_eps,
-                                       sq_b, trows, stream));
-        VSB_TRY(K::gemm_rowscale(xt, d, L.wgu, d, gu, inter, (int)trows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, sq_b,
-                                       sqc, rms_eps, nullptr, trows, stream));
-      } else {
-        VSB_TRY(K::gemm(attn, d, L.wo, d, xt, d, (int)trows, d, d, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
-        VSB_TRY(K::rmsnorm(xt, d, L.ln2, h, d, (int)trows, d, rms_eps, stream));
-        VSB_TRY(K::gemm(h, d, L.wgu, d, gu, inter, (int)trows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, 0, stream));
-      }
-      VSB_TRY(K::gemm(gu, inter, L.wdown, inter, xt, d, (int)trows, d, inter, nullptr, xt, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
+      // compact tail rows: same kernels on trows rows (sq_b is indexed by compact row, leading dimension trows)
+      VSB_TRY(post_attention(L, xt, trows, nullptr));
       VSB_TRY(vsb_copy2d_b16(xt, (long long)tail_rows * d, xb + (long long)(Tn - tail_rows) * d, (long long)Tn * d, B, tail_rows * d, stream));
       break;
     }
@@ -148,79 +180,8 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
     else
       VSB_TRY(K::flash_attn(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
                                   (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, 1, scale, stream));
-    if (fused) {
-      VSB_TRY(K::gemm_rowscale(attn, d, L.wo, d, xb, d, (int)rows, d, d, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0, rms_eps, sq_b,
-                                     rows, stream));
-      VSB_TRY(K::gemm_rowscale(xb, d, L.wgu, d, gu, inter, (int)rows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, sq_b, sqc,
-                                     rms_eps, nullptr, rows, stream));
-      // the down projection leaves the row statistics the NEXT layer's QKV GEMM needs (nobody reads them after the last layer)
-      VSB_TRY(K::gemm_rowscale(gu, inter, L.wdown, inter, xb, d, (int)rows, d, inter, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, nullptr, 0,
-                                     rms_eps, sq_a, rows, stream));
-      sq_a_chunks = sqc;
-    } else {
-      VSB_TRY(K::gemm(attn, d, L.wo, d, xb, d, (int)rows, d, d, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
-      VSB_TRY(K::rmsnorm(xb, d, L.ln2, h, d, (int)rows, d, rms_eps, stream));
-      VSB_TRY(K::gemm(h, d, L.wgu, d, gu, inter, (int)rows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0, 0, 0, stream));
-      VSB_TRY(K::gemm(gu, inter, L.wdown, inter, xb, d, (int)rows, d, inter, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0, stream));
-    }
-  }
-  return VSB_OK;
-}
-
-int vsb_nf4_variant(int M);   // nf4.cu: 0 = the NF4 GEMM of M rows dequantises W and runs the tile kernels
-
-// NF4 projections (the SEAL VQA LLM's 4-bit mode): the unfused sequence above on vsb_gemm_nf4.  Where an M-row NF4 GEMM takes
-// the dequant + tile path, the QKV projection dequantises wqkv itself and uses the fused-RoPE tile epilogue like the f16 runner.
-extern "C" int vsb_llama_layers_nf4(const vsb_llama_layer_nf4_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache,
-                                        int Bc, int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
-                                        const void* positions, const void* k_start, const void* q_seg, int seg_lo, void* scratch,
-                                        void* deq_scratch, void* stream) {
-  using K = LayerOps<half>;
-  VSB_CHECK_ARG(layers && x && cache && rope_cos && rope_sin && scratch && deq_scratch, "vsb_llama_layers_nf4: null pointer");
-  VSB_CHECK_ARG(n_layers > 0 && B > 0 && Tn > 0 && past >= 0 && d > 0 && H > 0 && inter > 0, "vsb_llama_layers_nf4: bad shape");
-  VSB_CHECK_ARG(B <= Bc && past + Tn <= Tmax, "vsb_llama_layers_nf4: B=%d Tn=%d past=%d exceed the cache [%d, %d]", B, Tn, past, Bc, Tmax);
-  VSB_CHECK_ARG(d % H == 0, "vsb_llama_layers_nf4: hidden %d not divisible by heads %d", d, H);
-  VSB_CHECK_ARG(k_start == nullptr || Tn <= 4, "vsb_llama_layers_nf4: ragged batches (k_start) need Tn <= 4, got %d", Tn);
-  VSB_CHECK_ARG(q_seg == nullptr || k_start == nullptr, "vsb_llama_layers_nf4: q_seg excludes k_start");
-  const int hd = d / H;
-  const long long rows = (long long)B * Tn;
-  const long long ld = 3LL * d;
-  const float scale = 1.0f / sqrtf((float)hd);
-  half* xb = reinterpret_cast<half*>(x);
-  half* h = reinterpret_cast<half*>(scratch);           // [rows, d]
-  half* attn = h + rows * d;                            // [rows, d]
-  half* gu = attn + rows * d;                           // [rows, inter]
-  const bool tiles = vsb_nf4_variant((int)rows) == 0;
-  const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && tiles;
-  for (int li = 0; li < n_layers; ++li) {
-    const vsb_llama_layer_nf4_t& L = layers[li];
-    half* cl = reinterpret_cast<half*>(cache) + (long long)li * Bc * Tmax * ld;
-    VSB_TRY(K::rmsnorm(xb, d, L.ln1, h, d, (int)rows, d, rms_eps, stream));
-    if (rope_fused) {
-      VSB_TRY(vsb_nf4_dequant(L.wqkv_codes, L.wqkv_scales, 3 * d, d, deq_scratch, d, stream));
-      VSB_TRY(K::gemm_qkv_rope(h, d, deq_scratch, d, cl, ld, (int)rows, 3 * d, d, Tn, Tmax, past, nullptr, 0, rms_eps, rows, rope_cos,
-                               rope_sin, positions, Tn, past, hd, stream));
-    } else {
-      VSB_TRY(vsb_gemm_nf4(h, d, L.wqkv_codes, L.wqkv_scales, cl, ld, (int)rows, 3 * d, d, nullptr, nullptr, 0, VSB_EPI_NONE, 0, Tn,
-                               Tmax, past, deq_scratch, stream));
-      VSB_TRY(K::rope(cl, ld, (int)rows, Tn, H, hd, past, rope_cos, rope_sin, positions, Tmax, past, stream));
-    }
-    if (q_seg != nullptr)
-      VSB_TRY(K::flash_attn_seg(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
-                                (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, scale, q_seg, seg_lo, stream));
-    else if (k_start != nullptr)
-      VSB_TRY(K::attn_decode(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
-                             (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, 1, scale, k_start, stream));
-    else
-      VSB_TRY(K::flash_attn(cl + (long long)past * ld, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, (long long)Tmax * ld, ld,
-                            (long long)Tmax * ld, ld, (long long)Tn * d, d, B, H, Tn, past + Tn, hd, 1, scale, stream));
-    VSB_TRY(vsb_gemm_nf4(attn, d, L.wo_codes, L.wo_scales, xb, d, (int)rows, d, d, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0, deq_scratch,
-                             stream));
-    VSB_TRY(K::rmsnorm(xb, d, L.ln2, h, d, (int)rows, d, rms_eps, stream));
-    VSB_TRY(vsb_gemm_nf4(h, d, L.wgu_codes, L.wgu_scales, gu, inter, (int)rows, 2 * inter, d, nullptr, nullptr, 0, VSB_EPI_SWIGLU, 0, 0,
-                             0, 0, deq_scratch, stream));
-    VSB_TRY(vsb_gemm_nf4(gu, inter, L.wdown_codes, L.wdown_scales, xb, d, (int)rows, d, inter, nullptr, xb, d, VSB_EPI_NONE, 0, 0, 0, 0,
-                             deq_scratch, stream));
+    // the down projection leaves the row statistics the NEXT layer's QKV GEMM needs (nobody reads them after the last layer)
+    VSB_TRY(post_attention(L, xb, rows, fused ? sq_a : nullptr));
   }
   return VSB_OK;
 }
@@ -228,14 +189,14 @@ extern "C" int vsb_llama_layers_nf4(const vsb_llama_layer_nf4_t* layers, int n_l
 extern "C" int vsb_llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
                                 int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
                                 const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,
-                                void* scratch, void* stream) {
+                                void* scratch, void* deq_scratch, void* stream) {
   return llama_layers<bf16>(layers, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, positions, k_start,
-                            tail_rows, q_seg, seg_lo, norm_folded, scratch, stream);
+                            tail_rows, q_seg, seg_lo, norm_folded, scratch, deq_scratch, stream);
 }
 extern "C" int vsb_llama_layers_f16(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
                                     int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
                                     const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,
-                                    void* scratch, void* stream) {
+                                    void* scratch, void* deq_scratch, void* stream) {
   return llama_layers<half>(layers, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, positions, k_start,
-                            tail_rows, q_seg, seg_lo, norm_folded, scratch, stream);
+                            tail_rows, q_seg, seg_lo, norm_folded, scratch, deq_scratch, stream);
 }

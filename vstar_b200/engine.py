@@ -345,7 +345,7 @@ class LlamaClipCore:
         self._graph_seen.clear()
         return self._cache
 
-    def _llm_layers(self, x, B, Tn, past, Tmax, positions=None, k_start=None, cache_row_offset=0, tail_rows=0, q_seg=None, seg_lo=0):
+    def _llm_layers(self, x, B, Tn, past, positions=None, k_start=None, cache_row_offset=0, tail_rows=0, q_seg=None, seg_lo=0):
         """Run all decoder layers over the Tn new rows per sequence in x [B*Tn, d] (in place on the residual stream).
         Fused q|k|v rows live in the per-layer cache [B, Tmax, 3d] at positions past..past+Tn.  One native call
         (csrc/llama_layers.cu) sequences the 8 kernels of every layer: RMSNorm, QKV GEMM writing cache rows, RoPE in
@@ -429,7 +429,7 @@ class LlamaClipCore:
                 self._cache[:, self._prefix_slots:B, :P].copy_(self._prefix_kv[:, None])
                 self._prefix_slots = B
             self.stats["prefix_shared"] += B
-        self._llm_layers(x, B, Tn, P, self.max_tokens, tail_rows=tail_rows if self.tail_only else 0)
+        self._llm_layers(x, B, Tn, P, tail_rows=tail_rows if self.tail_only else 0)
         if not P:
             # a full prefill has just overwritten rows 0.. of slots 0..B-1: whatever prefix they held is gone
             self._prefix_slots = 0
@@ -448,7 +448,7 @@ class LlamaClipCore:
         if past + 1 > self._cache_shape[2]:
             self._ensure_cache(self._cache_shape[1], self._capacity(past + 64), keep=True)
         x = ops.gather_rows(tokens.contiguous(), self.w.embed)
-        self._llm_layers(x, B, 1, past, self.max_tokens)
+        self._llm_layers(x, B, 1, past)
         hn = ops.rmsnorm(x, self.w.final_norm, c.rms_eps)
         logits = ops.gemm(hn, self.w.lm_head, out_dtype=torch.float32)
         idx, _ = ops.argmax_rows(logits)

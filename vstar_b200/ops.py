@@ -186,32 +186,27 @@ def _layer_nf4(L):
 
 def llama_layer_table(layers):
     """layers: list of dicts with ln1, wqkv, wo, ln2, wgu, wdown tensors (kept alive by the caller), all bf16 or all fp16
-    -> ctypes array.  NF4 layers (wqkv, wo, wgu, wdown NF4Weight, fp16 ln1 / ln2) -> the vsb_llama_layer_nf4_t array; a table
-    cannot mix NF4 and dense layers."""
-    kinds = {_layer_nf4(L) for L in layers}
-    if len(kinds) > 1 or any(isinstance(L[k], NF4Weight) != _layer_nf4(L) for L in layers for k in NF4_LINEARS):
+    -> vsb_llama_layer_t ctypes array.  NF4 layers (wqkv, wo, wgu, wdown NF4Weight, fp16 ln1 / ln2) fill the codes into the
+    weight fields and their scales into the *_scales fields; a table cannot mix NF4 and dense layers."""
+    nf4 = _layer_nf4(layers[0])
+    if any(isinstance(L[k], NF4Weight) != nf4 for L in layers for k in NF4_LINEARS):
         raise _lib.VsbError("a layer table cannot mix NF4 and fp16 / bf16 projections")
-    if kinds == {True}:
-        arr = (_lib.LlamaLayerNF4 * len(layers))()
-        for i, L in enumerate(layers):
-            for k in ("ln1", "ln2"):
-                _chk(L[k], F16)
-                assert L[k].is_contiguous(), k
-                setattr(arr[i], k, L[k].data_ptr())
-            for k in NF4_LINEARS:
-                setattr(arr[i], k + "_codes", L[k].codes.data_ptr())
-                setattr(arr[i], k + "_scales", L[k].scales.data_ptr())
-        return arr
     arr = (_lib.LlamaLayer * len(layers))()
     dtypes = set()
     for i, L in enumerate(layers):
         for k in ("ln1", "wqkv", "wo", "ln2", "wgu", "wdown"):
             t = L[k]
-            dtypes.add(t.dtype)
-            assert t.dtype in _SUFFIX and t.is_contiguous() and t.is_cuda, k
+            if isinstance(t, NF4Weight):
+                setattr(arr[i], k + "_scales", t.scales.data_ptr())
+                t = t.codes
+            else:
+                dtypes.add(t.dtype)
+                assert t.dtype in _SUFFIX and t.is_contiguous() and t.is_cuda, k
             setattr(arr[i], k, t.data_ptr())
     if len(dtypes) > 1:
         raise _lib.VsbError(f"mixed layer weight dtypes {sorted(map(str, dtypes))}")
+    if nf4 and dtypes != {F16}:
+        raise _lib.VsbError(f"NF4 layers take fp16 ln1 / ln2, got {dtypes.pop()}")
     return arr
 
 
@@ -225,8 +220,7 @@ def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, 
     row r attends the prefix and its own continuation from key q_seg[r] on;
     norm_folded: ln1 / ln2 are already multiplied into wqkv / wgu (fused RMSNorm path, see vsb_llama_layers).
     x, cache, scratch, the RoPE tables and the table's weights are all bf16 or all fp16 (vsb_llama_layers_f16).
-    An NF4 table (fp16 only, norms not folded, tail_rows 0) runs vsb_llama_layers_nf4 and needs deq_scratch, fp16 with
-    2 * inter * d elements."""
+    An NF4 table (fp16 only, norms not folded, tail_rows 0) needs deq_scratch, fp16 with 2 * inter * d elements."""
     sfx = _sfx(x, cache, scratch, rope_cos, rope_sin)
     fn = "vsb_llama_layers" if sfx == "bf16" else "vsb_llama_layers_f16"
     assert x.is_contiguous() and cache.is_contiguous() and x.shape == (B * Tn, d)
@@ -236,21 +230,18 @@ def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, 
     assert q_seg is None or (q_seg.numel() == B * Tn and positions is not None)
     assert positions is None or positions.numel() == B * Tn
     assert k_start is None or k_start.numel() == B
-    if isinstance(table[0], _lib.LlamaLayerNF4):
+    if table[0].wqkv_scales:                    # NF4 table
         if sfx != "f16" or norm_folded or tail_rows:
             raise _lib.VsbError("NF4 layers run in fp16 with unfolded norms and tail_rows = 0")
         _chk(deq_scratch, F16)
         assert deq_scratch.is_contiguous() and deq_scratch.numel() >= 2 * inter * d
         _lib.launches += 9 * n_layers
-        call("vsb_llama_layers_nf4", table, n_layers, x.data_ptr(), B, Tn, past, cache.data_ptr() + cache_row_offset * 3 * d * 2, Bc,
-             Tmax, d, H, inter, float(eps), rope_cos.data_ptr(), rope_sin.data_ptr(), _p(positions), _p(k_start), _p(q_seg), int(seg_lo),
-             scratch.data_ptr(), deq_scratch.data_ptr(), _stream())
-        return x
-    _lib.launches += (6 if (norm_folded and k_start is None and (B * Tn > 16 or batch_invariant.depth > 0)) else 8) * n_layers + \
-        (2 if (tail_rows > 0 and 2 * tail_rows <= Tn and k_start is None) else 0)
+    else:
+        _lib.launches += (6 if (norm_folded and k_start is None and (B * Tn > 16 or batch_invariant.depth > 0)) else 8) * n_layers + \
+            (2 if (tail_rows > 0 and 2 * tail_rows <= Tn and k_start is None) else 0)
     call(fn, table, n_layers, x.data_ptr(), B, Tn, past, cache.data_ptr() + cache_row_offset * 3 * d * 2, Bc, Tmax, d, H,
          inter, float(eps), rope_cos.data_ptr(), rope_sin.data_ptr(), _p(positions), _p(k_start), int(tail_rows), _p(q_seg), int(seg_lo),
-         1 if norm_folded else 0, scratch.data_ptr(), _stream())
+         1 if norm_folded else 0, scratch.data_ptr(), _p(deq_scratch), _stream())
     return x
 
 
@@ -267,54 +258,37 @@ def _gemm_out(a, M, n_out, out, out_dtype, out_rows, residual):
     return out
 
 
-def _gemm_nf4(a, w, out, bias, residual, epilogue, out_dtype, rows_per_group, group_stride, group_offset, out_rows, deq_scratch):
-    _sfx(a, bias)
-    _chk(a, F16)
-    pa, M, K, lda = _rows2d(a)
-    assert K == w.K, (a.shape, w.shape)
-    N = w.N
-    out = _gemm_out(a, M, N // 2 if epilogue == EPI_SWIGLU else N, out, out_dtype, out_rows, residual)
-    if bias is not None:
-        assert bias.numel() == N and bias.is_contiguous()
-    if deq_scratch is None:
-        deq_scratch = torch.empty((N * K,), dtype=F16, device=a.device)
-    _chk(deq_scratch, F16)
-    assert deq_scratch.is_contiguous() and deq_scratch.numel() >= N * K
-    _lib.launches += 1
-    call("vsb_gemm_nf4", pa, lda, w.codes.data_ptr(), w.scales.data_ptr(), out.data_ptr(), out.stride(0), M, N, K, _p(bias), _p(residual),
-         residual.stride(0) if residual is not None else 0, epilogue, 1 if out.dtype == torch.float32 else 0, rows_per_group, group_stride,
-         group_offset, deq_scratch.data_ptr(), _stream())
-    return out
-
-
 def gemm(a, w, out=None, bias=None, residual=None, epilogue=EPI_NONE, out_dtype=None, rows_per_group=0,
          group_stride=0, group_offset=0, out_rows=None, deq_scratch=None):
     """out = epi(a @ w.T + bias) (+ residual).  a [M,K], w [N,K] bf16 or fp16 (row stride arbitrary, inner stride 1); out is
     fp32 or the operands' dtype (default).  w may be an NF4Weight (fp16 a): vsb_gemm_nf4, with deq_scratch (fp16, N*K
     elements) allocated here unless given."""
-    if isinstance(w, NF4Weight):
-        return _gemm_nf4(a, w, out, bias, residual, epilogue, out_dtype, rows_per_group, group_stride, group_offset, out_rows, deq_scratch)
-    sfx = _sfx(a, w, bias)
+    nf4 = isinstance(w, NF4Weight)
+    if nf4:
+        _sfx(a, bias)
+        _chk(a, F16)
+        N, K2 = w.shape
+        fn, w_args = "vsb_gemm_nf4", (w.codes.data_ptr(), w.scales.data_ptr())
+    else:
+        fn = "vsb_gemm_" + _sfx(a, w, bias)
+        pw, N, K2, ldw = _rows2d(w)
+        w_args = (pw, ldw)
     pa, M, K, lda = _rows2d(a)
-    pw, N, K2, ldw = _rows2d(w)
     assert K == K2, (a.shape, w.shape)
-    n_out = N // 2 if epilogue == EPI_SWIGLU else N
-    if out is None:
-        out = torch.empty((out_rows if out_rows is not None else M, n_out), dtype=out_dtype or a.dtype, device=a.device)
-    _chk(out)
-    assert out.dim() == 2 and out.stride(1) == 1 and out.shape[1] >= n_out
-    out_fp32 = 1 if out.dtype == torch.float32 else 0
-    if not out_fp32:
-        _sfx(a, out)
-    if residual is not None:
-        _chk(residual, out.dtype)
-        assert residual.stride(1) == 1
+    out = _gemm_out(a, M, N // 2 if epilogue == EPI_SWIGLU else N, out, out_dtype, out_rows, residual)
     if bias is not None:
         assert bias.numel() == N and bias.is_contiguous()
+    deq = ()
+    if nf4:
+        if deq_scratch is None:
+            deq_scratch = torch.empty((N * K,), dtype=F16, device=a.device)
+        _chk(deq_scratch, F16)
+        assert deq_scratch.is_contiguous() and deq_scratch.numel() >= N * K
+        deq = (deq_scratch.data_ptr(),)
     _lib.launches += 1
-    call("vsb_gemm_" + sfx, pa, lda, pw, ldw, out.data_ptr(), out.stride(0), M, N, K, _p(bias), _p(residual),
-         residual.stride(0) if residual is not None else 0, epilogue, out_fp32, rows_per_group, group_stride, group_offset,
-         _stream())
+    call(fn, pa, lda, *w_args, out.data_ptr(), out.stride(0), M, N, K, _p(bias), _p(residual),
+         residual.stride(0) if residual is not None else 0, epilogue, 1 if out.dtype == torch.float32 else 0, rows_per_group, group_stride,
+         group_offset, *deq, _stream())
     return out
 
 

@@ -212,7 +212,7 @@ class VQAEngine(LlamaClipCore):
         T = x.shape[0]
         self._ensure_cache(1, self._capacity(T + reserve))
         self._prefix_slots = 0
-        self._llm_layers(x, 1, T, 0, self.max_tokens)
+        self._llm_layers(x, 1, T, 0)
         self.kv_epoch = getattr(self, "kv_epoch", 0) + 1        # handles to an older prefix are stale from here on
         return x
 
@@ -222,7 +222,7 @@ class VQAEngine(LlamaClipCore):
         x = ops.gather_rows(ids, self.w.embed)
         if past + len(tokens) > self._cache_shape[2]:
             self._ensure_cache(self._cache_shape[1], self._capacity(past + len(tokens) + 64), keep=True)
-        self._llm_layers(x, 1, len(tokens), past, self.max_tokens)
+        self._llm_layers(x, 1, len(tokens), past)
         hn = ops.rmsnorm(x, self.w.final_norm, self.cfg.rms_eps)
         return ops.gemm(hn, self.w.lm_head, out_dtype=torch.float32)
 
@@ -286,7 +286,7 @@ class VQAEngine(LlamaClipCore):
                 G += 1
             T = lens[b]
             x = torch.cat(xs[b:b + G], 0).contiguous() if G > 1 else xs[b]
-            self._llm_layers(x, G, T, 0, Tm, cache_row_offset=b * Tm + (Tpad - T))
+            self._llm_layers(x, G, T, 0, cache_row_offset=b * Tm + (Tpad - T))
             last += [x[g * T + T - 1:g * T + T] for g in range(G)]
             b += G
         self.kv_epoch = getattr(self, "kv_epoch", 0) + 1
@@ -302,7 +302,7 @@ class VQAEngine(LlamaClipCore):
             self._ensure_cache(self._cache_shape[1], self._capacity(Tpad + step + 64), keep=True)
         positions = torch.tensor([n + step for n in lens], dtype=torch.int32, device=self.dev)
         k_start = torch.tensor([Tpad - n for n in lens], dtype=torch.int32, device=self.dev)
-        self._llm_layers(x, B, 1, Tpad + step, self._cache_shape[2], positions=positions, k_start=k_start)
+        self._llm_layers(x, B, 1, Tpad + step, positions=positions, k_start=k_start)
         hn = ops.rmsnorm(x, self.w.final_norm, self.cfg.rms_eps)
         return ops.gemm(hn, self.w.lm_head, out_dtype=torch.float32)
 
@@ -389,7 +389,7 @@ class VQAEngine(LlamaClipCore):
             self._ensure_cache(G, self._capacity(Tq + Tn))
             self._prefix_slots = 0
             x = torch.cat([embeds[i] for i in members], 0).contiguous() if G > 1 else embeds[members[0]]
-            self._llm_layers(x, G, Tq, 0, self.max_tokens)
+            self._llm_layers(x, G, Tq, 0)
             self.kv_epoch = getattr(self, "kv_epoch", 0) + 1
             last = torch.tensor([g * Tq + Tq - 1 for g in range(G)], dtype=torch.int64, device=dev)
             _, _, q_last = self._logits_rows(x, last)                          # [G, V]: predicts the first token of every option
@@ -410,7 +410,7 @@ class VQAEngine(LlamaClipCore):
                 for r in range(off, Tn):
                     pos[g, r], seg[g, r] = Tq, Tq + r
             xo = ops.gather_rows(ids.view(-1).to(dev), self.w.embed)
-            self._llm_layers(xo, G, Tn, Tq, self.max_tokens, positions=pos.view(-1).to(dev), q_seg=seg.view(-1).to(dev), seg_lo=Tq)
+            self._llm_layers(xo, G, Tn, Tq, positions=pos.view(-1).to(dev), q_seg=seg.view(-1).to(dev), seg_lo=Tq)
             hn = ops.rmsnorm(xo, self.w.final_norm, self.cfg.rms_eps)
             lo = ops.gemm(hn, self.w.lm_head, out_dtype=torch.float32)
             rows = torch.cat([q_last, lo], 0).index_select(0, torch.tensor(pred, dtype=torch.int64, device=dev)).contiguous()
