@@ -139,6 +139,8 @@ int vsb_add_rows_f16(const void* a, const void* b, void* y, long long rows, int 
 int vsb_cast_f32_bf16(const void* x, void* y, long long n, void* stream);
 /* f16 twin of vsb_cast_f32_bf16 (the reference's .half() of fp32 pixels) */
 int vsb_cast_f32_f16(const void* x, void* y, long long n, void* stream);
+/* Greedy token of every row of fp32 logits [rows, n]: torch.argmax's index (the first maximum; NaN counts as the largest value,
+ * the first NaN wins) and its value */
 int vsb_argmax_rows_f32(const void* x, long long ld, int rows, int n, void* idx_i32, void* val_f32, void* stream);
 /* Sampled next token of every row of fp32 logits [rows, n] (HF `sample()` with TemperatureLogitsWarper, TopKLogitsWarper,
  * TopPLogitsWarper and multinomial(softmax), as transformers 4.31 runs them for free_form_inference(temperature > 0)).  Per row:

@@ -347,7 +347,15 @@ __global__ void cast_f32_kernel(const float* __restrict__ x, T* __restrict__ y, 
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) y[i] = ElemT<T>::from_f(x[i]);
 }
 
-// argmax over rows of fp32 logits [rows, n] -> idx (int32) and value
+// (v, i) replaces (best, bi) as the running argmax.  torch.argmax's order: NaN is larger than every number (the first NaN
+// wins), ties go to the smaller index.  So a row of NaN or of -inf still returns an index inside the row.
+__device__ __forceinline__ bool argmax_better(float v, int i, float best, int bi) {
+  const bool vn = v != v, bn = best != best;
+  if (vn || bn) return vn && (!bn || i < bi);
+  return v > best || (v == best && i < bi);
+}
+
+// argmax over rows of fp32 logits [rows, n] -> idx (int32) and value (= x[idx]), with torch.argmax's semantics (above)
 __global__ void __launch_bounds__(256) argmax_rows_kernel(const float* __restrict__ x, long long ld, int n, int* __restrict__ idx,
                                                           float* __restrict__ val) {
   __shared__ float sv[8];
@@ -357,18 +365,18 @@ __global__ void __launch_bounds__(256) argmax_rows_kernel(const float* __restric
   int bi = 0x7fffffff;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     float v = xr[i];
-    if (v > best || (v == best && i < bi)) { best = v; bi = i; }
+    if (argmax_better(v, i, best, bi)) { best = v; bi = i; }
   }
   for (int o = 16; o > 0; o >>= 1) {
     float ov = __shfl_xor_sync(0xffffffffu, best, o);
     int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+    if (argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
   }
   if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = best; si[threadIdx.x >> 5] = bi; }
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 1; w < (blockDim.x >> 5); ++w)
-      if (sv[w] > best || (sv[w] == best && si[w] < bi)) { best = sv[w]; bi = si[w]; }
+      if (argmax_better(sv[w], si[w], best, bi)) { best = sv[w]; bi = si[w]; }
     idx[blockIdx.x] = bi;
     if (val) val[blockIdx.x] = best;
   }

@@ -436,6 +436,8 @@ def cast_f32(x, dtype, out=None):
 
 
 def argmax_rows(x):
+    """fp32 x [rows, n] (unit inner stride) -> (idx int32 [rows], val fp32 [rows] = x[row, idx]), the index torch.argmax
+    returns: the first maximum, where NaN counts as larger than every number (the first NaN wins)"""
     _chk(x, torch.float32)
     p, rows, n, ld = _rows2d(x)
     idx = torch.empty((rows,), dtype=torch.int32, device=x.device)
