@@ -157,6 +157,26 @@ int vsb_sample_rows_f32(const void* logits, long long ld, int rows, int n, float
 int vsb_nll_rows_f32(const void* logits, long long ld, int rows, int n, const void* labels_i64, void* out_f32, void* stream);
 int vsb_copy2d_b16(const void* src, long long lds, void* dst, long long ldd, long long rows, int cols, void* stream);
 
+/* Beam search of the SEAL VQA LLM (HF `beam_search` of transformers 4.31 for free_form_inference(num_beams = k),
+ * /root/reference/vstar_bench_eval.py:91-103).  Candidates of one step for `requests` requests of k_in rows each (1 on the first
+ * step, k afterwards): rows_i32 [requests, k_in] are the rows of the fp32 logits [*, V] (cache-slot order) that hold the
+ * request's beams in beam order, scores_f32 [requests, k_in] their running scores.  Per row, logp = dtype(x - max - log sum
+ * exp(x - max)) of x = float(dtype(logit)) (sum and difference in fp64, rounded once to logit_dtype), candidate score
+ * float(logp) + beam score in fp32.  Output per request: the 2k largest candidate scores over k_in * V, descending, ties by
+ * ascending beam * V + token: out_score_f32, out_token_i32, out_beam_i32 [requests, 2k] (device).  1 <= k <= VSB_BEAM_MAX. */
+#define VSB_BEAM_MAX 16
+int vsb_beam_candidates_f32(const void* logits, long long ld, int V, int requests, int k_in, int k, const void* rows_i32,
+                            const void* scores_f32, int logit_dtype, void* out_score_f32, void* out_token_i32, void* out_beam_i32,
+                            void* stream);
+/* Beam reordering of the fused-QKV cache: for every layer l < layers and every pair p, rows [lo, hi) of slot
+ * pairs_i32[2p] are copied bit-exactly to slot pairs_i32[2p+1] (element (l, slot, row, c) at cache + l*layer_stride +
+ * slot*slot_stride + row*row_stride + c, c < row_elems; 2-byte elements).  pairs_i32 is a HOST array of npairs (src, dst)
+ * pairs, at most VSB_COPY_ROWS_MAX_PAIRS; a slot that is both a source and a destination, a destination named twice or a slot
+ * outside [0, slots) is refused with VSB_ERR_ARG.  One launch. */
+#define VSB_COPY_ROWS_MAX_PAIRS 256
+int vsb_copy_cache_rows_b16(void* cache, int layers, long long layer_stride, int slots, long long slot_stride, long long row_stride,
+                            int row_elems, const int* pairs_i32, int npairs, int lo, int hi, void* stream);
+
 /* The whole Llama decoder stack over Tn new rows per sequence, in place on the residual stream x [B*Tn, d] bf16
  * (HF LlamaModel layers as called from llava_llama.py:93-105 / llava_search_llama.py:80-92).  Fused q|k|v rows live in
  * cache [n_layers][Bc][Tmax][3d] at positions past..past+Tn; weights: wqkv [3d,d] (q|k|v rows), wo [d,d], wgu [2*inter,d]

@@ -13,7 +13,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libvstar_b200.so")
-SOURCES = ["api.cu", "gemm_tcgen05.cu", "gemm_skinny.cu", "llama_layers.cu", "attention.cu", "attention_tc.cu", "elementwise.cu", "heads.cu", "image.cu", "nf4.cu", "sampling.cu"]
+SOURCES = ["api.cu", "gemm_tcgen05.cu", "gemm_skinny.cu", "llama_layers.cu", "attention.cu", "attention_tc.cu", "elementwise.cu", "heads.cu", "image.cu", "nf4.cu", "sampling.cu",
+           "beam.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
@@ -26,7 +27,8 @@ def _newer(a, b):
 def build(force=False, verbose=False):
     objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
-    deps = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "wgmma.cuh"), os.path.join(ROOT, "include", "vstar_b200.h")]
+    deps = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "wgmma.cuh"), os.path.join(CSRC, "radix_select.cuh"),
+            os.path.join(ROOT, "include", "vstar_b200.h")]
     objs, procs = [], []
     for src in SOURCES:
         s = os.path.join(CSRC, src)

@@ -1,0 +1,299 @@
+// Beam search of the SEAL VQA LLM (free_form_inference(num_beams = k), HF `beam_search` of transformers 4.31 as restated in
+// oracle/beam_oracle.py): the per-step candidate selection and the KV-cache row copies that reorder the beams.
+//
+// vsb_beam_candidates_f32: one CTA per request.  For each of the request's k_in rows (cache-slot rows of the logits):
+//   logp_i = dtype(x_i - max - log sum_j exp(x_j - max)), x = float(dtype(logit)), the sum in fp64 over fp32 exp terms and the
+//   difference in fp64, rounded once to dtype; candidate score s = float(logp_i) + beam_score in fp32.
+// The 2k largest s over the request's k_in * V candidates, ties by ascending flattened index beam * V + token, are found by a
+// four-pass 8-bit radix select on the 32-bit order-preserving key of s (radix_select.cuh), so equal fp32 sums of distinct
+// log-probs tie exactly as they do in the oracle.  The candidates at or above the threshold are compacted into shared memory
+// and bitonic-sorted by (key desc, index asc); a tie at the threshold wider than that buffer is resolved by one ordered pass.
+//
+// vsb_copy_cache_rows_b16: rows [lo, hi) of the fused-QKV cache [L][B, Tmax, 3d] from slot src to slot dst for every layer and
+// every pair, in one launch.  Pairs travel in the kernel's parameters; a slot that is both a source and a destination (or two
+// pairs with one destination) is refused, so no CTA reads a row another CTA writes.
+#include <algorithm>
+
+#include "common.cuh"
+#include "radix_select.cuh"
+#include "vstar_b200.h"
+
+#define STREAM(s) reinterpret_cast<cudaStream_t>(s)
+
+namespace {
+
+constexpr int kThreads = 1024;
+constexpr int kWarps = kThreads / 32;
+constexpr int kMaxBeams = VSB_BEAM_MAX;
+constexpr int kCap = 2048;                     // candidates at or above the threshold sorted in shared memory
+
+template <bool F16>
+__device__ __forceinline__ float round_dt(float x) {
+  return F16 ? __half2float(__float2half_rn(x)) : __bfloat162float(__float2bfloat16_rn(x));
+}
+
+template <bool F16>
+__device__ __forceinline__ float round_dt_d(double x) {
+  return F16 ? __half2float(__double2half(x)) : __bfloat162float(__double2bfloat16(x));
+}
+
+// order-preserving 32-bit key of an fp32 value; -0 is folded onto +0 (they compare equal)
+__device__ __forceinline__ uint32_t f32_key(float s) {
+  uint32_t b = __float_as_uint(s);
+  if (b == 0x80000000u) b = 0;
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+__device__ __forceinline__ float key_f32(uint32_t key) {
+  return __uint_as_float((key & 0x80000000u) ? (key & 0x7FFFFFFFu) : ~key);
+}
+
+__device__ __forceinline__ float block_max_f(float v, float* red) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  __syncthreads();
+  if (lane == 0) red[w] = v;
+  __syncthreads();
+  v = red[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+__device__ __forceinline__ double block_sum_d(double v, double* red) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if (lane == 0) red[w] = v;
+  __syncthreads();
+  v = red[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+struct RowStats {
+  float mx[kMaxBeams];
+  double lse[kMaxBeams];
+  float score[kMaxBeams];
+  const float* row[kMaxBeams];
+};
+
+template <bool F16>
+__device__ __forceinline__ uint32_t cand_key(const RowStats& st, int j, int i) {
+  const float x = round_dt<F16>(st.row[j][i]);
+  const float lp = round_dt_d<F16>((double)x - (double)st.mx[j] - st.lse[j]);
+  return f32_key(lp + st.score[j]);
+}
+
+// sort cand[0, n) descending (bitonic over the next power of two, padded with 0 = below every real entry)
+__device__ void sort_desc(unsigned long long* cand, int n) {
+  const int t = threadIdx.x;
+  int P = 1;
+  while (P < n) P <<= 1;
+  for (int i = n + t; i < P; i += kThreads) cand[i] = 0ull;
+  __syncthreads();
+  for (int size = 2; size <= P; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int i = t; i < (P >> 1); i += kThreads) {
+        const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
+        const bool desc = (lo & size) == 0;
+        const unsigned long long a = cand[lo], b = cand[hi];
+        if ((a < b) == desc) {
+          cand[lo] = b;
+          cand[hi] = a;
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(kThreads, 1) beam_candidates_kernel(const float* __restrict__ logits, long long ld, int V, int k_in,
+                                                                      int need, const int* __restrict__ rows,
+                                                                      const float* __restrict__ scores, float* __restrict__ out_s,
+                                                                      int* __restrict__ out_t, int* __restrict__ out_b) {
+  __shared__ RowStats st;
+  __shared__ unsigned long long cand[kCap];     // (key << 32) | ~flat: descending order = score desc, flat index asc
+  __shared__ int hist[256];
+  __shared__ int wsum[kWarps];
+  __shared__ float redf[kWarps];
+  __shared__ double redd[kWarps];
+  __shared__ int s_bin, s_above, s_count;
+
+  const int t = threadIdx.x, lane = t & 31;
+  const int r = blockIdx.x;
+
+  // ---- per row: max and log-sum-exp of the dtype-rounded logits
+  for (int j = 0; j < k_in; ++j) {
+    const float* row = logits + (long long)rows[r * k_in + j] * ld;
+    float mx = -INFINITY;
+    for (int i = t; i < V; i += kThreads) mx = fmaxf(mx, round_dt<F16>(row[i]));
+    mx = block_max_f(mx, redf);
+    double s = 0.0;
+    for (int i = t; i < V; i += kThreads) s += (double)expf(round_dt<F16>(row[i]) - mx);
+    s = block_sum_d(s, redd);
+    if (t == 0) {
+      st.row[j] = row;
+      st.mx[j] = mx;
+      st.lse[j] = log(s);
+      st.score[j] = scores[r * k_in + j];
+    }
+  }
+  __syncthreads();
+
+  // ---- radix select of the need-th largest key (with multiplicity)
+  uint32_t prefix = 0, mask = 0;
+  int want = need;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    if (t < 256) hist[t] = 0;
+    __syncthreads();
+    for (int j = 0; j < k_in; ++j) {
+      for (int i0 = 0; i0 < V; i0 += kThreads) {
+        const int i = i0 + t;
+        int bin = -1;
+        if (i < V) {
+          const uint32_t key = cand_key<F16>(st, j, i);
+          if ((key & mask) == prefix) bin = (int)((key >> shift) & 255u);
+        }
+        const unsigned grp = __match_any_sync(0xffffffffu, bin);            // one shared atomic per distinct bin of the warp
+        if (bin >= 0 && lane == __ffs(grp) - 1) atomicAdd(&hist[bin], __popc(grp));
+      }
+    }
+    __syncthreads();
+    radix_bucket(hist, want, wsum, &s_bin, &s_above);
+    prefix |= (uint32_t)s_bin << shift;
+    mask |= 0xFFu << shift;
+    want -= s_above;
+  }
+  const uint32_t tau = prefix;
+  const int above = need - want;                                            // candidates with key > tau
+  const int ncand = above + hist[s_bin];                                    // ... and with key >= tau
+  if (t == 0) s_count = 0;
+  __syncthreads();
+
+  const bool wide = ncand > kCap;
+  for (int j = 0; j < k_in; ++j) {
+    for (int i = t; i < V; i += kThreads) {
+      const uint32_t key = cand_key<F16>(st, j, i);
+      if (key > tau || (!wide && key == tau))
+        cand[atomicAdd(&s_count, 1)] = ((unsigned long long)key << 32) | (uint32_t)~(uint32_t)(j * V + i);
+    }
+  }
+  __syncthreads();
+  int n = ncand;
+  if (wide) {
+    // the `want` ties at tau with the lowest flattened indices, by one ordered pass
+    int seen = 0;
+    for (int f0 = 0; f0 < k_in * V && seen < want; f0 += kThreads) {
+      const int f = f0 + t;
+      const int j = f / V;
+      const bool hit = f < k_in * V && cand_key<F16>(st, j, f - j * V) == tau;
+      const unsigned bal = __ballot_sync(0xffffffffu, hit);
+      if (lane == 0) wsum[t >> 5] = __popc(bal);
+      __syncthreads();
+      int before = seen, total = 0;
+      for (int q = 0; q < kWarps; ++q) {
+        if (q < (t >> 5)) before += wsum[q];
+        total += wsum[q];
+      }
+      const int pos = before + __popc(bal & ((1u << lane) - 1u));
+      if (hit && pos < want) cand[above + pos] = ((unsigned long long)tau << 32) | (uint32_t)~(uint32_t)f;
+      seen += total;
+      __syncthreads();
+    }
+    n = need;
+  }
+  sort_desc(cand, n);
+  if (t < need) {
+    const unsigned long long c = cand[t];
+    const int f = (int)~(uint32_t)c;
+    out_s[r * need + t] = key_f32((uint32_t)(c >> 32));
+    out_b[r * need + t] = f / V;
+    out_t[r * need + t] = f - (f / V) * V;
+  }
+}
+
+struct CopyPairs {
+  int src[VSB_COPY_ROWS_MAX_PAIRS];
+  int dst[VSB_COPY_ROWS_MAX_PAIRS];
+};
+
+// grid (chunks, layers, pairs): rows [lo, hi) of one slot of one layer, as VEC-element vectors
+template <typename VEC>
+__global__ void __launch_bounds__(256) copy_cache_rows_kernel(unsigned short* cache, long long layer_stride, long long slot_stride,
+                                                              long long row_stride, int row_elems, int lo, int hi, const CopyPairs pairs) {
+  constexpr int kVec = sizeof(VEC) / 2;
+  const int p = blockIdx.z;
+  unsigned short* base = cache + (long long)blockIdx.y * layer_stride;
+  const VEC* src = reinterpret_cast<const VEC*>(base + (long long)pairs.src[p] * slot_stride);
+  VEC* dst = reinterpret_cast<VEC*>(base + (long long)pairs.dst[p] * slot_stride);
+  const int per_row = row_elems / kVec;
+  const long long rs = row_stride / kVec;
+  const long long total = (long long)(hi - lo) * per_row;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const long long row = lo + e / per_row, c = e % per_row;
+    dst[row * rs + c] = src[row * rs + c];
+  }
+}
+
+}  // namespace
+
+extern "C" int vsb_beam_candidates_f32(const void* logits, long long ld, int V, int requests, int k_in, int k, const void* rows_i32,
+                                       const void* scores_f32, int logit_dtype, void* out_score_f32, void* out_token_i32,
+                                       void* out_beam_i32, void* stream) {
+  VSB_CHECK_ARG(logits && rows_i32 && scores_f32 && out_score_f32 && out_token_i32 && out_beam_i32, "vsb_beam_candidates_f32: null pointer");
+  VSB_CHECK_ARG(V > 0 && ld >= V, "vsb_beam_candidates_f32: bad V / ld");
+  VSB_CHECK_ARG(k >= 1 && k <= VSB_BEAM_MAX, "vsb_beam_candidates_f32: k must be in [1, %d], got %d", VSB_BEAM_MAX, k);
+  VSB_CHECK_ARG(k_in >= 1 && k_in <= k, "vsb_beam_candidates_f32: k_in must be in [1, k], got %d", k_in);
+  VSB_CHECK_ARG((long long)k_in * V >= 2 * k && (long long)k_in * V < (1ll << 31), "vsb_beam_candidates_f32: k_in * V must be in [2k, 2^31)");
+  VSB_CHECK_ARG(logit_dtype == VSB_DTYPE_BF16 || logit_dtype == VSB_DTYPE_F16, "vsb_beam_candidates_f32: logit_dtype must be VSB_DTYPE_BF16 or VSB_DTYPE_F16");
+  if (requests <= 0) return VSB_OK;
+  if (logit_dtype == VSB_DTYPE_F16)
+    beam_candidates_kernel<true><<<requests, kThreads, 0, STREAM(stream)>>>((const float*)logits, ld, V, k_in, 2 * k, (const int*)rows_i32,
+                                                                            (const float*)scores_f32, (float*)out_score_f32,
+                                                                            (int*)out_token_i32, (int*)out_beam_i32);
+  else
+    beam_candidates_kernel<false><<<requests, kThreads, 0, STREAM(stream)>>>((const float*)logits, ld, V, k_in, 2 * k, (const int*)rows_i32,
+                                                                             (const float*)scores_f32, (float*)out_score_f32,
+                                                                             (int*)out_token_i32, (int*)out_beam_i32);
+  VSB_LAUNCH_CHECK();
+  return VSB_OK;
+}
+
+extern "C" int vsb_copy_cache_rows_b16(void* cache, int layers, long long layer_stride, int slots, long long slot_stride, long long row_stride,
+                                       int row_elems, const int* pairs_i32, int npairs, int lo, int hi, void* stream) {
+  VSB_CHECK_ARG(cache && layers > 0 && slots > 0 && row_elems > 0 && row_stride >= row_elems, "vsb_copy_cache_rows_b16: bad args");
+  VSB_CHECK_ARG(npairs >= 0 && npairs <= VSB_COPY_ROWS_MAX_PAIRS, "vsb_copy_cache_rows_b16: npairs must be in [0, %d], got %d",
+                VSB_COPY_ROWS_MAX_PAIRS, npairs);
+  VSB_CHECK_ARG(0 <= lo && lo <= hi && (long long)hi * row_stride <= slot_stride, "vsb_copy_cache_rows_b16: bad row range [%d, %d)", lo, hi);
+  VSB_CHECK_ARG(npairs == 0 || pairs_i32, "vsb_copy_cache_rows_b16: null pair list");
+  CopyPairs pp;
+  for (int p = 0; p < npairs; ++p) {
+    const int s = pairs_i32[2 * p], d = pairs_i32[2 * p + 1];
+    VSB_CHECK_ARG(s >= 0 && s < slots && d >= 0 && d < slots, "vsb_copy_cache_rows_b16: pair %d (%d -> %d) outside [0, %d)", p, s, d, slots);
+    for (int q = 0; q < npairs; ++q) {
+      VSB_CHECK_ARG(pairs_i32[2 * q + 1] != s, "vsb_copy_cache_rows_b16: slot %d is both a source and a destination", s);
+      VSB_CHECK_ARG(q == p || pairs_i32[2 * q + 1] != d, "vsb_copy_cache_rows_b16: slot %d is the destination of two pairs", d);
+    }
+    pp.src[p] = s;
+    pp.dst[p] = d;
+  }
+  if (npairs == 0 || hi == lo) return VSB_OK;
+  const bool vec = ((reinterpret_cast<uintptr_t>(cache) | (uintptr_t)layer_stride * 2 | (uintptr_t)slot_stride * 2 |
+                     (uintptr_t)row_stride * 2 | (uintptr_t)row_elems * 2) & 15) == 0;
+  const long long elems = (long long)(hi - lo) * row_elems / (vec ? 8 : 1);
+  const int chunks = (int)std::min<long long>((elems + 255) / 256, 64);
+  dim3 grid(chunks, layers, npairs);
+  if (vec)
+    copy_cache_rows_kernel<uint4><<<grid, 256, 0, STREAM(stream)>>>((unsigned short*)cache, layer_stride, slot_stride, row_stride, row_elems,
+                                                                   lo, hi, pp);
+  else
+    copy_cache_rows_kernel<unsigned short><<<grid, 256, 0, STREAM(stream)>>>((unsigned short*)cache, layer_stride, slot_stride, row_stride,
+                                                                            row_elems, lo, hi, pp);
+  VSB_LAUNCH_CHECK();
+  return VSB_OK;
+}

@@ -15,6 +15,7 @@
 // k-th value): binary searches over the row's keys, each probe one block-reduced pass over the row; tokens of one key share one
 // probability, so the position inside the chosen key is found arithmetically and then by one ordered pass.
 #include "common.cuh"
+#include "radix_select.cuh"
 #include "vstar_b200.h"
 
 #define STREAM(s) reinterpret_cast<cudaStream_t>(s)
@@ -81,31 +82,6 @@ __device__ __forceinline__ double block_sum_d(double v, double* red) {
   __syncthreads();
   v = warp_sum_d(lane < kWarps ? red[lane] : 0.0);
   return v;
-}
-
-// hist[256] (by bin) -> the largest bin b whose count summed with every bin above it reaches k, and the count above b
-__device__ __forceinline__ void radix_bucket(const int* hist, int k, int* wsum, int* out_bin, int* out_above) {
-  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
-  int h = 0, s = 0;
-  if (t < 256) {
-    h = hist[255 - t];                                   // thread t holds bins in descending order
-    s = h;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += y;
-    }
-    if (lane == 31) wsum[w] = s;
-  }
-  __syncthreads();
-  if (t < 256) {
-    for (int i = 0; i < w; ++i) s += wsum[i];
-    if (s >= k && s - h < k) {
-      *out_bin = 255 - t;
-      *out_above = s - h;
-    }
-  }
-  __syncthreads();
 }
 
 template <bool F16>

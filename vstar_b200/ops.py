@@ -464,6 +464,53 @@ def sample_rows(x, temperature, top_k, top_p, dtype, seeds, step):
     return idx
 
 
+BEAM_MAX = 16                                   # VSB_BEAM_MAX
+COPY_ROWS_MAX_PAIRS = 256                       # VSB_COPY_ROWS_MAX_PAIRS
+
+
+def beam_candidates(x, rows, scores, k, dtype, out=None):
+    """one beam-search step (vsb_beam_candidates_f32) for R requests: x fp32 logits [*, V] (unit inner stride), rows int32
+    [R, k_in] the rows of x holding each request's beams in beam order, scores fp32 [R, k_in] their running scores (device).
+    Log-softmax of the logits rounded to `dtype`, + beam score, the 2k best per request (ties by ascending beam * V + token).
+    -> int32 [3, R, 2k]: scores (fp32 bits), tokens, beams - one buffer, so the host reads it with one copy"""
+    _chk(x, torch.float32)
+    p, _, V, ld = _rows2d(x)
+    _chk(rows, torch.int32)
+    _chk(scores, torch.float32)
+    assert rows.dim() == 2 and rows.is_contiguous() and scores.shape == rows.shape and scores.is_contiguous()
+    if dtype not in _SUFFIX:
+        raise _lib.VsbError(f"unsupported dtype {dtype}: the logits are rounded to bf16 or fp16")
+    R, k_in = rows.shape
+    if out is None:
+        out = torch.empty((3, R, 2 * k), dtype=torch.int32, device=x.device)
+    assert out.shape == (3, R, 2 * k) and out.dtype == torch.int32 and out.is_contiguous()
+    _lib.launches += 1
+    call("vsb_beam_candidates_f32", p, ld, V, R, k_in, int(k), rows.data_ptr(), scores.data_ptr(), 1 if dtype == F16 else 0,
+         out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(), _stream())
+    return out
+
+
+def copy_cache_rows(cache, pairs, lo, hi):
+    """rows [lo, hi) of every layer of the fused-QKV cache [L, B, Tmax, 3d] from slot s to slot d for every (s, d) in the host
+    list `pairs` (vsb_copy_cache_rows_b16, one launch per COPY_ROWS_MAX_PAIRS pairs).  A slot that is both a source and a
+    destination raises VsbError."""
+    import ctypes
+    _chk(cache)
+    assert cache.dim() == 4 and cache.element_size() == 2 and cache.stride(3) == 1
+    if len(pairs) > COPY_ROWS_MAX_PAIRS:
+        srcs = {s for s, _ in pairs}
+        if srcs & {d for _, d in pairs}:
+            raise _lib.VsbError("vsb_copy_cache_rows_b16: a slot is both a source and a destination")
+    L, B, _, W = cache.shape
+    for i in range(0, max(1, len(pairs)), COPY_ROWS_MAX_PAIRS):
+        chunk = pairs[i:i + COPY_ROWS_MAX_PAIRS]
+        arr = (ctypes.c_int * (2 * max(1, len(chunk))))(*[v for pr in chunk for v in pr])
+        _lib.launches += 1
+        call("vsb_copy_cache_rows_b16", cache.data_ptr(), L, cache.stride(0), B, cache.stride(1), cache.stride(2), W, arr, len(chunk),
+             int(lo), int(hi), _stream())
+    return cache
+
+
 def nll_rows(logits, labels):
     """logits fp32 [rows, V], labels int64 [rows] -> nll fp32 [rows]"""
     _chk(logits, torch.float32)

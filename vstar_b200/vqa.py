@@ -16,6 +16,8 @@ VQA_LLM(args) with args.vqa_dtype = "fp16".  fp16 brings the option NLLs and log
 numbers (tests/test_vqa_fp16_gpu.py; DESIGN.md §7b).  The VSM stays bf16, as in the reference.
 free_form_inference(temperature > 0, top_p) samples like the reference's `generate(do_sample=True)`: one vsb_sample_rows_f32
 launch per decode step in place of the greedy argmax (oracle/sampling_oracle.py; DESIGN.md §7b).
+free_form_inference(num_beams = k) runs HF's beam search (transformers 4.31): VQAEngine.beam_search, one vsb_beam_candidates_f32
+launch per step and copy-on-fork KV-row copies (vstar_b200/beam.py, oracle/beam_oracle.py; DESIGN.md §7b).
 """
 from __future__ import annotations
 
@@ -23,6 +25,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .beam import DEFAULT_EARLY_STOPPING, DEFAULT_LENGTH_PENALTY, BeamRequest, check_beams
 from .config import VSMConfig
 from .engine import CoreWeights, LlamaClipCore
 from .vsm import CLIP_MEAN, SyntheticTokenizer, _normalize_into
@@ -90,17 +93,24 @@ def draw_seeds(n):
     return torch.empty(n, dtype=torch.int64).random_().tolist()
 
 
-def generation_top_k(model_path):
-    """top_k of the checkpoint's generation_config.json, else the transformers 4.31 default (50)"""
+def generation_top_k(model_path, beams=False):
+    """top_k of the checkpoint's generation_config.json, else the transformers 4.31 default (50).
+    beams=True: -> (top_k, length_penalty, early_stopping), each from the file when it sets it, else the 4.31 default
+    (50, 1.0, False)"""
     import json
     import os
     path = os.path.join(str(model_path), "generation_config.json")
+    cfg = {}
     if os.path.isfile(path):
         with open(path) as f:
-            k = json.load(f).get("top_k")
-        if k is not None:
-            return int(k)
-    return DEFAULT_TOP_K
+            cfg = json.load(f)
+    k = cfg.get("top_k")
+    k = DEFAULT_TOP_K if k is None else int(k)
+    if not beams:
+        return k
+    lp = cfg.get("length_penalty")
+    es = cfg.get("early_stopping")
+    return k, DEFAULT_LENGTH_PENALTY if lp is None else float(lp), DEFAULT_EARLY_STOPPING if es is None else es
 
 
 class VQAWeights(CoreWeights):
@@ -243,11 +253,17 @@ class VQAEngine(LlamaClipCore):
         return lambda logits, step: ops.sample_rows(logits, T, top_k, top_p, dtype, sd, step)
 
     def generate(self, input_ids, image, object_crops=None, images_long=None, objects_long=None, max_new_tokens=200, eos_token_id=2,
-                 stop_ids=None, stop_fn=None, temperature=0, top_k=DEFAULT_TOP_K, top_p=None, seed=None):
+                 stop_ids=None, stop_fn=None, temperature=0, top_k=DEFAULT_TOP_K, top_p=None, seed=None, num_beams=1,
+                 length_penalty=DEFAULT_LENGTH_PENALTY, early_stopping=DEFAULT_EARLY_STOPPING):
         """greedy `model.generate(use_cache=True, do_sample=False)` (vstar_bench_eval.py:91-103) -> list of new token ids.
         stop_ids: stop once the output ends with these ids; stop_fn(new_ids) -> bool: HF-style stopping criterion.
         temperature > 0: sampled decoding instead (`do_sample=True` with top_k / top_p, ops.sample_rows); token t is drawn with
-        (seed, step t), seed None = one draw from torch's default generator."""
+        (seed, step t), seed None = one draw from torch's default generator.
+        num_beams > 1: beam search (beam_search; its chosen hypothesis' ids), stop_ids at most [eos_token_id], stop_fn then
+        receives the k running beams' new ids."""
+        if self._beam_args(num_beams, temperature, stop_ids, eos_token_id, early_stopping):
+            return self.beam_search([(input_ids, image, object_crops, images_long, objects_long)], num_beams, max_new_tokens,
+                                    eos_token_id, length_penalty, early_stopping, stop_fn)[0][0]
         sampler = self._sampler(temperature, top_k, top_p, None if seed is None else [seed])
         x = self.build_embeds(input_ids, image, object_crops, images_long, objects_long)
         T = x.shape[0]
@@ -266,16 +282,17 @@ class VQAEngine(LlamaClipCore):
         return out
 
     # ------------------------------------------------------------------ continuous-batched greedy decode (SURVEY.md §8f-1)
-    def prefill_ragged(self, xs, reserve=0):
+    def prefill_ragged(self, xs, reserve=0, slots=0):
         """xs: list of [T_b, d] input embeddings (consumed).  Sequences are LEFT-padded in the shared cache: sequence b
         occupies cache rows [Tpad - T_b, Tpad) of batch slot b, so every sequence ends at the same row and one decode
         step is ONE set of kernels for the whole batch (each weight byte read once for B tokens).  Runs of neighbouring
         sequences of EQUAL length are prefilled as one batch (M = G * T rows) - generate_batch orders its requests by length.
+        slots: cache slots to hold (at least B; beam search keeps its other beams on slots B..).
         -> (last-position logits fp32 [B, V], Tpad, lengths)"""
         B = len(xs)
         lens = [int(x.shape[0]) for x in xs]
         Tpad = max(lens)
-        self._ensure_cache(B, self._capacity(Tpad + reserve))
+        self._ensure_cache(max(B, slots), self._capacity(Tpad + reserve))
         self._prefix_slots = 0
         Tm = self._cache_shape[2]
         last = []
@@ -307,11 +324,14 @@ class VQAEngine(LlamaClipCore):
         return ops.gemm(hn, self.w.lm_head, out_dtype=torch.float32)
 
     def generate_batch(self, requests, max_new_tokens=200, eos_token_id=2, stop_ids=None, temperature=0, top_k=DEFAULT_TOP_K, top_p=None,
-                       seeds=None):
+                       seeds=None, num_beams=1, length_penalty=DEFAULT_LENGTH_PENALTY, early_stopping=DEFAULT_EARLY_STOPPING):
         """greedy generation for several (input_ids, image, object_crops, images_long, objects_long) requests at once.
         Same per-sequence semantics as generate(); finished sequences idle (their slots keep stepping, results ignored).
         temperature > 0: sampled decoding as in generate(), request i with seeds[i] (None = one default-generator draw per
-        request, in request order).  -> list of new-token lists"""
+        request, in request order).  num_beams > 1: beam search as in generate(), every request on its own k slots.
+        -> list of new-token lists"""
+        if self._beam_args(num_beams, temperature, stop_ids, eos_token_id, early_stopping):
+            return [ids for ids, _ in self.beam_search(requests, num_beams, max_new_tokens, eos_token_id, length_penalty, early_stopping)]
         if temperature is not None and temperature > 0 and seeds is None:
             seeds = draw_seeds(len(requests))
         xs = self.build_embeds_batch(list(requests))           # one CLIP + projector pass for every image of the batch
@@ -337,6 +357,95 @@ class VQAEngine(LlamaClipCore):
         res = [None] * B
         for k, i in enumerate(perm):
             res[i] = outs[k]
+        return res
+
+    def _beam_args(self, num_beams, temperature, stop_ids, eos_token_id, early_stopping):
+        """True when the call runs beam search (num_beams > 1); raises on the combinations beam search does not serve"""
+        check_beams(num_beams, early_stopping)
+        if num_beams == 1:
+            return False
+        if temperature is not None and temperature > 0:
+            raise NotImplementedError("num_beams > 1 with temperature > 0 (HF beam_sample) is not implemented")
+        if stop_ids and list(stop_ids) != [eos_token_id]:
+            raise ValueError(f"with num_beams > 1 the only stop sequence is eos ([{eos_token_id}]), got {list(stop_ids)}")
+        return True
+
+    def beam_search(self, requests, num_beams, max_new_tokens=200, eos_token_id=2, length_penalty=DEFAULT_LENGTH_PENALTY,
+                    early_stopping=DEFAULT_EARLY_STOPPING, stop_fn=None, on_step=None):
+        """HF `beam_search` (transformers 4.31, one returned sequence) for several (input_ids, image, object_crops, images_long,
+        objects_long) requests at once -> [(new token ids, score of the chosen hypothesis)], the ids as the reference's
+        generate(num_beams=k) returns them after the prompt (the hypothesis, then eos if it is shorter than max_length).
+
+        Request r is prefilled once (left-padded as in generate_batch) and its prompt rows are copied to its k - 1 other cache
+        slots; every step then decodes all R * k slots in one decode_ragged call.  One vsb_beam_candidates_f32 launch selects
+        each request's 2k candidates, one copy brings them to the host, and vstar_b200.beam applies the scorer.  Beams move by
+        copy-on-fork: a surviving parent keeps its slot for its first child, later children take the slots of beams that died
+        and get the parent's generated rows [Tpad, Tpad + step) by one vsb_copy_cache_rows_b16 launch, so no launch reads a
+        slot it writes.  stop_fn(running beams' new ids, k lists in beam order) -> bool ends the search (HF stopping
+        criteria, called after every step); requests that are done idle.  on_step(step, logits, slots, beams): observes every
+        step's logits fp32 [*, V] with, per request in order of length, its beams' logits rows and new ids (tests replay it)."""
+        check_beams(num_beams, early_stopping)
+        k = num_beams
+        dev = self.dev
+        xs = self.build_embeds_batch(list(requests))
+        perm = sorted(range(len(xs)), key=lambda i: int(xs[i].shape[0]))
+        xs = [xs[i] for i in perm]
+        R = len(xs)
+        reqs = [BeamRequest(k, len(requests[i][0]), max_new_tokens, eos_token_id, length_penalty, early_stopping) for i in perm]
+        longest = max(int(x.shape[0]) for x in xs)
+        logits, Tpad, lens = self.prefill_ragged(xs, reserve=max(0, min(max_new_tokens, self.MAX_POSITIONS - longest)), slots=R * k)
+        # request r: beam 0 on slot r (prefilled), slots R + r*(k-1) .. for its other beams
+        owned = [[r] + [R + r * (k - 1) + j for j in range(k - 1)] for r in range(R)]
+        if k > 1:
+            ops.copy_cache_rows(self._cache, [(r, s) for r in range(R) for s in owned[r][1:]], 0, Tpad)
+        slot_lens = [0] * (R * k)
+        for r in range(R):
+            for s in owned[r]:
+                slot_lens[s] = lens[r]
+        beam_slot = [[r] for r in range(R)]                 # logical beam -> cache slot (logits row) per request
+        tokens = [0] * (R * k)
+        host = torch.empty(2 * R * k, dtype=torch.int32).pin_memory()
+        cand = torch.empty((3, R, 2 * k), dtype=torch.int32, device=dev)
+        for step in range(max_new_tokens):
+            k_in = len(beam_slot[0])
+            n = R * k_in
+            host[:n] = torch.tensor([s for bs in beam_slot for s in bs], dtype=torch.int32)
+            host[n:2 * n].view(torch.float32)[:] = torch.tensor([x for q in reqs for x in q.scores], dtype=torch.float32)
+            if on_step is not None:
+                on_step(step, logits, [list(bs) for bs in beam_slot], [[list(b) for b in q.beams] for q in reqs])
+            up = host[:2 * n].to(dev, non_blocking=True)
+            ops.beam_candidates(logits, up[:n].view(R, k_in), up[n:].view(torch.float32).view(R, k_in), k, self.dtype, out=cand)
+            c = cand.cpu()                                  # the one device-to-host copy of the step
+            sc, tok, bm = c[0].view(torch.float32).tolist(), c[1].tolist(), c[2].tolist()
+            pairs = []
+            for r, q in enumerate(reqs):
+                if q.done:
+                    continue
+                nxt = q.process(list(zip(sc[r], tok[r], bm[r])))
+                old = beam_slot[r]
+                parents = {b for _, _, b in nxt}
+                free = [s for s in owned[r] if s not in {old[p] for p in parents}]
+                new, claimed = [], set()
+                for _, t, p in nxt:
+                    if p not in claimed:                    # the parent's first child keeps its slot
+                        claimed.add(p)
+                        s = old[p]
+                    else:                                   # later children fork into the slot of a beam that died
+                        s = free.pop(0)
+                        pairs.append((old[p], s))
+                    new.append(s)
+                    tokens[s] = t
+                beam_slot[r] = new
+            if all(q.done for q in reqs) or step == max_new_tokens - 1:
+                break
+            if stop_fn is not None and any(not q.done and stop_fn([list(b) for b in q.beams]) for q in reqs):
+                break
+            if pairs and step > 0:
+                ops.copy_cache_rows(self._cache, pairs, Tpad, Tpad + step)
+            logits = self.decode_ragged(tokens, slot_lens, Tpad, step)
+        res = [None] * R
+        for r, i in enumerate(perm):
+            res[i] = reqs[r].finalize()
         return res
 
     def option_losses(self, question_ids, options_ids, image, object_crops=None, images_long=None, objects_long=None):
@@ -478,6 +587,8 @@ class LlavaSearchModel:
         self.eos_token_id = eos_token_id
         self.device = torch.device(engine.dev)
         self.top_k = DEFAULT_TOP_K                      # the top_k VQA_LLM samples with (generation_config.json's, if any)
+        self.length_penalty = DEFAULT_LENGTH_PENALTY    # beam-search settings (generation_config.json's, if any)
+        self.early_stopping = DEFAULT_EARLY_STOPPING
 
     def eval(self):
         return self
@@ -492,17 +603,26 @@ class LlavaSearchModel:
 
     @torch.inference_mode()
     def generate(self, input_ids, images=None, object_features=None, images_long=None, objects_long=None, do_sample=False, num_beams=1,
-                 temperature=0, top_p=None, max_new_tokens=200, use_cache=True, stopping_criteria=None, **_):
-        if do_sample or num_beams != 1:
+                 temperature=0, top_p=None, max_new_tokens=200, use_cache=True, stopping_criteria=None, length_penalty=None,
+                 early_stopping=None, **_):
+        """greedy decoding, or beam search with num_beams > 1 (HF's output: prompt ids + the chosen hypothesis + eos when it is
+        shorter than max_length; stopping_criteria see the k running beams as a [k, len] tensor in beam order, as HF's do).
+        length_penalty / early_stopping None: the checkpoint's generation_config.json values (else the 4.31 defaults)."""
+        if do_sample:
             raise NotImplementedError("greedy decoding only (vstar_bench_eval.py:196 runs temperature=0, num_beams=1)")
+        check_beams(num_beams, self.early_stopping if early_stopping is None else early_stopping)
         ids = input_ids.view(-1).tolist()
         stop_fn = None
         if stopping_criteria:
             def stop_fn(new):
-                full = torch.tensor([ids + list(new)], dtype=torch.int64)
+                new = [list(new)] if num_beams == 1 else new
+                full = torch.tensor([ids + list(b) for b in new], dtype=torch.int64)
                 return any(bool(sc(full, None)) for sc in stopping_criteria)
+        beam = {} if num_beams == 1 else dict(
+            num_beams=num_beams, length_penalty=self.length_penalty if length_penalty is None else length_penalty,
+            early_stopping=self.early_stopping if early_stopping is None else early_stopping)
         new = self.engine.generate(ids, self._px(images), self._px(object_features), images_long, objects_long, max_new_tokens,
-                                   self.eos_token_id, stop_fn=stop_fn)
+                                   self.eos_token_id, stop_fn=stop_fn, **beam)
         return torch.cat([input_ids.view(1, -1).cpu(), torch.tensor([new], dtype=torch.int64)], dim=1).to(input_ids.device)
 
     @torch.inference_mode()
@@ -546,7 +666,7 @@ def load_pretrained_model(model_path, model_base=None, model_name=None, load_8bi
     engine = VQAEngine(VQAWeights(cfg, open_checkpoint(model_path, device=device), device=device, dtype=dtype,
                                   quant="nf4" if load_4bit else None))
     model = LlavaSearchModel(engine, getattr(tokenizer, "eos_token_id", 2))
-    model.top_k = generation_top_k(model_path)
+    model.top_k, model.length_penalty, model.early_stopping = generation_top_k(model_path, beams=True)
     return tokenizer, model, _Proc(), 2048
 
 
@@ -564,6 +684,7 @@ class VQA_LLM:
                 args.vqa_model_path, None, None, load_4bit=load_4bit, torch_dtype=None if load_4bit else VQA_DTYPES[name])
             self.engine = self.model.engine
             self.top_k = self.model.top_k
+            self.length_penalty, self.early_stopping = self.model.length_penalty, self.model.early_stopping
             self.conv_type = getattr(args, "conv_type", "v1")
             self.eos = getattr(self.tokenizer, "eos_token_id", 2)
             return
@@ -573,6 +694,7 @@ class VQA_LLM:
         self.image_processor = _Proc()
         self.context_len = 2048
         self.top_k = DEFAULT_TOP_K
+        self.length_penalty, self.early_stopping = DEFAULT_LENGTH_PENALTY, DEFAULT_EARLY_STOPPING
         self.conv_type = conv_type
         self.eos = getattr(self.tokenizer, "eos_token_id", 2)
 
@@ -655,10 +777,14 @@ class VQA_LLM:
     def free_form_inference(self, image, question, temperature=0, top_p=None, num_beams=1, max_new_tokens=200, object_crops=None,
                             images_long=None, objects_long=None):
         """temperature > 0 samples (the reference's do_sample = temperature > 0, vstar_bench_eval.py:97) with top_k = self.top_k
-        and top_p; the request takes one seed from torch's default generator"""
+        and top_p; the request takes one seed from torch's default generator.  num_beams > 1: beam search with
+        self.length_penalty / self.early_stopping; eos ends a hypothesis, and no other stopping criterion applies (the
+        v1 stop keyword "</s>" is eos; the reference's KeywordsStoppingCriteria would assert on k beams, INTEGRATION.md)"""
         sample = temperature is not None and temperature > 0
         if sample:
             check_sampling(self.top_k, top_p)
+        if num_beams != 1:
+            return self._beam_texts([(image, question, object_crops, images_long, objects_long)], num_beams, max_new_tokens, temperature)[0]
         prompt = build_prompt_v1(DEFAULT_IMAGE_TOKEN + "\n" + question)
         stop_str = "</s>"
         ids = tokenizer_image_object_token(prompt, self.tokenizer)
@@ -675,15 +801,39 @@ class VQA_LLM:
         return text.strip()
 
     @torch.inference_mode()
-    def free_form_inference_batch(self, images, questions, max_new_tokens=200, originals=None, temperature=0, top_p=None):
+    def _beam_texts(self, items, num_beams, max_new_tokens, temperature):
+        """items: [(image, question, object_crops, images_long, objects_long)] -> decoded best hypotheses"""
+        stop_str = "</s>"
+        reqs = []
+        for image, question, crops, il, ol in items:
+            ids = tokenizer_image_object_token(build_prompt_v1(DEFAULT_IMAGE_TOKEN + "\n" + question), self.tokenizer)
+            img, crops = self._pixels(image, crops)
+            reqs.append((ids, img, crops, il, ol))
+        outs = self.engine.generate_batch(reqs, max_new_tokens, self.eos, temperature=temperature, num_beams=num_beams,
+                                          length_penalty=self.length_penalty, early_stopping=self.early_stopping)
+        texts = []
+        for out in outs:
+            text = self.tokenizer.batch_decode([out], skip_special_tokens=True)[0].strip()
+            if text.endswith(stop_str):
+                text = text[:-len(stop_str)]
+            texts.append(text.strip())
+        return texts
+
+    def free_form_inference_batch(self, images, questions, max_new_tokens=200, originals=None, temperature=0, top_p=None, num_beams=1):
         """free_form_inference for several (image, question) pairs in ONE continuous-batched decode (not in the reference,
         which answers one image at a time, vstar_bench_eval.py:196): same prompt, stop string and post-processing per
         sample; each decode step reads the 7B weights once for the whole batch.  originals: the un-padded images the padded
         `images` were made from; with `use_device_images` the pixels are then produced on the GPU (bit-identical).
-        temperature / top_p as in free_form_inference; each request takes one seed from torch's default generator, in order."""
+        temperature / top_p as in free_form_inference; each request takes one seed from torch's default generator, in order.
+        num_beams > 1: beam search per request as in free_form_inference, all requests in one decode."""
         sample = temperature is not None and temperature > 0
         if sample:
             check_sampling(self.top_k, top_p)
+        if num_beams != 1:
+            if originals is not None and self._img_src is not None:
+                images = [self.device_pixels(o, None)[0] for o in originals]
+            return self._beam_texts([(im, q, None, None, None) for im, q in zip(images, questions)], num_beams, max_new_tokens,
+                                    temperature)
         stop_str = "</s>"
         kw = self.tokenizer(stop_str).input_ids
         if len(kw) > 1 and kw[0] == self.tokenizer.bos_token_id:
