@@ -217,6 +217,28 @@ int vsb_llama_layers_f16(const vsb_llama_layer_t* layers, int n_layers, void* x,
                          const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded, void* scratch,
                          void* deq_scratch, void* stream);
 
+/* Slot decode: one new token for each of B sequences that sit at their OWN cache slot and length, so a decode batch can admit a
+ * sequence whenever another one ends (VQAEngine.decode_stream).  slot_i32 / len_i32 / pos_i32: device int32 [B]: row b's cache slot
+ * (< Bc, distinct), the rows already cached in it (its new q|k|v row is written at slot*Tmax + len) and its RoPE position.
+ * max_len >= every len[b] (< Tmax) sizes the attention launch.  Same per-layer sequence and weight tables (dense or NF4) as
+ * vsb_llama_layers with Tn = 1, with the QKV projection written to scratch, placed by vsb_rope_scatter and attended by
+ * vsb_attn_decode_slots.  scratch: B*(5d+inter) elements; batch-invariant mode as in vsb_llama_layers.  The three slot-decode
+ * entry points take the element type as an argument, dtype = VSB_DTYPE_BF16 or VSB_DTYPE_F16 (f16 and NF4 tables). */
+int vsb_llama_layers_slots(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, void* cache, int Bc, int Tmax, int d, int H,
+                           int inter, float rms_eps, const void* rope_cos, const void* rope_sin, const void* slot_i32, const void* len_i32,
+                           const void* pos_i32, int max_len, int norm_folded, void* scratch, void* deq_scratch, int dtype, void* stream);
+/* Row b of qkv [B, 3*H*D] (row stride ldq) to cache row slot_i32[b]*Tmax + len_i32[b] (row stride ldc): q and k rotated at position
+ * pos_i32[b] with the arithmetic of vsb_rope_bf16 / vsb_rope_f16, v copied. */
+int vsb_rope_scatter(const void* qkv, long long ldq, int B, int H, int D, void* cache, long long ldc, int Tmax, const void* slot_i32,
+                     const void* len_i32, const void* pos_i32, const void* cos_table, const void* sin_table, int dtype, void* stream);
+/* Decode attention over per-row slots and lengths: row b's query is at q + slot[b]*slot_stride + len[b]*row_stride, and it attends
+ * keys / values [0, len[b]] of its slot (k/v + slot[b]*slot_stride + j*row_stride); output o + b*o_rs.  Cluster split-KV as
+ * vsb_attn_decode_bf16, with each row's split chosen from its own key count (in batch-invariant mode from nothing else).  In the
+ * default mode, with equal lengths and slot[b] = b, it is bit-identical to vsb_attn_decode_bf16 / _f16 (Sq = 1, k_start NULL);
+ * in batch-invariant mode it may split differently (vsb_attn_decode_* keeps its batch-size term there).  max_len >= every len[b]. */
+int vsb_attn_decode_slots(const void* q, const void* k, const void* v, void* o, long long slot_stride, long long row_stride, long long o_rs,
+                          int B, int H, int D, float scale, const void* slot_i32, const void* len_i32, int max_len, int dtype, void* stream);
+
 /* NF4 weights: the SEAL VQA LLM's 4-bit mode (the reference's load_4bit: bitsandbytes NF4, double-quantised scales, fp16 compute,
  * LLaVA/llava/model/builder.py:26-43).  Format of W [N, K], K % 64 == 0 (csrc/nf4.cu, oracle/nf4_oracle.py): codes u8 [N, K/2], two
  * 4-bit codes per byte with the first element in the high nibble, one fp32 scale per 64-value block [N, K/64]; a weight is

@@ -77,6 +77,13 @@ SIGNATURES.update({
     "vsb_gemm_nf4": [c_p, c_ll, c_p, c_p, c_p, c_ll, c_i, c_i, c_i, c_p, c_p, c_ll, c_i, c_i, c_i, c_ll, c_ll, c_p, c_p],
 })
 
+# slot decode (VQAEngine.decode_stream): every row at its own cache slot and length; the element type is an argument
+SIGNATURES.update({
+    "vsb_llama_layers_slots": [c_p, c_i, c_p, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_i, c_p],
+    "vsb_rope_scatter": [c_p, c_ll, c_i, c_i, c_i, c_p, c_ll, c_i, c_p, c_p, c_p, c_p, c_p, c_i, c_p],
+    "vsb_attn_decode_slots": [c_p, c_p, c_p, c_p, c_ll, c_ll, c_ll, c_i, c_i, c_i, c_f, c_p, c_p, c_i, c_i, c_p],
+})
+
 
 class LlamaLayer(ctypes.Structure):
     """vsb_llama_layer_t"""

@@ -504,6 +504,179 @@ static int launch_decode(const AttnParams& p, cudaStream_t st) {
   return VSB_OK;
 }
 
+// ------------------------------------------------------------------ decode attention over per-row cache slots and lengths
+// A decode batch whose rows were admitted at different times: row b owns cache slot slot[b] and has len[b] cached rows; its
+// query is the row the QKV step has just written, slot[b]*slot_stride + len[b]*row_stride, and it attends keys [0, len[b]] of
+// its slot.  The kernel above with Sq = 1, except that the split of a row comes from its OWN key count: launch_decode's rule
+// for Sk = len[b] + 1, with the batch-size term folded into `cap` on the host (dropped in batch-invariant mode, so a row's
+// result depends on nothing but its own keys).  Surplus CTAs of the cluster stream no keys and rank 0 combines only the
+// row's own splits, in rank order: in the default mode, with equal lengths and slot[b] = b, this is vsb_attn_decode_* with
+// k_start = 0, bit for bit (in batch-invariant mode vsb_attn_decode_* keeps the batch-size term, so the splits may differ).
+struct SlotAttnParams {
+  const void *q, *k, *v;
+  void* o;
+  long long slot_stride, row_stride, o_rs;
+  const int *slot, *len;
+  float scale_log2;
+  int cap;                       // largest split the batch-size term of launch_decode allows (1..8)
+};
+
+__device__ __forceinline__ int dec_row_splits(int nk, int cap) {
+  int s = cap;
+  while (s > 1 && nk / s < 64) s >>= 1;
+  return s;
+}
+
+template <int D, typename T>
+__global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_slots_kernel(const SlotAttnParams p) {
+  using E = ElemT<T>;
+  pdl_prologue();
+  constexpr int EPL = D / 32;
+  cg::cluster_group cluster = cg::this_cluster();
+  const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __shared__ float s_m[DEC_WARPS], s_l[DEC_WARPS];
+  __shared__ float s_acc[DEC_WARPS][D];
+  __shared__ float c_m, c_l;
+  __shared__ float c_acc[D];
+
+  const int len = p.len[b];
+  const int nk = len + 1;
+  const int nsplit = min(dec_row_splits(nk, p.cap), (int)gridDim.x);
+  const int chunk = (nk + nsplit - 1) / nsplit;
+  const int k_begin = split < nsplit ? split * chunk : nk;
+  const int k_end = min(nk, k_begin + chunk);
+  const long long base = (long long)p.slot[b] * p.slot_stride + (long long)h * D + lane * EPL;
+  const T* qb = reinterpret_cast<const T*>(p.q) + base + (long long)len * p.row_stride;
+  const T* kb = reinterpret_cast<const T*>(p.k) + base;
+  const T* vb = reinterpret_cast<const T*>(p.v) + base;
+
+  float q[EPL], acc[EPL], m = -INFINITY, l = 0.f;
+#pragma unroll
+  for (int e = 0; e < EPL; ++e) {
+    acc[e] = 0.f;
+    q[e] = E::to_f(qb[e]) * p.scale_log2;
+  }
+  for (int j0 = k_begin + warp; j0 < k_end; j0 += DEC_WARPS * DEC_U) {
+    uint32_t kr[DEC_U][EPL / 2], vr[DEC_U][EPL / 2];
+#pragma unroll
+    for (int u = 0; u < DEC_U; ++u) {
+      const int j = j0 + u * DEC_WARPS;
+      if (j < k_end) {
+        if (EPL == 4) {
+          const uint2 k2 = *reinterpret_cast<const uint2*>(kb + (long long)j * p.row_stride);
+          const uint2 v2 = *reinterpret_cast<const uint2*>(vb + (long long)j * p.row_stride);
+          kr[u][0] = k2.x; kr[u][(EPL / 2) - 1] = k2.y;
+          vr[u][0] = v2.x; vr[u][(EPL / 2) - 1] = v2.y;
+        } else {
+          kr[u][0] = *reinterpret_cast<const uint32_t*>(kb + (long long)j * p.row_stride);
+          vr[u][0] = *reinterpret_cast<const uint32_t*>(vb + (long long)j * p.row_stride);
+        }
+      } else {
+#pragma unroll
+        for (int e = 0; e < EPL / 2; ++e) kr[u][e] = vr[u][e] = 0u;
+      }
+    }
+    float sc[DEC_U];
+    float mx = m;
+#pragma unroll
+    for (int u = 0; u < DEC_U; ++u) {
+      float d = 0.f;
+#pragma unroll
+      for (int e = 0; e < EPL / 2; ++e) {
+        const float2 kk = E::unpack2(kr[u][e]);
+        d = fmaf(q[2 * e], kk.x, d);
+        d = fmaf(q[2 * e + 1], kk.y, d);
+      }
+      d = warp_sum(d);
+      sc[u] = (j0 + u * DEC_WARPS < k_end) ? d : -INFINITY;
+      mx = fmaxf(mx, sc[u]);
+    }
+    if (mx != -INFINITY) {
+      const float corr = exp2f(m - mx);
+      m = mx;
+      float ls = 0.f;
+#pragma unroll
+      for (int e = 0; e < EPL; ++e) acc[e] *= corr;
+#pragma unroll
+      for (int u = 0; u < DEC_U; ++u) {
+        const float pr = exp2f(sc[u] - mx);
+        ls += pr;
+#pragma unroll
+        for (int e = 0; e < EPL / 2; ++e) {
+          const float2 vv = E::unpack2(vr[u][e]);
+          acc[2 * e] = fmaf(pr, vv.x, acc[2 * e]);
+          acc[2 * e + 1] = fmaf(pr, vv.y, acc[2 * e + 1]);
+        }
+      }
+      l = l * corr + ls;
+    }
+  }
+  // warps -> CTA partial -> rank 0, in the order of attn_decode_kernel
+  if (lane == 0) { s_m[warp] = m; s_l[warp] = l; }
+#pragma unroll
+  for (int e = 0; e < EPL; ++e) s_acc[warp][lane * EPL + e] = acc[e];
+  __syncthreads();
+  for (int d = threadIdx.x; d < D; d += DEC_WARPS * 32) {
+    float M = -INFINITY;
+#pragma unroll
+    for (int w = 0; w < DEC_WARPS; ++w) M = fmaxf(M, s_m[w]);
+    float a = 0.f, ll = 0.f;
+#pragma unroll
+    for (int w = 0; w < DEC_WARPS; ++w) {
+      const float f = (s_m[w] == -INFINITY) ? 0.f : exp2f(s_m[w] - M);
+      a += s_acc[w][d] * f;
+      ll += s_l[w] * f;
+    }
+    c_acc[d] = a;
+    if (d == 0) { c_m = M; c_l = ll; }
+  }
+  cluster.sync();
+  if (cluster.block_rank() == 0) {
+    for (int d = threadIdx.x; d < D; d += DEC_WARPS * 32) {
+      float M = -INFINITY;
+      for (int r = 0; r < nsplit; ++r) M = fmaxf(M, *cluster.map_shared_rank(&c_m, r));
+      float a = 0.f, ll = 0.f;
+      for (int r = 0; r < nsplit; ++r) {
+        const float mr = *cluster.map_shared_rank(&c_m, r);
+        const float f = (mr == -INFINITY) ? 0.f : exp2f(mr - M);
+        a += *cluster.map_shared_rank(&c_acc[d], r) * f;
+        ll += *cluster.map_shared_rank(&c_l, r) * f;
+      }
+      reinterpret_cast<T*>(p.o)[(long long)b * p.o_rs + (long long)h * D + d] = E::from_f(ll > 0.f ? a / ll : 0.f);
+    }
+  }
+  cluster.sync();
+}
+
+template <typename T>
+static int attn_decode_slots(const void* q, const void* k, const void* v, void* o, long long slot_stride, long long row_stride, long long o_rs,
+                             int B, int H, int D, float scale, const void* slot, const void* len, int max_len, void* stream) {
+  VSB_CHECK_ARG(q && k && v && o && slot && len, "vsb_attn_decode_slots: null pointer");
+  VSB_CHECK_ARG(D == 64 || D == 128, "vsb_attn_decode_slots: head_dim %d unsupported (64/128)", D);
+  VSB_CHECK_ARG(B > 0 && H > 0 && max_len >= 0, "vsb_attn_decode_slots: bad shape (B=%d, H=%d, max_len=%d)", B, H, max_len);
+  VSB_CHECK_ARG(slot_stride % 4 == 0 && row_stride % 4 == 0 && ((uintptr_t)q & 7) == 0 && ((uintptr_t)k & 7) == 0 && ((uintptr_t)v & 7) == 0,
+                "vsb_attn_decode_slots: q/k/v must be 8-byte aligned with strides that are multiples of 4 elements");
+  SlotAttnParams p;
+  p.q = q; p.k = k; p.v = v; p.o = o;
+  p.slot_stride = slot_stride; p.row_stride = row_stride; p.o_rs = o_rs;
+  p.slot = reinterpret_cast<const int*>(slot); p.len = reinterpret_cast<const int*>(len);
+  p.scale_log2 = scale * 1.4426950408889634f;
+  // launch_decode's rule, split into its batch-size term (cap) and its key-count term (per row in the kernel; here for the
+  // longest row, which sizes the cluster)
+  p.cap = DEC_SPLITS;
+  if (!vsb_batch_invariant())
+    while (p.cap > 1 && (long long)p.cap * H * B > 2LL * vsb_num_sms() + H) p.cap >>= 1;
+  int splits = p.cap;
+  while (splits > 1 && (max_len + 1) / splits < 64) splits >>= 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (D == 64)
+    VSB_CUDA(vsb_launch_pdl(attn_decode_slots_kernel<64, T>, dim3(splits, H, B), dim3(DEC_WARPS * 32), 0, st, splits, p));
+  else
+    VSB_CUDA(vsb_launch_pdl(attn_decode_slots_kernel<128, T>, dim3(splits, H, B), dim3(DEC_WARPS * 32), 0, st, splits, p));
+  return VSB_OK;
+}
+
 void vsb_attn_tc_set_variant(int v);
 static int g_attn_impl = 0;   // 0 auto, 1 = mma.sync kernel, 2 = wgmma kernel, 3 = wgmma kernel with one query warpgroup per CTA, 4 = decode kernel
 extern "C" int vsb_attn_set_impl(int impl) {
@@ -641,6 +814,14 @@ VSB_ATTN_ENTRY(vsb_flash_attn_f16, flash_attn, half)
   }
 VSB_ATTN_DECODE_ENTRY(vsb_attn_decode_bf16, bf16)
 VSB_ATTN_DECODE_ENTRY(vsb_attn_decode_f16, half)
+
+extern "C" int vsb_attn_decode_slots(const void* q, const void* k, const void* v, void* o, long long slot_stride, long long row_stride,
+                                     long long o_rs, int B, int H, int D, float scale, const void* slot_i32, const void* len_i32, int max_len,
+                                     int dtype, void* stream) {
+  VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_attn_decode_slots: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)", dtype);
+  return dtype == VSB_DTYPE_F16 ? attn_decode_slots<half>(q, k, v, o, slot_stride, row_stride, o_rs, B, H, D, scale, slot_i32, len_i32, max_len, stream)
+                                : attn_decode_slots<bf16>(q, k, v, o, slot_stride, row_stride, o_rs, B, H, D, scale, slot_i32, len_i32, max_len, stream);
+}
 
 #define VSB_ATTN_SEG_ENTRY(NAME, T)                                                                                                \
   extern "C" int NAME(const void* q, const void* k, const void* v, void* o, long long q_bs, long long q_rs, long long k_bs,        \

@@ -208,6 +208,47 @@ __global__ void rope_kernel(E_T* __restrict__ qkv, long long ld, int rows, int T
   }
 }
 
+// RoPE + scatter of one fused q|k|v row per decode row into the KV cache: row b of qkv goes to cache row
+// slot[b]*Tmax + len[b] with q and k rotated at position pos[b] (the arithmetic of rope_kernel) and v copied, so every row of a
+// decode batch can sit at its own slot and length.
+template <typename E_T>
+__global__ void rope_scatter_kernel(const E_T* __restrict__ qkv, long long ldq, int H, int D, E_T* __restrict__ cache, long long ldc,
+                                    int Tmax, const int* __restrict__ slot, const int* __restrict__ len, const int* __restrict__ positions,
+                                    const E_T* __restrict__ cos_t, const E_T* __restrict__ sin_t) {
+  using E = ElemT<E_T>;
+  pdl_prologue();
+  const int row = blockIdx.x;
+  const int pos = positions[row];
+  const int half = D >> 1;
+  const int hv = half >> 3;
+  const E_T* src = qkv + (long long)row * ldq;
+  E_T* dst = cache + ((long long)slot[row] * Tmax + len[row]) * ldc;
+  const E_T* cr = cos_t + (long long)pos * half;
+  const E_T* sr = sin_t + (long long)pos * half;
+  for (int idx = threadIdx.x; idx < 2 * H * hv; idx += blockDim.x) {
+    const int hh = idx / hv;
+    const int v = idx - hh * hv;
+    const long long o = (long long)hh * D + v * 8;
+    const uint4 a = *reinterpret_cast<const uint4*>(src + o);
+    const uint4 b = *reinterpret_cast<const uint4*>(src + o + half);
+    const uint4 c = __ldg(reinterpret_cast<const uint4*>(cr + v * 8));
+    const uint4 s = __ldg(reinterpret_cast<const uint4*>(sr + v * 8));
+    const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w}, cw[4] = {c.x, c.y, c.z, c.w}, sw[4] = {s.x, s.y, s.z, s.w};
+    uint32_t oa[4], ob[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 x1 = E::unpack2(aw[j]), x2 = E::unpack2(bw[j]), cs = E::unpack2(cw[j]), sn = E::unpack2(sw[j]);
+      oa[j] = E::pack2(E::round(x1.x * cs.x) + E::round(-x2.x * sn.x), E::round(x1.y * cs.y) + E::round(-x2.y * sn.y));
+      ob[j] = E::pack2(E::round(x2.x * cs.x) + E::round(x1.x * sn.x), E::round(x2.y * cs.y) + E::round(x1.y * sn.y));
+    }
+    *reinterpret_cast<uint4*>(dst + o) = make_uint4(oa[0], oa[1], oa[2], oa[3]);
+    *reinterpret_cast<uint4*>(dst + o + half) = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+  }
+  const int d = H * D;
+  for (int i = threadIdx.x * 8; i < d; i += blockDim.x * 8)
+    *reinterpret_cast<uint4*>(dst + 2 * d + i) = *reinterpret_cast<const uint4*>(src + 2 * d + i);
+}
+
 // ------------------------------------------------------------------ embedding splice
 // out[b, t, :] = table[ids[b, t']] for text positions; image rows are left untouched (the
 // mm_projector GEMM writes them directly through its row remap).  ids layout [B, L] with
@@ -483,6 +524,25 @@ static int rope(void* qkv, long long ld, int rows, int T, int H, int D, int pos0
   VSB_CUDA(vsb_launch_pdl(rope_kernel<E_T>, dim3(rows), dim3(256), 0, STREAM(stream), 1, (E_T*)qkv, ld, rows, T, H, D, pos0,
                           (const E_T*)cos_table, (const E_T*)sin_table, (const int*)positions, group_stride, group_offset));
   return VSB_OK;
+}
+
+template <typename E_T>
+static int rope_scatter(const void* qkv, long long ldq, int B, int H, int D, void* cache, long long ldc, int Tmax, const void* slot,
+                        const void* len, const void* positions, const void* cos_table, const void* sin_table, void* stream) {
+  VSB_CHECK_ARG(qkv && cache && slot && len && positions && cos_table && sin_table, "vsb_rope_scatter: null pointer");
+  VSB_CHECK_ARG(B >= 0 && H > 0 && Tmax > 0 && D % 16 == 0 && ldq % 8 == 0 && ldc % 8 == 0 && ldq >= 3LL * H * D && ldc >= 3LL * H * D,
+                "vsb_rope_scatter: bad args (D %% 16, ld %% 8, ld >= 3*H*D)");
+  if (B == 0) return VSB_OK;
+  VSB_CUDA(vsb_launch_pdl(rope_scatter_kernel<E_T>, dim3(B), dim3(256), 0, STREAM(stream), 1, (const E_T*)qkv, ldq, H, D, (E_T*)cache, ldc,
+                          Tmax, (const int*)slot, (const int*)len, (const int*)positions, (const E_T*)cos_table, (const E_T*)sin_table));
+  return VSB_OK;
+}
+
+extern "C" int vsb_rope_scatter(const void* qkv, long long ldq, int B, int H, int D, void* cache, long long ldc, int Tmax, const void* slot_i32,
+                                const void* len_i32, const void* pos_i32, const void* cos_table, const void* sin_table, int dtype, void* stream) {
+  VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_rope_scatter: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)", dtype);
+  return dtype == VSB_DTYPE_F16 ? rope_scatter<half>(qkv, ldq, B, H, D, cache, ldc, Tmax, slot_i32, len_i32, pos_i32, cos_table, sin_table, stream)
+                                : rope_scatter<bf16>(qkv, ldq, B, H, D, cache, ldc, Tmax, slot_i32, len_i32, pos_i32, cos_table, sin_table, stream);
 }
 
 extern "C" int vsb_embed_splice_bf16(const void* ids, const void* table, void* out, int B, int L, int img_pos, int n_img, int d,

@@ -60,11 +60,18 @@ struct LayerOps<half> {
 
 int vsb_nf4_variant(int M);   // nf4.cu: 0 = the NF4 GEMM of M rows dequantises W and runs the tile kernels
 
+// slot decode (vsb_llama_layers_slots): one new row per sequence, each at its own cache slot and length
+struct SlotRows {
+  const void* slot;   // int32 [B] cache slot of row b
+  const void* len;    // int32 [B] rows already cached in that slot: the new row is written at slot*Tmax + len
+  int max_len;        // >= every len[b]
+};
+
 template <typename T>
 static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int Tn, int past, void* cache, int Bc,
                         int Tmax, int d, int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin,
                         const void* positions, const void* k_start, int tail_rows, const void* q_seg, int seg_lo, int norm_folded,
-                        void* scratch, void* deq_scratch, void* stream) {
+                        void* scratch, void* deq_scratch, void* stream, const SlotRows* slots = nullptr) {
   using K = LayerOps<T>;
   VSB_CHECK_ARG(layers && x && cache && rope_cos && rope_sin && scratch, "vsb_llama_layers: null pointer");
   VSB_CHECK_ARG(n_layers > 0 && B > 0 && Tn > 0 && past >= 0 && d > 0 && H > 0 && inter > 0, "vsb_llama_layers: bad shape");
@@ -72,6 +79,11 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
   VSB_CHECK_ARG(d % H == 0, "vsb_llama_layers: hidden %d not divisible by heads %d", d, H);
   VSB_CHECK_ARG(k_start == nullptr || Tn <= 4, "vsb_llama_layers: ragged batches (k_start) need Tn <= 4, got %d", Tn);
   VSB_CHECK_ARG(q_seg == nullptr || (k_start == nullptr && tail_rows == 0), "vsb_llama_layers: q_seg excludes k_start / tail_rows");
+  if (slots) {
+    VSB_CHECK_ARG(slots->slot && slots->len && positions, "vsb_llama_layers_slots: null slot / len / pos");
+    VSB_CHECK_ARG(slots->max_len >= 0 && slots->max_len < Tmax, "vsb_llama_layers_slots: max_len %d outside the %d cache rows of a slot",
+                  slots->max_len, Tmax);
+  }
   // weight format: NF4 codes where the block scales are set, dense weights where they are NULL
   const bool nf4 = layers[0].wqkv_scales != nullptr;
   for (int li = 0; li < n_layers; ++li) {
@@ -95,7 +107,7 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
   // tail mode: the caller consumes only the last `tail_rows` rows of every sequence (answer-predicting rows and the [LOC]
   // row of the guided search).  K/V of the last layer are needed by nobody else, so that layer runs its attention,
   // o-projection and MLP over B*tail rows only (same kernels, same per-row arithmetic => same values on those rows).
-  const bool tail = tail_rows > 0 && 2 * tail_rows <= Tn && k_start == nullptr && (hd == 64 || hd == 128);
+  const bool tail = tail_rows > 0 && 2 * tail_rows <= Tn && k_start == nullptr && slots == nullptr && (hd == 64 || hd == 128);
   // the projections of this call run on the wgmma tile kernels, whose epilogues alone fold RMSNorm and RoPE in (row counts
   // that take the skinny / weight-streaming decode kernels keep the separate RMSNorm and RoPE kernels)
   const bool tiles = nf4 ? vsb_nf4_variant((int)rows) == 0 : (rows > 16 || vsb_batch_invariant());
@@ -111,7 +123,7 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
     VSB_TRY(K::rowsq(xb, d, sq_a, (int)rows, d, stream));
   }
   // RoPE in the QKV epilogue (head_dim 128): q / k reach the cache already rotated
-  const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && tiles;
+  const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && slots == nullptr && tiles;
 
   // C [M, N] (leading dimension ldc) = epi(A W^T), A [M, Kd] with leading dimension Kd, plus C itself when `accumulate` (the
   // residual stream).  NF4 W (scales set): vsb_gemm_nf4.  Dense W: the tile / skinny GEMM, or its row-scale form when the folded
@@ -146,6 +158,17 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
     const T* qkv_in = fused ? xb : h;
     const float* sq_in = fused ? sq_a : nullptr;
     const int sq_in_chunks = !fused ? 0 : li == 0 ? 1 : sqc;   // layer 0: one full-row sum from K::rowsq
+    if (slots) {
+      // q|k|v into scratch, then rotated and scattered to each row's own cache row; attention over each row's own keys
+      T* qkv = gu + rows * inter;                                                      // [B, 3d]
+      VSB_TRY(proj(qkv_in, L.wqkv, L.wqkv_scales, qkv, ld, rows, 3 * d, d, false, VSB_EPI_NONE, 0, 0, 0, sq_in, sq_in_chunks, nullptr));
+      const int dt = ElemT<T>::is_f16 ? VSB_DTYPE_F16 : VSB_DTYPE_BF16;
+      VSB_TRY(vsb_rope_scatter(qkv, ld, B, H, hd, cl, ld, Tmax, slots->slot, slots->len, positions, rope_cos, rope_sin, dt, stream));
+      VSB_TRY(vsb_attn_decode_slots(cl, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, d, B, H, hd, scale, slots->slot, slots->len,
+                                    slots->max_len, dt, stream));
+      VSB_TRY(post_attention(L, xb, rows, fused ? sq_a : nullptr));
+      continue;
+    }
     if (rope_fused) {
       const void* wqkv = L.wqkv;
       if (nf4) {                                               // the RoPE epilogue has no NF4 form: it runs on deq(wqkv)
@@ -199,4 +222,20 @@ extern "C" int vsb_llama_layers_f16(const vsb_llama_layer_t* layers, int n_layer
                                     void* scratch, void* deq_scratch, void* stream) {
   return llama_layers<half>(layers, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, positions, k_start,
                             tail_rows, q_seg, seg_lo, norm_folded, scratch, deq_scratch, stream);
+}
+
+// Slot decode: one new token per sequence, every sequence at its own cache slot and length (a decode batch that admits a new
+// sequence whenever another one ends).  Same per-layer sequence as vsb_llama_layers with Tn = 1, except that the QKV projection
+// goes to scratch and vsb_rope_scatter / vsb_attn_decode_slots place and read each row's keys.
+extern "C" int vsb_llama_layers_slots(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, void* cache, int Bc, int Tmax, int d,
+                                      int H, int inter, float rms_eps, const void* rope_cos, const void* rope_sin, const void* slot_i32,
+                                      const void* len_i32, const void* pos_i32, int max_len, int norm_folded, void* scratch,
+                                      void* deq_scratch, int dtype, void* stream) {
+  VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_llama_layers_slots: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)", dtype);
+  const SlotRows s{slot_i32, len_i32, max_len};
+  if (dtype == VSB_DTYPE_F16)
+    return llama_layers<half>(layers, n_layers, x, B, 1, 0, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr, 0,
+                              nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
+  return llama_layers<bf16>(layers, n_layers, x, B, 1, 0, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr, 0,
+                            nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
 }

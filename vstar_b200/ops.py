@@ -245,6 +245,70 @@ def llama_layers(table, n_layers, x, B, Tn, past, cache, Bc, Tmax, d, H, inter, 
     return x
 
 
+_DTYPE = {"bf16": 0, "f16": 1}                 # VSB_DTYPE_BF16 / VSB_DTYPE_F16
+
+
+def _i32_rows(*ts, n):
+    for t in ts:
+        assert t.dtype == torch.int32 and t.is_contiguous() and t.is_cuda and t.numel() == n
+
+
+def llama_layers_slots(table, n_layers, x, cache, eps, rope_cos, rope_sin, scratch, slot, length, pos, max_len, H, inter,
+                       norm_folded=False, deq_scratch=None):
+    """one decode step of B sequences that each sit at their own slot and length of cache [n_layers, Bc, Tmax, 3d]
+    (vsb_llama_layers_slots): in place on x [B, d]; slot / length / pos int32 [B] on the device (row b's new q|k|v goes to
+    cache row slot[b]*Tmax + length[b] at RoPE position pos[b], and it attends rows [0, length[b]]); max_len >= max(length).
+    scratch: B * (5d + inter) elements; NF4 tables as in llama_layers."""
+    sfx = _sfx(x, cache, scratch, rope_cos, rope_sin)
+    B, d = x.shape
+    L, Bc, Tmax, W = cache.shape
+    assert x.is_contiguous() and cache.is_contiguous() and W == 3 * d and L >= n_layers
+    assert scratch.numel() >= B * (5 * d + inter)
+    _i32_rows(slot, length, pos, n=B)
+    if table[0].wqkv_scales:
+        if sfx != "f16" or norm_folded:
+            raise _lib.VsbError("NF4 layers run in fp16 with unfolded norms")
+        _chk(deq_scratch, F16)
+        assert deq_scratch.is_contiguous() and deq_scratch.numel() >= 2 * inter * d
+    _lib.launches += 8 * n_layers
+    call("vsb_llama_layers_slots", table, n_layers, x.data_ptr(), B, cache.data_ptr(), Bc, Tmax, d, H, inter, float(eps), rope_cos.data_ptr(),
+         rope_sin.data_ptr(), slot.data_ptr(), length.data_ptr(), pos.data_ptr(), int(max_len), 1 if norm_folded else 0, scratch.data_ptr(),
+         _p(deq_scratch), _DTYPE[sfx], _stream())
+    return x
+
+
+def rope_scatter(qkv, cache, H, D, cos_t, sin_t, slot, length, pos):
+    """row b of qkv [B, 3*H*D] -> cache row slot[b]*Tmax + length[b] of cache [Bc, Tmax, 3*H*D] (one layer), q and k rotated at
+    position pos[b] like rope_, v copied (vsb_rope_scatter)"""
+    sfx = _sfx(qkv, cache, cos_t, sin_t)
+    p, B, cols, ld = _rows2d(qkv)
+    assert cols == 3 * H * D and cache.dim() == 3 and cache.shape[2] == cols and cache.is_contiguous()
+    _i32_rows(slot, length, pos, n=B)
+    _lib.launches += 1
+    call("vsb_rope_scatter", p, ld, B, H, D, cache.data_ptr(), cache.stride(1), cache.shape[1], slot.data_ptr(), length.data_ptr(),
+         pos.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), _DTYPE[sfx], _stream())
+    return cache
+
+
+def attn_decode_slots(cache, out, H, D, scale, slot, length, max_len=None):
+    """decode attention over per-row slots and lengths (vsb_attn_decode_slots) on one layer's fused cache [Bc, Tmax, 3*H*D]:
+    row b's query is cache[slot[b], length[b], :H*D] and it attends rows [0, length[b]] of its slot -> out [B, H*D].
+    max_len: a bound on length (default: read from the device)"""
+    sfx = _sfx(cache, out)
+    assert cache.dim() == 3 and cache.is_contiguous() and cache.shape[2] == 3 * H * D and out.stride(1) == 1
+    B = out.shape[0]
+    _i32_rows(slot, length, n=B)
+    if max_len is None:
+        max_len = int(length.max())
+    d = H * D
+    ld = cache.stride(1)
+    base = cache.data_ptr()
+    _lib.launches += 1
+    call("vsb_attn_decode_slots", base, base + 2 * d, base + 4 * d, out.data_ptr(), cache.stride(0), ld, out.stride(0), B, H, D,
+         float(scale), slot.data_ptr(), length.data_ptr(), int(max_len), _DTYPE[sfx], _stream())
+    return out
+
+
 def _gemm_out(a, M, n_out, out, out_dtype, out_rows, residual):
     if out is None:
         out = torch.empty((out_rows if out_rows is not None else M, n_out), dtype=out_dtype or a.dtype, device=a.device)

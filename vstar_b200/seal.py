@@ -3,6 +3,9 @@ free-form answer -> "missing objects" -> guided visual search for each -> object
 Same per-sample logic and result keys as `eval_model` (/root/reference/vstar_bench_eval.py:186-273); the searches for all
 missing objects of an image run in lock-step so their crop frontiers share GPU batches (the reference runs them one after
 another, vstar_bench_eval.py:208-211).
+
+Open-ended questions (the reference demo's `inference()`, app.py:130-233, below its Gradio UI): answer_open /
+answer_open_many, and the command line `python -m vstar_b200.seal`.
 """
 from __future__ import annotations
 
@@ -11,7 +14,7 @@ from copy import deepcopy
 import numpy as np
 import torch
 
-from .visual_search import visual_search_many
+from .visual_search import SearchController, SearchState, visual_search_many
 
 MISSING_OBJECTS_MSG = ("Sorry, I can not answer the question. Some visual information about the following objects is missing or "
                        "unclear:")
@@ -45,12 +48,17 @@ def parse_missing_objects(prediction):
     return [t.strip() for t in tail.split(",")]
 
 
-def focus_question(question, object_names, norm_boxes):
+def focus_message(object_names, norm_boxes):
+    """vstar_bench_eval.py:240-246 / app.py:198-204: the focus message over the located objects' normalised boxes"""
     msg = FOCUS_MSG
     for i, (name, b) in enumerate(zip(object_names, norm_boxes)):
         msg += "{} <object> at location [{:.3f},{:.3f},{:.3f},{:.3f}]".format(name, b[0], b[1], b[2], b[3])
         msg += "; " if i != len(norm_boxes) - 1 else "."
-    return msg + "\n" + question
+    return msg
+
+
+def focus_question(question, object_names, norm_boxes):
+    return focus_message(object_names, norm_boxes) + "\n" + question
 
 
 def smallest_size_for(image, minimum_size_scale=4.0, minimum_size=224):
@@ -125,3 +133,185 @@ def seal_answer(vqa_llm, vsm, image, question, options, minimum_size_scale=4.0, 
     chosen = choose_option(vqa_llm, image, question, options, missing, search_result)
     return dict(question=question, options=options, prediction_freeform=prediction, missing_objects=missing,
                 search_result=search_result, option_chosen=chosen, correct=1 if chosen == 0 else 0)
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# open-ended questions (app.py:130-233)
+OPEN_MAX_NEW_TOKENS = 512          # both generations of app.py's inference()
+OPEN_CONFIDENCE_LOW = 0.3
+NEED_SEARCH_MSG = "Need to conduct visual search to search for: {}."
+
+
+def open_focus_question(question, object_names, norm_boxes, failed_objects, last_name):
+    """app.py:198-213: the focus message over the located boxes, then one "not existent" clause per failed search.  That clause
+    formats `last_name` (app.py's leaked loop variable `object_name`), not the failed object's name - kept as the reference
+    prompts its model."""
+    msg = focus_message(object_names, norm_boxes)
+    if failed_objects:
+        if object_names:
+            msg = msg[:-1] + "; "
+        for i, _failed in enumerate(failed_objects):
+            msg += "{} not existent in the image".format(last_name)
+            msg += "; " if i != len(failed_objects) - 1 else "."
+    return msg + "\n" + question
+
+
+def open_final_request(vqa_llm, image, question, missing, results):
+    """everything app.py:158-215 computes between the searches and the final answer.  results: visual_search's
+    (final_step, path_length, success, all_valid_boxes) per missing object.
+    -> (final free_form_inference item (padded image, focused question, object crops, images_long, objects_long),
+        search-summary string, annotated image)"""
+    from .visualize import visualize_bbox
+    search_result = collect_search_results(missing, results)
+    failed = [name for name, (_, _, ok, _) in zip(missing, results) if not ok]
+    names = [r["name"] for r in search_result]
+    boxes = deepcopy([r["bbox"] for r in search_result])
+    annotated = np.array(image).copy()
+    for name, b in zip(names, boxes):
+        annotated = visualize_bbox(annotated, b, class_name=name, color=(255, 0, 0))
+    images_long = [False]
+    objects_long = [True] * len(names) if len(names) <= 2 else [False] * len(names)
+    crops = torch.stack([vqa_llm.get_object_crop(image, b, patch_scale=1.2) for b in boxes], 0) if boxes else None
+    bg = tuple(int(x * 255) for x in vqa_llm.image_processor.image_mean)
+    padded, left, top = expand2square_center(image, bg)
+    nboxes = [normalize_bbox([b[0] + left, b[1] + top, b[2], b[3]], padded.width, padded.height) for b in boxes]
+    last_name = names[-1] if names else missing[-1]
+    q = open_focus_question(question, names, nboxes, failed, last_name)
+    summary = ""
+    if names:
+        summary += "Targets located after search: {}.".format(", ".join(names))
+    if failed:
+        summary += "Targets unable to locate after search: {}.".format(", ".join(failed))
+    return (padded, q, crops, images_long, objects_long), summary, annotated
+
+
+def answer_open_many(vqa_llm, vsm, items, slots=16, searches_in_flight=8, minimum_size_scale=4.0, minimum_size=224, search_batch=16,
+                     search_kwargs=None):
+    """app.py's inference() for many (image, question) pairs (PIL images), in three phases:
+      A. every direct answer on one decode stream (vqa_llm.free_form_inference_stream, `slots` answers decoding at a time);
+      B. every missing object's search on one SearchController.stream, `searches_in_flight` searches at a time;
+      C. every final answer on one decode stream.
+    -> per item, in input order, app.py's four outputs: (direct answer, None, None, None) when nothing is missing, else
+    ("Need to conduct visual search to search for: ...", search-summary string, annotated np.ndarray image, final answer)."""
+    items = [(image.convert("RGB"), question) for image, question in items]
+    bg = tuple(int(x * 255) for x in vqa_llm.image_processor.image_mean)
+    first = [(expand2square_center(image, bg)[0], q, None, None, None) for image, q in items]
+    direct = [None] * len(items)
+    for i, text in vqa_llm.free_form_inference_stream(first, max_new_tokens=OPEN_MAX_NEW_TOKENS, slots=slots):
+        direct[i] = text
+    missing = [parse_missing_objects(p) for p in direct]
+    states, owner = [], []
+    for i, (image, _) in enumerate(items):
+        smallest = smallest_size_for(image, minimum_size_scale, minimum_size)
+        for name in missing[i]:
+            states.append(SearchState(image, name, smallest, confidence_low=OPEN_CONFIDENCE_LOW, **(search_kwargs or {})))
+            owner.append(i)
+    found = {}
+    if states:
+        ctl = SearchController(vsm, None, search_batch)
+        for st, res in ctl.stream(states, window=searches_in_flight):
+            found[id(st)] = res
+    per_item = [[] for _ in items]
+    for st, i in zip(states, owner):
+        per_item[i].append(found[id(st)])
+    out = [None] * len(items)
+    finals, where = [], []
+    for i, (image, question) in enumerate(items):
+        if not missing[i]:
+            out[i] = (direct[i], None, None, None)
+            continue
+        req, summary, annotated = open_final_request(vqa_llm, image, question, missing[i], per_item[i])
+        finals.append(req)
+        where.append(i)
+        out[i] = [NEED_SEARCH_MSG.format(", ".join(missing[i])), summary, annotated, None]
+    if finals:
+        for k, text in vqa_llm.free_form_inference_stream(finals, max_new_tokens=OPEN_MAX_NEW_TOKENS, slots=slots):
+            out[where[k]][3] = text
+    return [tuple(o) for o in out]
+
+
+def answer_open(vqa_llm, vsm, image, question, minimum_size_scale=4.0, minimum_size=224, **kw):
+    """app.py:130-233 `inference()` below the UI for one PIL image and question -> its four outputs (see answer_open_many)"""
+    return answer_open_many(vqa_llm, vsm, [(image, question)], minimum_size_scale=minimum_size_scale, minimum_size=minimum_size, **kw)[0]
+
+
+def build_parser():
+    """app.py's model flags (parse_args_vqallm, app.py:40-48), bench_eval's dtype / NF4 flags and the questions to answer"""
+    import argparse
+    p = argparse.ArgumentParser(description="SEAL open-ended answering: direct answer, visual search for the missing objects, "
+                                            "final answer (the reference demo's inference(), without its web UI)")
+    p.add_argument("--vqa-model-path", type=str, default="craigwu/seal_vqa_7b")
+    p.add_argument("--vqa-model-base", type=str, default=None)
+    p.add_argument("--conv_type", default="v1", type=str)
+    p.add_argument("--vsm-model-path", type=str, default="craigwu/seal_vsm_7b")
+    p.add_argument("--minimum_size_scale", default=4.0, type=float)
+    p.add_argument("--minimum_size", default=224, type=int)
+    p.add_argument("--vqa-dtype", default="bf16", choices=("bf16", "fp16"))
+    p.add_argument("--vqa-load-4bit", action="store_true")
+    q = p.add_mutually_exclusive_group(required=True)
+    q.add_argument("--image", type=str, help="one image (with --question)")
+    q.add_argument("--questions", type=str, help='JSONL file, one {"image": path, "question": str} per line')
+    p.add_argument("--question", type=str)
+    p.add_argument("--output-path", type=str, default="seal_answers.json")
+    p.add_argument("--save-images", type=str, default=None, help="directory for the annotated search-result images")
+    p.add_argument("--slots", default=16, type=int, help="answers decoding at a time")
+    p.add_argument("--searches-in-flight", default=8, type=int)
+    p.add_argument("--search-batch", default=16, type=int, help="frontier crops per VSM call")
+    return p
+
+
+def read_questions(args):
+    """-> [(image path, question)] from --image/--question or the --questions JSONL file"""
+    import json
+    if args.image is not None:
+        if not args.question:
+            raise SystemExit("--image needs --question")
+        return [(args.image, args.question)]
+    out = []
+    with open(args.questions) as f:
+        for line in f:
+            if line.strip():
+                rec = json.loads(line)
+                out.append((rec["image"], rec["question"]))
+    return out
+
+
+def write_answers(path, questions, answers, save_images=None):
+    """one JSON record per question: image, question, direct_answer, search_summary, final_answer, annotated_image"""
+    import json
+    import os
+    recs = []
+    for k, ((img_path, question), (a0, a1, a2, a3)) in enumerate(zip(questions, answers)):
+        rec = dict(image=img_path, question=question, direct_answer=a0, search_summary=a1, final_answer=a3, annotated_image=None)
+        if a2 is not None and save_images:
+            from PIL import Image
+            os.makedirs(save_images, exist_ok=True)
+            rec["annotated_image"] = os.path.join(save_images, f"{k:05d}_search_result.png")
+            Image.fromarray(a2).save(rec["annotated_image"])
+        recs.append(rec)
+    with open(path, "w") as f:
+        json.dump(recs, f, indent=1)
+    return recs
+
+
+def main(argv=None, vqa_llm=None, vsm=None):
+    from PIL import Image
+    args = build_parser().parse_args(argv)
+    questions = read_questions(args)
+    if vqa_llm is None:
+        from .vqa import VQA_LLM
+        vqa_llm = VQA_LLM(args)
+    if vsm is None:
+        from .visual_search import parse_args
+        from .vsm import VSM
+        vsm_args = parse_args({})
+        vsm_args.version = args.vsm_model_path
+        vsm = VSM(vsm_args)
+    items = [(Image.open(p).convert("RGB"), q) for p, q in questions]
+    answers = answer_open_many(vqa_llm, vsm, items, slots=args.slots, searches_in_flight=args.searches_in_flight,
+                               minimum_size_scale=args.minimum_size_scale, minimum_size=args.minimum_size, search_batch=args.search_batch)
+    return write_answers(args.output_path, questions, answers, args.save_images)
+
+
+if __name__ == "__main__":
+    main()

@@ -359,6 +359,30 @@ class VQAEngine(LlamaClipCore):
             res[i] = outs[k]
         return res
 
+    def decode_stream(self, max_slots, max_positions=None, eos_token_id=2, temperature=0, num_beams=1):
+        """Greedy decode batch that admits a request whenever a slot is free (DecodeStream).  max_positions: cache rows per slot
+        (default self.max_tokens); a request's prompt plus its max_new_tokens must fit in them.  Sampling (temperature > 0)
+        and beam search (num_beams > 1) are refused: the stream steps every slot with one argmax."""
+        if temperature is not None and temperature > 0:
+            raise NotImplementedError("decode_stream decodes greedily: temperature > 0 (sampling) is not supported")
+        if num_beams != 1:
+            raise NotImplementedError("decode_stream decodes greedily: num_beams > 1 (beam search) is not supported")
+        return DecodeStream(self, max_slots, self.max_tokens if max_positions is None else max_positions, eos_token_id)
+
+    def spliced_length(self, input_ids, n_crops=0, images_long=None, objects_long=None):
+        """rows the spliced sequence of build_embeds(input_ids, ...) has, computed on the host (the rule of _splice)"""
+        ids = list(input_ids)
+        n_obj = ids.count(OBJECT_TOKEN_INDEX)
+        if ids.count(IMAGE_TOKEN_INDEX) != 1 or n_obj > n_crops:
+            raise ValueError(f"a request needs one image token and at most {n_crops} object tokens (one per crop), got "
+                             f"{ids.count(IMAGE_TOKEN_INDEX)} and {n_obj}")
+        long_img = images_long is None or bool(images_long[0])
+        T = len(ids) - 1 - n_obj + (self.cfg.clip_tokens if long_img else self.NLAT)
+        for oi in range(n_obj):
+            short = objects_long is None or not bool(objects_long[oi])
+            T += self.NLAT if short else self.cfg.clip_tokens
+        return T
+
     def _beam_args(self, num_beams, temperature, stop_ids, eos_token_id, early_stopping):
         """True when the call runs beam search (num_beams > 1); raises on the combinations beam search does not serve"""
         check_beams(num_beams, early_stopping)
@@ -531,6 +555,148 @@ class VQAEngine(LlamaClipCore):
                 losses = torch.stack(per[g])
                 results[i] = (losses, int(losses.argmin()))
         return results
+
+
+class StreamRequest:
+    """handle of a request admitted to a DecodeStream: `tokens` grows by one id per step, `done` once it ended"""
+
+    def __init__(self, rid, slot, length, max_new_tokens, stop_ids):
+        self.id, self.slot, self.prompt_len = rid, slot, length
+        self.max_new_tokens, self.stop_ids = max_new_tokens, list(stop_ids) if stop_ids else None
+        self.tokens, self.done = [], False
+
+    def __repr__(self):
+        return f"StreamRequest(id={self.id}, slot={self.slot}, tokens={len(self.tokens)}, done={self.done})"
+
+
+class DecodeStream:
+    """Greedy decoding of many requests on a decode batch that admits a new request whenever a slot frees (iteration-level
+    admission), instead of generate_batch's static batch that steps until its longest answer ends.
+
+    The stream owns its KV cache [n_layers, max_slots, max_positions, 3d], separate from the engine's, so option scoring,
+    generate() or a VSM call in between neither disturbs it nor is disturbed by it.  A request is prefilled alone into a free
+    slot at rows [0, T) and takes its first token from the prefill logits, as in generate().  Every step() then runs ONE
+    vsb_llama_layers_slots call for all active slots (each row writes its new q|k|v at its own slot and length and attends
+    only its own keys), one argmax_rows launch and one device-to-host copy.  A request ends at eos, at its stop_ids (the rule of
+    generate_batch) or after its own max_new_tokens, and its slot is free for the next admit().  In batch-invariant mode
+    (ops.batch_invariant) a request's logits do not depend on the other requests in the batch or on its slot."""
+
+    def __init__(self, engine, max_slots, max_positions, eos_token_id=2):
+        max_slots, max_positions = int(max_slots), int(max_positions)
+        if max_slots < 1:
+            raise ValueError(f"max_slots must be >= 1, got {max_slots}")
+        if not 1 <= max_positions <= engine.MAX_POSITIONS:
+            raise ops._lib.VsbError(f"max_positions {max_positions} outside [1, {engine.MAX_POSITIONS}] (the rows of the RoPE tables)")
+        c = engine.cfg
+        self.engine, self.eos = engine, eos_token_id
+        self.max_slots, self.max_positions = max_slots, max_positions
+        if engine._layer_table is None:
+            engine._layer_table = ops.llama_layer_table(engine.w.layers)
+        dev, dt = engine.dev, engine.dtype
+        self._cache = torch.empty((c.n_layers, max_slots, max_positions, 3 * c.hidden), dtype=dt, device=dev)
+        self._scratch = torch.empty((max_slots * (5 * c.hidden + c.intermediate),), dtype=dt, device=dev)
+        self._deq = torch.empty((2 * c.intermediate * c.hidden,), dtype=dt, device=dev) if getattr(engine.w, "quant", None) else None
+        self._slots = [None] * max_slots                 # slot -> active StreamRequest
+        self._finished = []                              # ended at admission; reported by the next step()
+        self._next_id = 0
+        self.steps = 0
+        self.occupied = 0                                # sum over steps of the rows decoded
+        self.last_logits = None                          # (requests in row order, fp32 logits [rows, V]) of the latest call
+
+    @property
+    def free_slots(self):
+        return sum(r is None for r in self._slots)
+
+    @property
+    def active(self):
+        return [r for r in self._slots if r is not None]
+
+    def _check_open(self):
+        if self._cache is None:
+            raise RuntimeError("decode stream is closed")
+
+    def _ended(self, r):
+        t = r.tokens
+        return t[-1] == self.eos or (r.stop_ids and t[-len(r.stop_ids):] == r.stop_ids) or len(t) >= r.max_new_tokens
+
+    def admit(self, request, max_new_tokens, stop_ids=None):
+        """request = (input_ids, image, object_crops, images_long, objects_long) as generate_batch takes it -> StreamRequest.
+        Raises (before any launch) when no slot is free or the prompt plus max_new_tokens exceeds max_positions."""
+        self._check_open()
+        ids, image, crops, il, ol = request
+        max_new_tokens = int(max_new_tokens)
+        if max_new_tokens < 1:
+            raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
+        e = self.engine
+        T = e.spliced_length(ids, 0 if crops is None else int(crops.shape[0]), il, ol)
+        if T + max_new_tokens > self.max_positions:
+            raise ops._lib.VsbError(f"prompt of {T} rows + {max_new_tokens} new tokens exceeds the stream's {self.max_positions} "
+                                    "positions per slot")
+        if self.free_slots == 0:
+            raise RuntimeError(f"no free slot: all {self.max_slots} slots of the decode stream are in use")
+        slot = self._slots.index(None)
+        x = e.build_embeds(ids, image, crops, il, ol)
+        assert x.shape[0] == T
+        c = e.cfg
+        scratch = torch.empty((T * (2 * c.hidden + c.intermediate),), dtype=e.dtype, device=e.dev)
+        Bc, Tm = self.max_slots, self.max_positions
+        ops.llama_layers(e._layer_table, len(e.w.layers), x, 1, T, 0, self._cache, Bc, Tm, c.hidden, c.n_heads, c.intermediate,
+                         c.rms_eps, e.w.rope_cos, e.w.rope_sin, scratch, cache_row_offset=slot * Tm,
+                         norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
+        _, idx, logits = e._logits_rows(x, torch.tensor([T - 1], dtype=torch.int64, device=e.dev))
+        r = StreamRequest(self._next_id, slot, T, max_new_tokens, stop_ids)
+        self._next_id += 1
+        self.last_logits = ([r], logits)
+        r.tokens.append(int(idx[0]))
+        if self._ended(r):
+            r.done = True
+            self._finished.append(r)
+        else:
+            self._slots[slot] = r
+        return r
+
+    def step(self):
+        """one decode step of every active request -> [(handle, new token ids)] of the requests that ended in it (and of those
+        that ended at admission since the previous step)"""
+        self._check_open()
+        done, self._finished = [(r, r.tokens) for r in self._finished], []
+        act = self.active
+        if not act:
+            return done
+        e, c = self.engine, self.engine.cfg
+        B = len(act)
+        lens = [r.prompt_len + len(r.tokens) - 1 for r in act]        # rows cached; the newest token goes to row `len`
+        meta = torch.tensor([[r.slot for r in act], lens, lens], dtype=torch.int32).to(e.dev)
+        ids = torch.tensor([r.tokens[-1] for r in act], dtype=torch.int64).to(e.dev)
+        x = ops.gather_rows(ids, e.w.embed)
+        ops.llama_layers_slots(e._layer_table, len(e.w.layers), x, self._cache, c.rms_eps, e.w.rope_cos, e.w.rope_sin, self._scratch,
+                               meta[0], meta[1], meta[2], max(lens), c.n_heads, c.intermediate,
+                               norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
+        hn = ops.rmsnorm(x, e.w.final_norm, c.rms_eps)
+        logits = ops.gemm(hn, e.w.lm_head, out_dtype=torch.float32)
+        nxt = ops.argmax_rows(logits)[0].tolist()                       # the one device-to-host copy of the step
+        self.last_logits = (act, logits)
+        self.steps += 1
+        self.occupied += B
+        for r, t in zip(act, nxt):
+            r.tokens.append(int(t))
+            if self._ended(r):
+                r.done = True
+                self._slots[r.slot] = None
+                done.append((r, r.tokens))
+        return done
+
+    def close(self):
+        """free the stream's cache and scratch (requests still running are abandoned)"""
+        self._cache = self._scratch = self._deq = None
+        self._slots = [None] * self.max_slots
+        self.last_logits = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -785,39 +951,23 @@ class VQA_LLM:
             check_sampling(self.top_k, top_p)
         if num_beams != 1:
             return self._beam_texts([(image, question, object_crops, images_long, objects_long)], num_beams, max_new_tokens, temperature)[0]
-        prompt = build_prompt_v1(DEFAULT_IMAGE_TOKEN + "\n" + question)
-        stop_str = "</s>"
-        ids = tokenizer_image_object_token(prompt, self.tokenizer)
-        kw = self.tokenizer(stop_str).input_ids
-        if len(kw) > 1 and kw[0] == self.tokenizer.bos_token_id:
-            kw = kw[1:]
+        ids = self._prompt_ids(question)
         img, crops = self._pixels(image, object_crops)
-        out = self.engine.generate(ids, img, crops, images_long, objects_long, max_new_tokens, self.eos, stop_ids=kw,
+        out = self.engine.generate(ids, img, crops, images_long, objects_long, max_new_tokens, self.eos, stop_ids=self._stop_ids(),
                                    temperature=temperature if sample else 0, top_k=self.top_k, top_p=top_p,
                                    seed=draw_seeds(1)[0] if sample else None)
-        text = self.tokenizer.batch_decode([out], skip_special_tokens=True)[0].strip()
-        if text.endswith(stop_str):
-            text = text[:-len(stop_str)]
-        return text.strip()
+        return self._answer_text(out)
 
     @torch.inference_mode()
     def _beam_texts(self, items, num_beams, max_new_tokens, temperature):
         """items: [(image, question, object_crops, images_long, objects_long)] -> decoded best hypotheses"""
-        stop_str = "</s>"
         reqs = []
         for image, question, crops, il, ol in items:
-            ids = tokenizer_image_object_token(build_prompt_v1(DEFAULT_IMAGE_TOKEN + "\n" + question), self.tokenizer)
             img, crops = self._pixels(image, crops)
-            reqs.append((ids, img, crops, il, ol))
+            reqs.append((self._prompt_ids(question), img, crops, il, ol))
         outs = self.engine.generate_batch(reqs, max_new_tokens, self.eos, temperature=temperature, num_beams=num_beams,
                                           length_penalty=self.length_penalty, early_stopping=self.early_stopping)
-        texts = []
-        for out in outs:
-            text = self.tokenizer.batch_decode([out], skip_special_tokens=True)[0].strip()
-            if text.endswith(stop_str):
-                text = text[:-len(stop_str)]
-            texts.append(text.strip())
-        return texts
+        return [self._answer_text(out) for out in outs]
 
     def free_form_inference_batch(self, images, questions, max_new_tokens=200, originals=None, temperature=0, top_p=None, num_beams=1):
         """free_form_inference for several (image, question) pairs in ONE continuous-batched decode (not in the reference,
@@ -834,27 +984,83 @@ class VQA_LLM:
                 images = [self.device_pixels(o, None)[0] for o in originals]
             return self._beam_texts([(im, q, None, None, None) for im, q in zip(images, questions)], num_beams, max_new_tokens,
                                     temperature)
-        stop_str = "</s>"
-        kw = self.tokenizer(stop_str).input_ids
-        if len(kw) > 1 and kw[0] == self.tokenizer.bos_token_id:
-            kw = kw[1:]
         reqs = []
         for k, (image, question) in enumerate(zip(images, questions)):
-            ids = tokenizer_image_object_token(build_prompt_v1(DEFAULT_IMAGE_TOKEN + "\n" + question), self.tokenizer)
+            ids = self._prompt_ids(question)
             if originals is not None and self._img_src is not None:
                 img, _ = self.device_pixels(originals[k], None)
             else:
                 img, _ = self._pixels(image, None)
             reqs.append((ids, img, None, None, None))
-        outs = self.engine.generate_batch(reqs, max_new_tokens, self.eos, stop_ids=kw, temperature=temperature if sample else 0,
-                                          top_k=self.top_k, top_p=top_p, seeds=draw_seeds(len(reqs)) if sample else None)
-        texts = []
-        for out in outs:
-            text = self.tokenizer.batch_decode([out], skip_special_tokens=True)[0].strip()
-            if text.endswith(stop_str):
-                text = text[:-len(stop_str)]
-            texts.append(text.strip())
-        return texts
+        outs = self.engine.generate_batch(reqs, max_new_tokens, self.eos, stop_ids=self._stop_ids(),
+                                          temperature=temperature if sample else 0, top_k=self.top_k, top_p=top_p,
+                                          seeds=draw_seeds(len(reqs)) if sample else None)
+        return [self._answer_text(out) for out in outs]
+
+    def _prompt_ids(self, question):
+        """ids of the v1 conversation prompt with the image token before `question` (vstar_bench_eval.py:79-85)"""
+        return tokenizer_image_object_token(build_prompt_v1(DEFAULT_IMAGE_TOKEN + "\n" + question), self.tokenizer)
+
+    def _stop_ids(self):
+        """ids of the v1 stop string "</s>" without the tokenizer's bos (KeywordsStoppingCriteria)"""
+        kw = self.tokenizer("</s>").input_ids
+        if len(kw) > 1 and kw[0] == self.tokenizer.bos_token_id:
+            kw = kw[1:]
+        return kw
+
+    def _answer_text(self, out):
+        """new token ids -> answer text: decoded without special tokens, the stop string cut off, stripped"""
+        stop_str = "</s>"
+        text = self.tokenizer.batch_decode([out], skip_special_tokens=True)[0].strip()
+        if text.endswith(stop_str):
+            text = text[:-len(stop_str)]
+        return text.strip()
+
+    @torch.inference_mode()
+    def free_form_inference_stream(self, items, max_new_tokens=200, slots=16):
+        """free_form_inference (greedy) for many items on one decode stream (VQAEngine.decode_stream): items are (image,
+        question, object_crops, images_long, objects_long); yields (index, text) as each answer completes, with the prompt,
+        stop string and post-processing of free_form_inference.  The next item is admitted whenever a slot frees, so up to
+        `slots` answers decode together however much their lengths differ.  As in free_form_inference, an answer whose prompt
+        plus max_new_tokens would pass the 2048 positions of the RoPE tables gets the positions that are left."""
+        reqs = [(self._prompt_ids(question), image, crops, il, ol) for image, question, crops, il, ol in items]
+        for i, out in self._decode_stream(reqs, int(max_new_tokens), int(slots)):
+            yield i, self._answer_text(out)
+
+    def _decode_stream(self, reqs, max_new_tokens, slots):
+        """(prompt ids, image, object_crops, images_long, objects_long) requests -> (index, new token ids) as each ends, on one
+        decode stream with min(slots, len(reqs)) slots"""
+        if not reqs:
+            return
+        e = self.engine
+        kw = self._stop_ids()
+        lens = [e.spliced_length(ids, 0 if crops is None else len(crops), il, ol) for ids, _, crops, il, ol in reqs]
+        # generate() reserves min(max_new_tokens, 2048 - T) positions: the same budget here
+        budgets = [max(1, min(max_new_tokens, e.MAX_POSITIONS - T)) for T in lens]
+        positions = min(e.MAX_POSITIONS, max(T + n for T, n in zip(lens, budgets)))
+        stream = e.decode_stream(min(slots, len(reqs)), positions, self.eos)
+        try:
+            index = {}
+            nxt = 0
+
+            def admit():
+                nonlocal nxt
+                ids, image, crops, il, ol = reqs[nxt]
+                img, crops = self._pixels(image, crops)
+                index[stream.admit((ids, img, crops, il, ol), budgets[nxt], stop_ids=kw).id] = nxt
+                nxt += 1
+
+            while nxt < len(reqs) and stream.free_slots:
+                admit()
+            remaining = len(reqs)
+            while remaining:
+                for r, out in stream.step():
+                    remaining -= 1
+                    yield index[r.id], out
+                while nxt < len(reqs) and stream.free_slots:
+                    admit()
+        finally:
+            stream.close()
 
     def _choice_item(self, image, question, options, object_crops, images_long, objects_long):
         qs = DEFAULT_IMAGE_TOKEN + "\n" + question
