@@ -45,7 +45,7 @@ def gpu_info():
     return dict(device=torch.cuda.get_device_name(), nvidia_smi=q, sms=torch.cuda.get_device_properties(0).multi_processor_count)
 
 
-def tile_bn(M, N, sms, rope=False):
+def tile_bn(M, N, sms, rope=False, swiglu=False):
     """the tile width gemm_dispatch (gemm_tcgen05.cu) picks for an M x N tile-kernel GEMM"""
     if rope:
         return 256
@@ -53,6 +53,8 @@ def tile_bn(M, N, sms, rope=False):
     if N > 64:
         tm, best = -(-M // BM), None
         for c in (256, 128, 64):
+            if c == 256 and not swiglu:
+                continue
             if c == 64 and N > 512:
                 continue
             cost = -(-(tm * -(-N // c)) // sms) * c
@@ -160,7 +162,7 @@ def cublas_fn(bf, M, N, K):
 def row(bf, sms, name, M, N, K, rope, fn, cublas=True):
     ms, lo, hi = time_ms(fn)
     flops = 2.0 * M * N * K
-    bn = tile_bn(M, N, sms, rope)
+    bn = tile_bn(M, N, sms, rope, swiglu=name.split(".")[0].split("@")[0] == "gu")
     tiles = -(-M // BM) * -(-N // bn)
     r = dict(name=name, M=M, N=N, K=K, bn=bn, tiles=tiles, waves=-(-tiles // sms), ms=ms, ms_spread=[lo, hi], tflops=flops / ms / 1e9)
     if cublas:

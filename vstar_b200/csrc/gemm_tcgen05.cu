@@ -934,7 +934,10 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
   }
   VSB_CHECK_ARG(g_force_bn != 1 && g_force_bn != 2, "vsb_gemm_bf16: skinny kernel forced but M=%d too large or K %% 8 != 0", M);
   const int sms = g_max_ctas > 0 ? g_max_ctas : vsb_num_sms();
-  // tile-width choice: minimise (waves * BN) ~ time; prefer the wider tile on ties (less A re-streaming)
+  // tile-width choice: minimise (waves * BN) ~ time; prefer the wider tile on ties (less A re-streaming).  256-wide tiles only
+  // for SwiGLU (and the fused RoPE, below): with every other epilogue a 256-wide tile writes 256 output columns per tile row,
+  // and on H100 its fixed cost per wave (~39 us against ~18 us at BN = 128) and its main-loop rate (~410 against ~715 TFLOP/s)
+  // make it slower than two 128-wide tiles at the same waves * BN (e.g. OWL-B qkv, M = 18440, N = 2304, K = 768: 0.49 -> 0.34 ms)
   int bn = 64;
   if (g_force_bn) {
     bn = g_force_bn;
@@ -944,6 +947,7 @@ static int gemm_dispatch(const void* A, long long lda, const void* W, long long 
     const int cands[3] = {256, 128, 64};
     for (int i = 0; i < 3; ++i) {
       int c = cands[i];
+      if (c == 256 && epilogue != VSB_EPI_SWIGLU) continue;
       if (c == 64 && N > 512) continue;
       long long tiles = (long long)tm * ((N + c - 1) / c);
       long long waves = (tiles + sms - 1) / sms;
