@@ -82,7 +82,7 @@ int vsb_gemm_qkv_rope_f16(const void* A, long long lda, const void* W, long long
                           int rows_per_group, long long group_stride, long long group_offset, const void* rowsq_in, int sq_in_chunks,
                           float eps, long long sq_ld, const void* cos_table, const void* sin_table, const void* positions, int T, int pos0,
                           int head_dim, void* stream);
-/* 1 (default): vsb_llama_layers applies RoPE in the QKV GEMM epilogue (head_dim 128); 0: separate vsb_rope_bf16 launch */
+/* 1: vsb_llama_layers applies RoPE in the QKV GEMM epilogue (head_dim 128); 0 (default): separate vsb_rope_bf16 launch */
 int vsb_llama_set_fuse_rope(int on);
 /* per-row sum of squares (fp32) of a bf16 matrix: the first rowsq_in of a chain of folded GEMMs (sq_in_chunks = 1) */
 int vsb_rowsq_bf16(const void* x, long long ldx, void* out_f32, int rows, int cols, void* stream);
