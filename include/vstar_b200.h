@@ -152,6 +152,12 @@ int vsb_argmax_rows_f32(const void* x, long long ld, int rows, int n, void* idx_
  * depends only on the row's logits, its seed and step.  seeds_i64: device int64 [rows]; idx_i32: device int32 [rows]. */
 int vsb_sample_rows_f32(const void* logits, long long ld, int rows, int n, float temperature, int top_k, float top_p, int logit_dtype,
                         const void* seeds_i64, int step, void* idx_i32, void* stream);
+/* vsb_sample_rows_f32 with every row's own settings (a decode stream, each request at its own step): temperature_f32 (> 0),
+ * top_k_i32 (0 = off), top_p_f32 (1 = off), seeds_i64 and steps_i32 are device arrays [rows]; the row's token is the one
+ * vsb_sample_rows_f32 draws for the same logits, settings, seed and step.  The caller validates the settings. */
+int vsb_sample_rows_var_f32(const void* logits, long long ld, int rows, int n, const void* temperature_f32, const void* top_k_i32,
+                            const void* top_p_f32, int logit_dtype, const void* seeds_i64, const void* steps_i32, void* idx_i32,
+                            void* stream);
 /* per-row negative log-likelihood of labels under softmax(logits) — option scoring of the SEAL VQA LLM
  * (CrossEntropyLoss, /root/reference/vstar_bench_eval.py:154-159) */
 int vsb_nll_rows_f32(const void* logits, long long ld, int rows, int n, const void* labels_i64, void* out_f32, void* stream);
@@ -176,6 +182,12 @@ int vsb_beam_candidates_f32(const void* logits, long long ld, int V, int request
 #define VSB_COPY_ROWS_MAX_PAIRS 256
 int vsb_copy_cache_rows_b16(void* cache, int layers, long long layer_stride, int slots, long long slot_stride, long long row_stride,
                             int row_elems, const int* pairs_i32, int npairs, int lo, int hi, void* stream);
+/* vsb_copy_cache_rows_b16 with a row range per pair: quads_i32 is a HOST array of npairs (src, dst, lo, hi), rows [lo, hi) of
+ * slot src copied to slot dst for every layer.  Refused with VSB_ERR_ARG before any launch: a slot that is both a source and a
+ * destination, a destination named twice, a slot outside [0, slots), lo > hi or a range past the slot; slots <= 65536.
+ * One launch. */
+int vsb_copy_slot_rows_b16(void* cache, int layers, long long layer_stride, int slots, long long slot_stride, long long row_stride,
+                           int row_elems, const int* quads_i32, int npairs, void* stream);
 
 /* The whole Llama decoder stack over Tn new rows per sequence, in place on the residual stream x [B*Tn, d] bf16
  * (HF LlamaModel layers as called from llava_llama.py:93-105 / llava_search_llama.py:80-92).  Fused q|k|v rows live in

@@ -36,9 +36,11 @@ SIGNATURES = {
     "vsb_nll_rows_f32": [c_p, c_ll, c_i, c_i, c_p, c_p, c_p],
     "vsb_argmax_rows_f32": [c_p, c_ll, c_i, c_i, c_p, c_p, c_p],
     "vsb_sample_rows_f32": [c_p, c_ll, c_i, c_i, c_f, c_i, c_f, c_i, c_p, c_i, c_p, c_p],
+    "vsb_sample_rows_var_f32": [c_p, c_ll, c_i, c_i, c_p, c_p, c_p, c_i, c_p, c_p, c_p, c_p],
     "vsb_copy2d_b16": [c_p, c_ll, c_p, c_ll, c_ll, c_i, c_p],
     "vsb_beam_candidates_f32": [c_p, c_ll, c_i, c_i, c_i, c_i, c_p, c_p, c_i, c_p, c_p, c_p, c_p],
     "vsb_copy_cache_rows_b16": [c_p, c_i, c_ll, c_i, c_ll, c_ll, c_i, c_p, c_i, c_i, c_i, c_p],
+    "vsb_copy_slot_rows_b16": [c_p, c_i, c_ll, c_i, c_ll, c_ll, c_i, c_p, c_i, c_p],
     "vsb_llama_layers": [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_i, c_p, c_i, c_i, c_p, c_p,
                          c_p],
     "vsb_gemm_rowscale_bf16": [c_p, c_ll, c_p, c_ll, c_p, c_ll, c_i, c_i, c_i, c_p, c_p, c_ll, c_i, c_i, c_ll, c_ll, c_p, c_i, c_f, c_p, c_ll, c_p],

@@ -86,3 +86,23 @@ class BeamRequest:
         if self.prompt_len + len(ids) < self.max_length:
             ids = ids + [self.eos]
         return ids, score
+
+
+def fork_slots(old, nxt, owned):
+    """copy-on-fork slot management of one request's beams.  old: cache slot of each running beam (beam order), nxt: the new
+    beams as BeamRequest.process returns them ((score, token, parent beam) in rank order), owned: every slot the request holds.
+    A surviving parent keeps its slot for its first child; later children take the slots of beams that died (in `owned`
+    order) and must receive the parent's generated rows.  -> (slot of each new beam, [(parent slot, child slot)] forks).
+    No slot is both the source and the destination of a fork."""
+    kept = {old[p] for _, _, p in nxt}
+    free = [s for s in owned if s not in kept]
+    new, claimed, forks = [], set(), []
+    for _, _, p in nxt:
+        if p not in claimed:                    # the parent's first child keeps its slot
+            claimed.add(p)
+            s = old[p]
+        else:                                   # later children fork into the slot of a beam that died
+            s = free.pop(0)
+            forks.append((old[p], s))
+        new.append(s)
+    return new, forks

@@ -9,9 +9,10 @@
 // log-probs tie exactly as they do in the oracle.  The candidates at or above the threshold are compacted into shared memory
 // and bitonic-sorted by (key desc, index asc); a tie at the threshold wider than that buffer is resolved by one ordered pass.
 //
-// vsb_copy_cache_rows_b16: rows [lo, hi) of the fused-QKV cache [L][B, Tmax, 3d] from slot src to slot dst for every layer and
-// every pair, in one launch.  Pairs travel in the kernel's parameters; a slot that is both a source and a destination (or two
-// pairs with one destination) is refused, so no CTA reads a row another CTA writes.
+// vsb_copy_cache_rows_b16 / vsb_copy_slot_rows_b16: rows of the fused-QKV cache [L][B, Tmax, 3d] from slot src to slot dst for
+// every layer and every pair, in one launch; one row range [lo, hi) for all pairs, or each pair's own (a decode stream, where
+// every beam request forks at its own length).  Pairs travel in the kernel's parameters; a slot that is both a source and a
+// destination (or two pairs with one destination) is refused, so no CTA reads a row another CTA writes.
 #include <algorithm>
 
 #include "common.cuh"
@@ -217,17 +218,32 @@ __global__ void __launch_bounds__(kThreads, 1) beam_candidates_kernel(const floa
   }
 }
 
-struct CopyPairs {
+// one row range for every pair (vsb_copy_cache_rows_b16)
+struct UniformPairs {
   int src[VSB_COPY_ROWS_MAX_PAIRS];
   int dst[VSB_COPY_ROWS_MAX_PAIRS];
+  int lo, hi;
+  __device__ __forceinline__ int lo_of(int) const { return lo; }
+  __device__ __forceinline__ int hi_of(int) const { return hi; }
+};
+
+// a row range per pair (vsb_copy_slot_rows_b16); 16-bit slots keep the parameters inside the 4 KB kernel-argument limit
+struct RangedPairs {
+  unsigned short src[VSB_COPY_ROWS_MAX_PAIRS];
+  unsigned short dst[VSB_COPY_ROWS_MAX_PAIRS];
+  int lo[VSB_COPY_ROWS_MAX_PAIRS];
+  int hi[VSB_COPY_ROWS_MAX_PAIRS];
+  __device__ __forceinline__ int lo_of(int p) const { return lo[p]; }
+  __device__ __forceinline__ int hi_of(int p) const { return hi[p]; }
 };
 
 // grid (chunks, layers, pairs): rows [lo, hi) of one slot of one layer, as VEC-element vectors
-template <typename VEC>
+template <typename VEC, typename PAIRS>
 __global__ void __launch_bounds__(256) copy_cache_rows_kernel(unsigned short* cache, long long layer_stride, long long slot_stride,
-                                                              long long row_stride, int row_elems, int lo, int hi, const CopyPairs pairs) {
+                                                              long long row_stride, int row_elems, const PAIRS pairs) {
   constexpr int kVec = sizeof(VEC) / 2;
   const int p = blockIdx.z;
+  const int lo = pairs.lo_of(p), hi = pairs.hi_of(p);
   unsigned short* base = cache + (long long)blockIdx.y * layer_stride;
   const VEC* src = reinterpret_cast<const VEC*>(base + (long long)pairs.src[p] * slot_stride);
   VEC* dst = reinterpret_cast<VEC*>(base + (long long)pairs.dst[p] * slot_stride);
@@ -238,6 +254,23 @@ __global__ void __launch_bounds__(256) copy_cache_rows_kernel(unsigned short* ca
     const long long row = lo + e / per_row, c = e % per_row;
     dst[row * rs + c] = src[row * rs + c];
   }
+}
+
+// one launch for npairs pairs of at most `rows` rows each
+template <typename PAIRS>
+void launch_copy_rows(void* cache, int layers, long long layer_stride, long long slot_stride, long long row_stride, int row_elems,
+                      const PAIRS& pp, int npairs, int rows, void* stream) {
+  const bool vec = ((reinterpret_cast<uintptr_t>(cache) | (uintptr_t)layer_stride * 2 | (uintptr_t)slot_stride * 2 |
+                     (uintptr_t)row_stride * 2 | (uintptr_t)row_elems * 2) & 15) == 0;
+  const long long elems = (long long)rows * row_elems / (vec ? 8 : 1);
+  const int chunks = (int)std::min<long long>((elems + 255) / 256, 64);
+  dim3 grid(chunks, layers, npairs);
+  if (vec)
+    copy_cache_rows_kernel<uint4, PAIRS><<<grid, 256, 0, STREAM(stream)>>>((unsigned short*)cache, layer_stride, slot_stride, row_stride,
+                                                                          row_elems, pp);
+  else
+    copy_cache_rows_kernel<unsigned short, PAIRS><<<grid, 256, 0, STREAM(stream)>>>((unsigned short*)cache, layer_stride, slot_stride,
+                                                                                   row_stride, row_elems, pp);
 }
 
 }  // namespace
@@ -271,7 +304,7 @@ extern "C" int vsb_copy_cache_rows_b16(void* cache, int layers, long long layer_
                 VSB_COPY_ROWS_MAX_PAIRS, npairs);
   VSB_CHECK_ARG(0 <= lo && lo <= hi && (long long)hi * row_stride <= slot_stride, "vsb_copy_cache_rows_b16: bad row range [%d, %d)", lo, hi);
   VSB_CHECK_ARG(npairs == 0 || pairs_i32, "vsb_copy_cache_rows_b16: null pair list");
-  CopyPairs pp;
+  UniformPairs pp;
   for (int p = 0; p < npairs; ++p) {
     const int s = pairs_i32[2 * p], d = pairs_i32[2 * p + 1];
     VSB_CHECK_ARG(s >= 0 && s < slots && d >= 0 && d < slots, "vsb_copy_cache_rows_b16: pair %d (%d -> %d) outside [0, %d)", p, s, d, slots);
@@ -282,18 +315,40 @@ extern "C" int vsb_copy_cache_rows_b16(void* cache, int layers, long long layer_
     pp.src[p] = s;
     pp.dst[p] = d;
   }
+  pp.lo = lo;
+  pp.hi = hi;
   if (npairs == 0 || hi == lo) return VSB_OK;
-  const bool vec = ((reinterpret_cast<uintptr_t>(cache) | (uintptr_t)layer_stride * 2 | (uintptr_t)slot_stride * 2 |
-                     (uintptr_t)row_stride * 2 | (uintptr_t)row_elems * 2) & 15) == 0;
-  const long long elems = (long long)(hi - lo) * row_elems / (vec ? 8 : 1);
-  const int chunks = (int)std::min<long long>((elems + 255) / 256, 64);
-  dim3 grid(chunks, layers, npairs);
-  if (vec)
-    copy_cache_rows_kernel<uint4><<<grid, 256, 0, STREAM(stream)>>>((unsigned short*)cache, layer_stride, slot_stride, row_stride, row_elems,
-                                                                   lo, hi, pp);
-  else
-    copy_cache_rows_kernel<unsigned short><<<grid, 256, 0, STREAM(stream)>>>((unsigned short*)cache, layer_stride, slot_stride, row_stride,
-                                                                            row_elems, lo, hi, pp);
+  launch_copy_rows(cache, layers, layer_stride, slot_stride, row_stride, row_elems, pp, npairs, hi - lo, stream);
+  VSB_LAUNCH_CHECK();
+  return VSB_OK;
+}
+
+extern "C" int vsb_copy_slot_rows_b16(void* cache, int layers, long long layer_stride, int slots, long long slot_stride, long long row_stride,
+                                      int row_elems, const int* quads_i32, int npairs, void* stream) {
+  VSB_CHECK_ARG(cache && layers > 0 && slots > 0 && slots <= 65536 && row_elems > 0 && row_stride >= row_elems,
+                "vsb_copy_slot_rows_b16: bad args");
+  VSB_CHECK_ARG(npairs >= 0 && npairs <= VSB_COPY_ROWS_MAX_PAIRS, "vsb_copy_slot_rows_b16: npairs must be in [0, %d], got %d",
+                VSB_COPY_ROWS_MAX_PAIRS, npairs);
+  VSB_CHECK_ARG(npairs == 0 || quads_i32, "vsb_copy_slot_rows_b16: null pair list");
+  RangedPairs pp;
+  int rows = 0;
+  for (int p = 0; p < npairs; ++p) {
+    const int s = quads_i32[4 * p], d = quads_i32[4 * p + 1], lo = quads_i32[4 * p + 2], hi = quads_i32[4 * p + 3];
+    VSB_CHECK_ARG(s >= 0 && s < slots && d >= 0 && d < slots, "vsb_copy_slot_rows_b16: pair %d (%d -> %d) outside [0, %d)", p, s, d, slots);
+    VSB_CHECK_ARG(0 <= lo && lo <= hi && (long long)hi * row_stride <= slot_stride, "vsb_copy_slot_rows_b16: pair %d: bad row range [%d, %d)",
+                  p, lo, hi);
+    for (int q = 0; q < npairs; ++q) {
+      VSB_CHECK_ARG(quads_i32[4 * q + 1] != s, "vsb_copy_slot_rows_b16: slot %d is both a source and a destination", s);
+      VSB_CHECK_ARG(q == p || quads_i32[4 * q + 1] != d, "vsb_copy_slot_rows_b16: slot %d is the destination of two pairs", d);
+    }
+    pp.src[p] = (unsigned short)s;
+    pp.dst[p] = (unsigned short)d;
+    pp.lo[p] = lo;
+    pp.hi[p] = hi;
+    rows = std::max(rows, hi - lo);
+  }
+  if (npairs == 0 || rows == 0) return VSB_OK;
+  launch_copy_rows(cache, layers, layer_stride, slot_stride, row_stride, row_elems, pp, npairs, rows, stream);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }

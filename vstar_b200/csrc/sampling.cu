@@ -10,6 +10,8 @@
 //      or after j exceeds (1 - top_p) of the total (HF's ascending cumsum rule; position 0 always kept).
 //   4. inverse CDF at u = Philox4x32-10(key = seed, counter = (step, 0, 0, 0)) -> 53-bit uniform, over the kept tokens in
 //      descending v, ties by ascending token id.
+// vsb_sample_rows_f32 takes one temperature / top_k / top_p / step for every row; vsb_sample_rows_var_f32 (the decode stream)
+// reads them per row from device arrays.  Both run the same kernel template, so a row draws the same token through either.
 // Fast path (<= kCap candidates, every default top_k = 50 row that is not a wide tie): compact the candidates into shared
 // memory, bitonic-sort them, scan their masses.  Otherwise (no top-k on a row wider than kCap, or a tie wider than kCap at the
 // k-th value): binary searches over the row's keys, each probe one block-reduced pass over the row; tokens of one key share one
@@ -109,9 +111,13 @@ __device__ __forceinline__ int count_eq(const float* row, int n, float T, uint32
   return r;
 }
 
-template <bool F16>
+// PER_ROW: temperature, top_k, top_p and step come from the row's entry of the device arrays (a decode stream, every request at
+// its own step with its own settings); otherwise from the scalar arguments, and the arrays are not read.
+template <bool F16, bool PER_ROW>
 __global__ void __launch_bounds__(kThreads, 1) sample_rows_kernel(const float* __restrict__ logits, long long ld, int n, float T, int top_k,
                                                                float top_p, const long long* __restrict__ seeds, int step,
+                                                               const float* __restrict__ T_row, const int* __restrict__ top_k_row,
+                                                               const float* __restrict__ top_p_row, const int* __restrict__ step_row,
                                                                int* __restrict__ out) {
   __shared__ unsigned long long cand[kCap];              // (key << 32) | ~id: descending order = v desc, id asc
   __shared__ double cum[kCap];
@@ -124,6 +130,12 @@ __global__ void __launch_bounds__(kThreads, 1) sample_rows_kernel(const float* _
 
   const int t = threadIdx.x, lane = t & 31, w = t >> 5;
   const float* row = logits + (long long)blockIdx.x * ld;
+  if (PER_ROW) {
+    T = T_row[blockIdx.x];
+    top_k = top_k_row[blockIdx.x];
+    top_p = top_p_row[blockIdx.x];
+    step = step_row[blockIdx.x];
+  }
   if (t == 0) {
     const unsigned long long seed = (unsigned long long)seeds[blockIdx.x];
     uint32_t c[4] = {(uint32_t)step, 0u, 0u, 0u};
@@ -305,6 +317,20 @@ __global__ void __launch_bounds__(kThreads, 1) sample_rows_kernel(const float* _
   }
 }
 
+template <bool PER_ROW>
+void launch_sample_rows(const void* logits, long long ld, int rows, int n, float temperature, int top_k, float top_p, int logit_dtype,
+                        const void* seeds, int step, const void* T_row, const void* top_k_row, const void* top_p_row,
+                        const void* step_row, void* idx, void* stream) {
+  if (logit_dtype == VSB_DTYPE_F16)
+    sample_rows_kernel<true, PER_ROW><<<rows, kThreads, 0, STREAM(stream)>>>(
+        (const float*)logits, ld, n, temperature, top_k, top_p, (const long long*)seeds, step, (const float*)T_row,
+        (const int*)top_k_row, (const float*)top_p_row, (const int*)step_row, (int*)idx);
+  else
+    sample_rows_kernel<false, PER_ROW><<<rows, kThreads, 0, STREAM(stream)>>>(
+        (const float*)logits, ld, n, temperature, top_k, top_p, (const long long*)seeds, step, (const float*)T_row,
+        (const int*)top_k_row, (const float*)top_p_row, (const int*)step_row, (int*)idx);
+}
+
 }  // namespace
 
 extern "C" int vsb_sample_rows_f32(const void* logits, long long ld, int rows, int n, float temperature, int top_k, float top_p,
@@ -315,12 +341,21 @@ extern "C" int vsb_sample_rows_f32(const void* logits, long long ld, int rows, i
   VSB_CHECK_ARG(top_p >= 0.f && top_p <= 1.f, "vsb_sample_rows_f32: top_p must be in [0, 1] (1 = no nucleus filter)");
   VSB_CHECK_ARG(logit_dtype == VSB_DTYPE_BF16 || logit_dtype == VSB_DTYPE_F16, "vsb_sample_rows_f32: logit_dtype must be VSB_DTYPE_BF16 or VSB_DTYPE_F16");
   if (rows <= 0) return VSB_OK;
-  if (logit_dtype == VSB_DTYPE_F16)
-    sample_rows_kernel<true><<<rows, kThreads, 0, STREAM(stream)>>>((const float*)logits, ld, n, temperature, top_k, top_p,
-                                                                    (const long long*)seeds_i64, step, (int*)idx_i32);
-  else
-    sample_rows_kernel<false><<<rows, kThreads, 0, STREAM(stream)>>>((const float*)logits, ld, n, temperature, top_k, top_p,
-                                                                     (const long long*)seeds_i64, step, (int*)idx_i32);
+  launch_sample_rows<false>(logits, ld, rows, n, temperature, top_k, top_p, logit_dtype, seeds_i64, step, nullptr, nullptr, nullptr,
+                            nullptr, idx_i32, stream);
+  VSB_LAUNCH_CHECK();
+  return VSB_OK;
+}
+
+extern "C" int vsb_sample_rows_var_f32(const void* logits, long long ld, int rows, int n, const void* temperature_f32,
+                                       const void* top_k_i32, const void* top_p_f32, int logit_dtype, const void* seeds_i64,
+                                       const void* steps_i32, void* idx_i32, void* stream) {
+  VSB_CHECK_ARG(logits && temperature_f32 && top_k_i32 && top_p_f32 && seeds_i64 && steps_i32 && idx_i32 && n > 0 && ld >= n,
+                "vsb_sample_rows_var_f32: bad args");
+  VSB_CHECK_ARG(logit_dtype == VSB_DTYPE_BF16 || logit_dtype == VSB_DTYPE_F16, "vsb_sample_rows_var_f32: logit_dtype must be VSB_DTYPE_BF16 or VSB_DTYPE_F16");
+  if (rows <= 0) return VSB_OK;
+  launch_sample_rows<true>(logits, ld, rows, n, 0.f, 0, 1.f, logit_dtype, seeds_i64, 0, temperature_f32, top_k_i32, top_p_f32, steps_i32,
+                           idx_i32, stream);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }

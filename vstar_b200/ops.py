@@ -499,16 +499,23 @@ def cast_f32(x, dtype, out=None):
     return out
 
 
-def argmax_rows(x):
+def argmax_rows(x, out=None):
     """fp32 x [rows, n] (unit inner stride) -> (idx int32 [rows], val fp32 [rows] = x[row, idx]), the index torch.argmax
-    returns: the first maximum, where NaN counts as larger than every number (the first NaN wins)"""
+    returns: the first maximum, where NaN counts as larger than every number (the first NaN wins).  out: idx buffer"""
     _chk(x, torch.float32)
     p, rows, n, ld = _rows2d(x)
-    idx = torch.empty((rows,), dtype=torch.int32, device=x.device)
+    idx = _idx_out(out, rows, x.device)
     val = torch.empty((rows,), dtype=torch.float32, device=x.device)
     _lib.launches += 1
     call("vsb_argmax_rows_f32", p, ld, rows, n, idx.data_ptr(), val.data_ptr(), _stream())
     return idx, val
+
+
+def _idx_out(out, rows, device):
+    if out is None:
+        return torch.empty((rows,), dtype=torch.int32, device=device)
+    assert out.dtype == torch.int32 and out.shape == (rows,) and out.is_contiguous()
+    return out
 
 
 def sample_rows(x, temperature, top_k, top_p, dtype, seeds, step):
@@ -525,6 +532,24 @@ def sample_rows(x, temperature, top_k, top_p, dtype, seeds, step):
     _lib.launches += 1
     call("vsb_sample_rows_f32", p, ld, rows, n, float(temperature), int(top_k), 1.0 if top_p is None else float(top_p),
          1 if dtype == F16 else 0, seeds.data_ptr(), int(step), idx.data_ptr(), _stream())
+    return idx
+
+
+def sample_rows_var(x, temperature, top_k, top_p, dtype, seeds, steps, out=None):
+    """sample_rows with every row's own settings (vsb_sample_rows_var_f32): temperature fp32, top_k int32 (0 = off), top_p
+    fp32 (1 = off), seeds int64 and steps int32, each [rows] on the device -> idx int32 [rows] (or into `out`).  The settings
+    are not checked on the device: the caller validates them (vqa.check_sampling, temperature > 0)."""
+    _chk(x, torch.float32)
+    p, rows, n, ld = _rows2d(x)
+    for t, dt in ((temperature, torch.float32), (top_k, torch.int32), (top_p, torch.float32), (seeds, torch.int64), (steps, torch.int32)):
+        _chk(t, dt)
+        assert t.shape == (rows,) and t.is_contiguous()
+    if dtype not in _SUFFIX:
+        raise _lib.VsbError(f"unsupported dtype {dtype}: the logits are rounded to bf16 or fp16")
+    idx = _idx_out(out, rows, x.device)
+    _lib.launches += 1
+    call("vsb_sample_rows_var_f32", p, ld, rows, n, temperature.data_ptr(), top_k.data_ptr(), top_p.data_ptr(), 1 if dtype == F16 else 0,
+         seeds.data_ptr(), steps.data_ptr(), idx.data_ptr(), _stream())
     return idx
 
 
@@ -572,6 +597,20 @@ def copy_cache_rows(cache, pairs, lo, hi):
         _lib.launches += 1
         call("vsb_copy_cache_rows_b16", cache.data_ptr(), L, cache.stride(0), B, cache.stride(1), cache.stride(2), W, arr, len(chunk),
              int(lo), int(hi), _stream())
+    return cache
+
+
+def copy_slot_rows(cache, quads):
+    """copy_cache_rows with a row range per pair: rows [lo, hi) of every layer from slot s to slot d for every (s, d, lo, hi) in
+    the host list `quads`, in one vsb_copy_slot_rows_b16 launch (at most COPY_ROWS_MAX_PAIRS pairs).  A slot that is both a
+    source and a destination, a destination named twice, a slot outside the cache or lo > hi raises VsbError."""
+    import ctypes
+    _chk(cache)
+    assert cache.dim() == 4 and cache.element_size() == 2 and cache.stride(3) == 1
+    L, B, _, W = cache.shape
+    arr = (ctypes.c_int * (4 * max(1, len(quads))))(*[int(v) for q in quads for v in q])
+    _lib.launches += 1
+    call("vsb_copy_slot_rows_b16", cache.data_ptr(), L, cache.stride(0), B, cache.stride(1), cache.stride(2), W, arr, len(quads), _stream())
     return cache
 
 

@@ -18,6 +18,8 @@ free_form_inference(temperature > 0, top_p) samples like the reference's `genera
 launch per decode step in place of the greedy argmax (oracle/sampling_oracle.py; DESIGN.md §7b).
 free_form_inference(num_beams = k) runs HF's beam search (transformers 4.31): VQAEngine.beam_search, one vsb_beam_candidates_f32
 launch per step and copy-on-fork KV-row copies (vstar_b200/beam.py, oracle/beam_oracle.py; DESIGN.md §7b).
+DecodeStream.admit takes the same settings per request, so one decode stream mixes greedy, sampled and beam requests
+(vsb_sample_rows_var_f32, vsb_copy_slot_rows_b16; DESIGN.md §7b).
 """
 from __future__ import annotations
 
@@ -25,7 +27,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .beam import DEFAULT_EARLY_STOPPING, DEFAULT_LENGTH_PENALTY, BeamRequest, check_beams
+from .beam import DEFAULT_EARLY_STOPPING, DEFAULT_LENGTH_PENALTY, BeamRequest, check_beams, fork_slots
 from .config import VSMConfig
 from .engine import CoreWeights, LlamaClipCore
 from .vsm import CLIP_MEAN, SyntheticTokenizer, _normalize_into
@@ -248,7 +250,7 @@ class VQAEngine(LlamaClipCore):
             return None
         top_k, top_p = check_sampling(top_k, top_p)
         seeds = draw_seeds(1) if seeds is None else seeds
-        sd = torch.tensor([(int(s) + (1 << 63)) % (1 << 64) - (1 << 63) for s in seeds], dtype=torch.int64, device=self.dev)   # any 64 bits
+        sd = torch.tensor([_signed64(s) for s in seeds], dtype=torch.int64, device=self.dev)
         T, dtype = float(temperature), self.dtype
         return lambda logits, step: ops.sample_rows(logits, T, top_k, top_p, dtype, sd, step)
 
@@ -360,13 +362,16 @@ class VQAEngine(LlamaClipCore):
         return res
 
     def decode_stream(self, max_slots, max_positions=None, eos_token_id=2, temperature=0, num_beams=1):
-        """Greedy decode batch that admits a request whenever a slot is free (DecodeStream).  max_positions: cache rows per slot
-        (default self.max_tokens); a request's prompt plus its max_new_tokens must fit in them.  Sampling (temperature > 0)
-        and beam search (num_beams > 1) are refused: the stream steps every slot with one argmax."""
+        """Decode batch that admits a request whenever a slot is free (DecodeStream).  max_positions: cache rows per slot
+        (default self.max_tokens); a request's prompt plus its max_new_tokens must fit in them.  Generation settings belong to
+        each request: DecodeStream.admit(..., temperature=, top_k=, top_p=, seed=, num_beams=, ...) samples or beam-searches
+        it; the stream-wide temperature > 0 and num_beams > 1 are refused, since every sampled request needs its own seed."""
         if temperature is not None and temperature > 0:
-            raise NotImplementedError("decode_stream decodes greedily: temperature > 0 (sampling) is not supported")
+            raise NotImplementedError("decode_stream takes no stream-wide temperature: sample a request with "
+                                      "DecodeStream.admit(..., temperature=, top_k=, top_p=, seed=)")
         if num_beams != 1:
-            raise NotImplementedError("decode_stream decodes greedily: num_beams > 1 (beam search) is not supported")
+            raise NotImplementedError("decode_stream takes no stream-wide num_beams: beam-search a request with "
+                                      "DecodeStream.admit(..., num_beams=, length_penalty=, early_stopping=)")
         return DecodeStream(self, max_slots, self.max_tokens if max_positions is None else max_positions, eos_token_id)
 
     def spliced_length(self, input_ids, n_crops=0, images_long=None, objects_long=None):
@@ -446,18 +451,9 @@ class VQAEngine(LlamaClipCore):
                 if q.done:
                     continue
                 nxt = q.process(list(zip(sc[r], tok[r], bm[r])))
-                old = beam_slot[r]
-                parents = {b for _, _, b in nxt}
-                free = [s for s in owned[r] if s not in {old[p] for p in parents}]
-                new, claimed = [], set()
-                for _, t, p in nxt:
-                    if p not in claimed:                    # the parent's first child keeps its slot
-                        claimed.add(p)
-                        s = old[p]
-                    else:                                   # later children fork into the slot of a beam that died
-                        s = free.pop(0)
-                        pairs.append((old[p], s))
-                    new.append(s)
+                new, forks = fork_slots(beam_slot[r], nxt, owned[r])
+                pairs += forks
+                for s, (_, t, _) in zip(new, nxt):
                     tokens[s] = t
                 beam_slot[r] = new
             if all(q.done for q in reqs) or step == max_new_tokens - 1:
@@ -558,28 +554,57 @@ class VQAEngine(LlamaClipCore):
 
 
 class StreamRequest:
-    """handle of a request admitted to a DecodeStream: `tokens` grows by one id per step, `done` once it ended"""
+    """handle of a request admitted to a DecodeStream: `tokens` grows by one id per step, `done` once it ended.
+    A beam request (num_beams = k > 1) holds k cache `slots` (`slot` is the first); `beams` are its running beams' new ids while
+    it decodes, and once it is done `tokens` / `score` are its chosen hypothesis' ids (eos appended as beam_search returns them)
+    and score."""
 
-    def __init__(self, rid, slot, length, max_new_tokens, stop_ids):
+    def __init__(self, rid, slot, length, max_new_tokens, stop_ids, temperature=0, top_k=0, top_p=None, seed=None, beam=None,
+                 slots=None):
         self.id, self.slot, self.prompt_len = rid, slot, length
         self.max_new_tokens, self.stop_ids = max_new_tokens, list(stop_ids) if stop_ids else None
         self.tokens, self.done = [], False
+        self.temperature, self.top_k, self.top_p, self.seed = temperature, top_k, top_p, seed     # temperature > 0: sampled
+        self.beam = beam                                 # BeamRequest of a beam request
+        self.slots = [slot] if slots is None else list(slots)
+        self.beam_slot = [slot]                          # cache slot of each running beam, in beam order
+        self.score = None
+
+    @property
+    def kind(self):
+        return "beam" if self.beam is not None else "sample" if self.temperature > 0 else "greedy"
+
+    @property
+    def beams(self):
+        return None if self.beam is None else [list(b) for b in self.beam.beams]
 
     def __repr__(self):
-        return f"StreamRequest(id={self.id}, slot={self.slot}, tokens={len(self.tokens)}, done={self.done})"
+        return f"StreamRequest(id={self.id}, slot={self.slot}, kind={self.kind}, tokens={len(self.tokens)}, done={self.done})"
+
+
+def _signed64(seed):
+    """any integer seed -> the int64 with the same low 64 bits (the sampler's seed argument)"""
+    return (int(seed) + (1 << 63)) % (1 << 64) - (1 << 63)
 
 
 class DecodeStream:
-    """Greedy decoding of many requests on a decode batch that admits a new request whenever a slot frees (iteration-level
+    """Decoding of many requests on a decode batch that admits a new request whenever a slot frees (iteration-level
     admission), instead of generate_batch's static batch that steps until its longest answer ends.
 
     The stream owns its KV cache [n_layers, max_slots, max_positions, 3d], separate from the engine's, so option scoring,
     generate() or a VSM call in between neither disturbs it nor is disturbed by it.  A request is prefilled alone into a free
     slot at rows [0, T) and takes its first token from the prefill logits, as in generate().  Every step() then runs ONE
-    vsb_llama_layers_slots call for all active slots (each row writes its new q|k|v at its own slot and length and attends
-    only its own keys), one argmax_rows launch and one device-to-host copy.  A request ends at eos, at its stop_ids (the rule of
-    generate_batch) or after its own max_new_tokens, and its slot is free for the next admit().  In batch-invariant mode
-    (ops.batch_invariant) a request's logits do not depend on the other requests in the batch or on its slot."""
+    vsb_llama_layers_slots call for all active rows (each row writes its new q|k|v at its own slot and length and attends
+    only its own keys) and selects every row's next token into one device buffer, read by one device-to-host copy.  A request
+    ends at eos, at its stop_ids (the rule of generate_batch) or after its own max_new_tokens, and its slot is free for the
+    next admit().  In batch-invariant mode (ops.batch_invariant) a request's logits do not depend on the other requests in the
+    batch or on its slot.
+
+    Each request brings its own generation settings (admit): greedy (argmax_rows), sampled (temperature > 0: one
+    vsb_sample_rows_var_f32 launch for every sampled row, each with its own temperature / top_k / top_p / seed / step) or beam
+    search (num_beams = k: the request holds k slots; one vsb_beam_candidates_f32 launch per distinct k, and the forked beams'
+    generated rows move by one vsb_copy_slot_rows_b16 launch).  Rows are ordered greedy, sampled, beam, each kind in slot
+    order, so a greedy-only stream issues the launches it always did."""
 
     def __init__(self, engine, max_slots, max_positions, eos_token_id=2):
         max_slots, max_positions = int(max_slots), int(max_positions)
@@ -596,7 +621,7 @@ class DecodeStream:
         self._cache = torch.empty((c.n_layers, max_slots, max_positions, 3 * c.hidden), dtype=dt, device=dev)
         self._scratch = torch.empty((max_slots * (5 * c.hidden + c.intermediate),), dtype=dt, device=dev)
         self._deq = torch.empty((2 * c.intermediate * c.hidden,), dtype=dt, device=dev) if getattr(engine.w, "quant", None) else None
-        self._slots = [None] * max_slots                 # slot -> active StreamRequest
+        self._slots = [None] * max_slots                 # slot -> active StreamRequest (a beam request in each of its slots)
         self._finished = []                              # ended at admission; reported by the next step()
         self._next_id = 0
         self.steps = 0
@@ -609,7 +634,13 @@ class DecodeStream:
 
     @property
     def active(self):
-        return [r for r in self._slots if r is not None]
+        """the running requests, in order of their first slot"""
+        out, seen = [], set()
+        for r in self._slots:
+            if r is not None and r.id not in seen:
+                seen.add(r.id)
+                out.append(r)
+        return out
 
     def _check_open(self):
         if self._cache is None:
@@ -619,22 +650,56 @@ class DecodeStream:
         t = r.tokens
         return t[-1] == self.eos or (r.stop_ids and t[-len(r.stop_ids):] == r.stop_ids) or len(t) >= r.max_new_tokens
 
-    def admit(self, request, max_new_tokens, stop_ids=None):
+    def _release(self, r):
+        r.done = True
+        for s in r.slots:
+            self._slots[s] = None
+
+    def _beam_advance(self, r, cand):
+        """one beam-search step of request r on its 2k candidates [(score, token, beam)] -> the (src, dst, lo, hi) row copies of
+        its forks, or None when it ended (tokens / score then hold its chosen hypothesis)"""
+        q = r.beam
+        n = len(q.beams[0])                              # tokens every beam had before this step: rows [T, T + n) are cached
+        nxt = q.process(cand)
+        r.beam_slot, forks = fork_slots(r.beam_slot, nxt, r.slots)
+        if q.done or len(q.beams[0]) >= r.max_new_tokens:
+            r.tokens, r.score = q.finalize()
+            return None
+        return [(a, b, r.prompt_len, r.prompt_len + n) for a, b in forks] if n else []
+
+    def admit(self, request, max_new_tokens, stop_ids=None, *, temperature=0, top_k=DEFAULT_TOP_K, top_p=None, seed=None, num_beams=1,
+              length_penalty=DEFAULT_LENGTH_PENALTY, early_stopping=DEFAULT_EARLY_STOPPING):
         """request = (input_ids, image, object_crops, images_long, objects_long) as generate_batch takes it -> StreamRequest.
-        Raises (before any launch) when no slot is free or the prompt plus max_new_tokens exceeds max_positions."""
+        The settings are generate()'s for this request alone: greedy by default; temperature > 0 samples with top_k / top_p
+        (check_sampling), token t drawn with (seed, step t), seed None = one draw from torch's default generator;
+        num_beams = k > 1 runs beam_search's scorer with length_penalty / early_stopping on k slots (stop_ids at most [eos]),
+        its first candidates selected here from the prefill logits.  Raises (before any launch) on settings generate() refuses,
+        when fewer than num_beams slots are free, num_beams exceeds max_slots or the prompt plus max_new_tokens exceeds
+        max_positions."""
         self._check_open()
         ids, image, crops, il, ol = request
         max_new_tokens = int(max_new_tokens)
         if max_new_tokens < 1:
             raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
         e = self.engine
+        beam = e._beam_args(num_beams, temperature, stop_ids, self.eos, early_stopping)
+        sample = not beam and temperature is not None and temperature > 0
+        if sample:
+            top_k, top_p = check_sampling(top_k, top_p)
+        k = num_beams
+        if k > self.max_slots:
+            raise ValueError(f"num_beams = {k} needs {k} slots, the decode stream has {self.max_slots}")
         T = e.spliced_length(ids, 0 if crops is None else int(crops.shape[0]), il, ol)
         if T + max_new_tokens > self.max_positions:
             raise ops._lib.VsbError(f"prompt of {T} rows + {max_new_tokens} new tokens exceeds the stream's {self.max_positions} "
                                     "positions per slot")
-        if self.free_slots == 0:
-            raise RuntimeError(f"no free slot: all {self.max_slots} slots of the decode stream are in use")
-        slot = self._slots.index(None)
+        if self.free_slots < k:
+            raise RuntimeError(f"no free slot: all {self.max_slots} slots of the decode stream are in use" if k == 1 else
+                               f"no free slot for {k} beams: {self.free_slots} of the decode stream's {self.max_slots} slots are free")
+        if sample and seed is None:
+            seed = draw_seeds(1)[0]
+        slots = [i for i, r in enumerate(self._slots) if r is None][:k]
+        slot = slots[0]
         x = e.build_embeds(ids, image, crops, il, ol)
         assert x.shape[0] == T
         c = e.cfg
@@ -644,15 +709,29 @@ class DecodeStream:
                          c.rms_eps, e.w.rope_cos, e.w.rope_sin, scratch, cache_row_offset=slot * Tm,
                          norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
         _, idx, logits = e._logits_rows(x, torch.tensor([T - 1], dtype=torch.int64, device=e.dev))
-        r = StreamRequest(self._next_id, slot, T, max_new_tokens, stop_ids)
+        r = StreamRequest(self._next_id, slot, T, max_new_tokens, stop_ids, temperature=float(temperature) if sample else 0,
+                          top_k=top_k if sample else 0, top_p=top_p if sample else None, seed=seed if sample else None,
+                          beam=BeamRequest(k, len(ids), max_new_tokens, self.eos, length_penalty, early_stopping) if beam else None,
+                          slots=slots)
         self._next_id += 1
         self.last_logits = ([r], logits)
-        r.tokens.append(int(idx[0]))
-        if self._ended(r):
-            r.done = True
-            self._finished.append(r)
+        for s in slots:
+            self._slots[s] = r
+        if beam:
+            ops.copy_slot_rows(self._cache, [(slot, s, 0, T) for s in slots[1:]])          # the prompt rows of the other beams
+            dev = e.dev
+            cand = ops.beam_candidates(logits, torch.zeros((1, 1), dtype=torch.int32, device=dev),
+                                       torch.zeros((1, 1), dtype=torch.float32, device=dev), k, e.dtype).cpu()
+            ended = self._beam_advance(r, list(zip(cand[0, 0].view(torch.float32).tolist(), cand[1, 0].tolist(), cand[2, 0].tolist()))) is None
         else:
-            self._slots[slot] = r
+            if sample:
+                sd = torch.tensor([_signed64(seed)], dtype=torch.int64, device=e.dev)
+                idx = ops.sample_rows(logits, r.temperature, top_k, top_p, e.dtype, sd, 0)
+            r.tokens.append(int(idx[0]))
+            ended = self._ended(r)
+        if ended:
+            self._release(r)
+            self._finished.append(r)
         return r
 
     def step(self):
@@ -664,27 +743,90 @@ class DecodeStream:
         if not act:
             return done
         e, c = self.engine, self.engine.cfg
-        B = len(act)
-        lens = [r.prompt_len + len(r.tokens) - 1 for r in act]        # rows cached; the newest token goes to row `len`
-        meta = torch.tensor([[r.slot for r in act], lens, lens], dtype=torch.int32).to(e.dev)
-        ids = torch.tensor([r.tokens[-1] for r in act], dtype=torch.int64).to(e.dev)
+        greedy = [r for r in act if r.kind == "greedy"]
+        sampled = [r for r in act if r.kind == "sample"]
+        beams = [r for r in act if r.kind == "beam"]
+        # rows (request, slot, rows cached, newest token): the newest token goes to row `rows cached` of the slot
+        rows = [(r, r.slot, r.prompt_len + len(r.tokens) - 1, r.tokens[-1]) for r in greedy + sampled]
+        first = {}                                       # beam request -> its first logits row
+        for r in beams:
+            first[r.id] = len(rows)
+            n = r.prompt_len + len(r.beam.beams[0]) - 1
+            rows += [(r, s, n, b[-1]) for s, b in zip(r.beam_slot, r.beam.beams)]
+        B = len(rows)
+        lens = [n for _, _, n, _ in rows]
+        meta = torch.tensor([[s for _, s, _, _ in rows], lens, lens], dtype=torch.int32).to(e.dev)
+        ids = torch.tensor([t for _, _, _, t in rows], dtype=torch.int64).to(e.dev)
         x = ops.gather_rows(ids, e.w.embed)
         ops.llama_layers_slots(e._layer_table, len(e.w.layers), x, self._cache, c.rms_eps, e.w.rope_cos, e.w.rope_sin, self._scratch,
                                meta[0], meta[1], meta[2], max(lens), c.n_heads, c.intermediate,
                                norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
         hn = ops.rmsnorm(x, e.w.final_norm, c.rms_eps)
         logits = ops.gemm(hn, e.w.lm_head, out_dtype=torch.float32)
-        nxt = ops.argmax_rows(logits)[0].tolist()                       # the one device-to-host copy of the step
-        self.last_logits = (act, logits)
+        G, S = len(greedy), len(sampled)
+        groups = {}                                      # k -> beam requests of that k, in row order
+        for r in beams:
+            groups.setdefault(r.beam.k, []).append(r)
+        sel = torch.empty((G + S + sum(3 * len(g) * 2 * k for k, g in groups.items()),), dtype=torch.int32, device=e.dev)
+        if G:
+            ops.argmax_rows(logits[:G], out=sel[:G])
+        if S or beams:
+            self._select(logits, G, sampled, groups, first, sel)
+        h = sel.cpu()                                    # the one device-to-host copy of the step
+        self.last_logits = ([r for r, _, _, _ in rows], logits)
         self.steps += 1
         self.occupied += B
-        for r, t in zip(act, nxt):
+        for r, t in zip(greedy + sampled, h[:G + S].tolist()):
             r.tokens.append(int(t))
             if self._ended(r):
-                r.done = True
-                self._slots[r.slot] = None
+                self._release(r)
                 done.append((r, r.tokens))
+        off, quads = G + S, []
+        for k, g in groups.items():
+            R = len(g)
+            cand = h[off:off + 3 * R * 2 * k].view(3, R, 2 * k)
+            off += 3 * R * 2 * k
+            sc, tok, bm = cand[0].view(torch.float32).tolist(), cand[1].tolist(), cand[2].tolist()
+            for i, r in enumerate(g):
+                q = self._beam_advance(r, list(zip(sc[i], tok[i], bm[i])))
+                if q is None:
+                    self._release(r)
+                    done.append((r, r.tokens))
+                else:
+                    quads += q
+        for i in range(0, len(quads), ops.COPY_ROWS_MAX_PAIRS):
+            ops.copy_slot_rows(self._cache, quads[i:i + ops.COPY_ROWS_MAX_PAIRS])
         return done
+
+    def _select(self, logits, G, sampled, groups, first, sel):
+        """the sampled and beam rows' selections into sel[G:] (after the greedy rows' tokens): one per-row sampler launch for
+        rows [G, G + S), then one candidate launch per beam width k (first: each beam request's first logits row); their
+        settings travel in one host-to-device copy"""
+        e, S = self.engine, len(sampled)
+        nb = sum(len(g) * k for k, g in groups.items())
+        host = np.empty(6 * S + 2 * nb, dtype=np.int32)                       # seeds (int64) first, so their view is aligned
+        host[:2 * S].view(np.int64)[:] = [_signed64(r.seed) for r in sampled]
+        host[2 * S:3 * S].view(np.float32)[:] = [r.temperature for r in sampled]
+        host[3 * S:4 * S] = [r.top_k for r in sampled]
+        host[4 * S:5 * S].view(np.float32)[:] = [1.0 if r.top_p is None else r.top_p for r in sampled]
+        host[5 * S:6 * S] = [len(r.tokens) for r in sampled]                  # token t is drawn at step t
+        o, spans = 6 * S, []
+        for k, g in groups.items():
+            n = len(g) * k
+            host[o:o + n] = [first[r.id] + b for r in g for b in range(k)]   # each request's beams, in beam order
+            host[o + n:o + 2 * n].view(np.float32)[:] = [s for r in g for s in r.beam.scores]
+            spans.append((k, len(g), o, n))
+            o += 2 * n
+        dev = torch.from_numpy(host).to(e.dev)
+        if S:
+            ops.sample_rows_var(logits[G:G + S], dev[2 * S:3 * S].view(torch.float32), dev[3 * S:4 * S],
+                                dev[4 * S:5 * S].view(torch.float32), e.dtype, dev[:2 * S].view(torch.int64), dev[5 * S:6 * S],
+                                out=sel[G:G + S])
+        off = G + S
+        for k, R, o, n in spans:
+            ops.beam_candidates(logits, dev[o:o + n].view(R, k), dev[o + n:o + 2 * n].view(torch.float32).view(R, k), k, e.dtype,
+                                out=sel[off:off + 3 * R * 2 * k].view(3, R, 2 * k))
+            off += 3 * R * 2 * k
 
     def close(self):
         """free the stream's cache and scratch (requests still running are abandoned)"""
@@ -1017,28 +1159,51 @@ class VQA_LLM:
         return text.strip()
 
     @torch.inference_mode()
-    def free_form_inference_stream(self, items, max_new_tokens=200, slots=16):
-        """free_form_inference (greedy) for many items on one decode stream (VQAEngine.decode_stream): items are (image,
-        question, object_crops, images_long, objects_long); yields (index, text) as each answer completes, with the prompt,
-        stop string and post-processing of free_form_inference.  The next item is admitted whenever a slot frees, so up to
-        `slots` answers decode together however much their lengths differ.  As in free_form_inference, an answer whose prompt
-        plus max_new_tokens would pass the 2048 positions of the RoPE tables gets the positions that are left."""
+    def free_form_inference_stream(self, items, max_new_tokens=200, slots=16, temperature=0, top_p=None, num_beams=1):
+        """free_form_inference for many items on one decode stream (VQAEngine.decode_stream): items are (image, question,
+        object_crops, images_long, objects_long); yields (index, text) as each answer completes, with the prompt, stop string
+        and post-processing of free_form_inference.  The next item is admitted whenever a slot frees, so up to `slots` answers
+        decode together however much their lengths differ.  As in free_form_inference, an answer whose prompt plus
+        max_new_tokens would pass the 2048 positions of the RoPE tables gets the positions that are left.
+        temperature > 0 samples every item with top_k = self.top_k and top_p; the items take one seed each from torch's
+        default generator, in item order, before the first admission (so torch.manual_seed(s) reproduces a call, and a call
+        equals free_form_inference of each item in order after the same seed).  num_beams = k > 1 beam-searches every item
+        with self.length_penalty / self.early_stopping on k slots; an item is admitted when k slots are free."""
         reqs = [(self._prompt_ids(question), image, crops, il, ol) for image, question, crops, il, ol in items]
-        for i, out in self._decode_stream(reqs, int(max_new_tokens), int(slots)):
+        if (temperature is None or not temperature > 0) and num_beams == 1:
+            answers = self._decode_stream(reqs, int(max_new_tokens), int(slots))
+        else:
+            answers = self._decode_stream(reqs, int(max_new_tokens), int(slots), settings=self._stream_settings(len(reqs), temperature,
+                                                                                                            top_p, num_beams))
+        for i, out in answers:
             yield i, self._answer_text(out)
 
-    def _decode_stream(self, reqs, max_new_tokens, slots):
+    def _stream_settings(self, n, temperature, top_p, num_beams):
+        """DecodeStream.admit keywords of n sampled or beam requests, validated and seeded as free_form_inference does"""
+        if num_beams != 1:
+            check_beams(num_beams, self.early_stopping)
+            if temperature is not None and temperature > 0:
+                raise NotImplementedError("num_beams > 1 with temperature > 0 (HF beam_sample) is not implemented")
+            return [dict(num_beams=num_beams, length_penalty=self.length_penalty, early_stopping=self.early_stopping)] * n
+        top_k, top_p = check_sampling(self.top_k, top_p)
+        return [dict(temperature=temperature, top_k=top_k, top_p=top_p, seed=s) for s in draw_seeds(n)]
+
+    def _decode_stream(self, reqs, max_new_tokens, slots, settings=None):
         """(prompt ids, image, object_crops, images_long, objects_long) requests -> (index, new token ids) as each ends, on one
-        decode stream with min(slots, len(reqs)) slots"""
+        decode stream with min(slots, len(reqs) * num_beams) slots.  settings: per request, DecodeStream.admit's generation
+        keywords (None: greedy)"""
         if not reqs:
             return
         e = self.engine
         kw = self._stop_ids()
+        need = settings[0].get("num_beams", 1) if settings else 1
+        if need > slots:
+            raise ValueError(f"num_beams = {need} needs {need} slots, got slots = {slots}")
         lens = [e.spliced_length(ids, 0 if crops is None else len(crops), il, ol) for ids, _, crops, il, ol in reqs]
         # generate() reserves min(max_new_tokens, 2048 - T) positions: the same budget here
         budgets = [max(1, min(max_new_tokens, e.MAX_POSITIONS - T)) for T in lens]
         positions = min(e.MAX_POSITIONS, max(T + n for T, n in zip(lens, budgets)))
-        stream = e.decode_stream(min(slots, len(reqs)), positions, self.eos)
+        stream = e.decode_stream(min(slots, len(reqs) * need), positions, self.eos)
         try:
             index = {}
             nxt = 0
@@ -1047,17 +1212,20 @@ class VQA_LLM:
                 nonlocal nxt
                 ids, image, crops, il, ol = reqs[nxt]
                 img, crops = self._pixels(image, crops)
-                index[stream.admit((ids, img, crops, il, ol), budgets[nxt], stop_ids=kw).id] = nxt
+                gen = {} if settings is None else settings[nxt]
+                # beam hypotheses end at eos alone, as in free_form_inference(num_beams > 1)
+                stop = None if need > 1 else kw
+                index[stream.admit((ids, img, crops, il, ol), budgets[nxt], stop_ids=stop, **gen).id] = nxt
                 nxt += 1
 
-            while nxt < len(reqs) and stream.free_slots:
+            while nxt < len(reqs) and stream.free_slots >= need:
                 admit()
             remaining = len(reqs)
             while remaining:
                 for r, out in stream.step():
                     remaining -= 1
                     yield index[r.id], out
-                while nxt < len(reqs) and stream.free_slots:
+                while nxt < len(reqs) and stream.free_slots >= need:
                     admit()
         finally:
             stream.close()
