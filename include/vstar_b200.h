@@ -251,6 +251,38 @@ int vsb_rope_scatter(const void* qkv, long long ldq, int B, int H, int D, void* 
 int vsb_attn_decode_slots(const void* q, const void* k, const void* v, void* o, long long slot_stride, long long row_stride, long long o_rs,
                           int B, int H, int D, float scale, const void* slot_i32, const void* len_i32, int max_len, int dtype, void* stream);
 
+/* Paged slot decode: the KV cache is a pool of pages of page_rows k|v rows (2d elements per row: k then v), page_rows a power of
+ * two >= 16.  page_table_i32 is device int32 [*, pt_ld]; the row of slot s lists its pages, so key row j of slot s sits in page
+ * page_table[s*pt_ld + j/page_rows] at row j % page_rows.  Rows of different slots may name the same page (a beam request's
+ * shared prompt pages); the caller keeps the pages a step writes private to their slot.
+ * vsb_llama_layers_slots_paged: vsb_llama_layers_slots on the pool [n_layers][n_pages][page_rows][2d] (same tables, scratch,
+ * dtype and batch-invariant mode), with vsb_rope_scatter_paged / vsb_attn_decode_paged in place of the slot kernels; max_len <
+ * pt_ld*page_rows.  Each row's logits are bit-identical to vsb_llama_layers_slots on the same logical keys. */
+int vsb_llama_layers_slots_paged(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, void* pool, int n_pages, int page_rows,
+                                 const void* page_table_i32, int pt_ld, int d, int H, int inter, float rms_eps, const void* rope_cos,
+                                 const void* rope_sin, const void* slot_i32, const void* len_i32, const void* pos_i32, int max_len,
+                                 int norm_folded, void* scratch, void* deq_scratch, int dtype, void* stream);
+/* vsb_rope_scatter into pages: row b of qkv [B, 3*H*D] (row stride ldq) has q rotated IN PLACE and k rotated at position
+ * pos_i32[b]; k|v go to row len_i32[b] of slot slot_i32[b]'s pages (pool + page*page_stride + row*ldc). */
+int vsb_rope_scatter_paged(void* qkv, long long ldq, int B, int H, int D, void* pool, long long page_stride, long long ldc, int page_rows,
+                           const void* page_table_i32, int pt_ld, const void* slot_i32, const void* len_i32, const void* pos_i32,
+                           const void* cos_table, const void* sin_table, int dtype, void* stream);
+/* vsb_attn_decode_slots over pages: row b's query at q + b*q_rs, its keys / values [0, len[b]] at k / v + page*page_stride +
+ * row*row_stride through slot_i32[b]'s page-table row; output o + b*o_rs.  Same split rule, key chunks and combine as
+ * vsb_attn_decode_slots, so the two agree bit for bit on the same logical keys in both modes. */
+int vsb_attn_decode_paged(const void* q, long long q_rs, const void* k, const void* v, void* o, long long o_rs, long long page_stride,
+                          long long row_stride, int page_rows, const void* page_table_i32, int pt_ld, int B, int H, int D, float scale,
+                          const void* slot_i32, const void* len_i32, int max_len, int dtype, void* stream);
+/* vsb_copy_slot_rows_b16 into a paged pool [layers] (layer_stride) of pages: for every pair (src, dst, lo, hi) of the HOST array
+ * quads_i32, rows [lo, hi) of every layer are copied to page-table row dst's pages.  src NULL: the source is page-table row src of
+ * the pool (a beam fork; the slot rules of vsb_copy_slot_rows_b16 apply).  src set: a contiguous cache, row r of slot s at
+ * src + l*src_layer_stride + s*src_slot_stride + r*src_row_stride (a prefilled prompt written into its pages).  row_elems
+ * 2-byte elements per row; at most VSB_COPY_ROWS_MAX_PAIRS pairs, slots <= 65536; refusals before any launch.  One launch. */
+int vsb_copy_page_rows_b16(void* pool, int layers, long long layer_stride, long long page_stride, int page_rows, long long row_stride,
+                           int row_elems, const void* page_table_i32, int pt_ld, int slots, const void* src, long long src_layer_stride,
+                           long long src_slot_stride, long long src_row_stride, int src_slots, const int* quads_i32, int npairs,
+                           void* stream);
+
 /* NF4 weights: the SEAL VQA LLM's 4-bit mode (the reference's load_4bit: bitsandbytes NF4, double-quantised scales, fp16 compute,
  * LLaVA/llava/model/builder.py:26-43).  Format of W [N, K], K % 64 == 0 (csrc/nf4.cu, oracle/nf4_oracle.py): codes u8 [N, K/2], two
  * 4-bit codes per byte with the first element in the high nibble, one fp32 scale per 64-value block [N, K/64]; a weight is

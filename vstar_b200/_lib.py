@@ -86,6 +86,15 @@ SIGNATURES.update({
     "vsb_attn_decode_slots": [c_p, c_p, c_p, c_p, c_ll, c_ll, c_ll, c_i, c_i, c_i, c_f, c_p, c_p, c_i, c_i, c_p],
 })
 
+# paged slot decode (DecodeStream(kv_pages=N)): k|v rows in pages found through a device page table
+SIGNATURES.update({
+    "vsb_llama_layers_slots_paged": [c_p, c_i, c_p, c_i, c_p, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p,
+                                     c_p, c_i, c_p],
+    "vsb_rope_scatter_paged": [c_p, c_ll, c_i, c_i, c_i, c_p, c_ll, c_ll, c_i, c_p, c_i, c_p, c_p, c_p, c_p, c_p, c_i, c_p],
+    "vsb_attn_decode_paged": [c_p, c_ll, c_p, c_p, c_p, c_ll, c_ll, c_ll, c_i, c_p, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_i, c_i, c_p],
+    "vsb_copy_page_rows_b16": [c_p, c_i, c_ll, c_ll, c_i, c_ll, c_i, c_p, c_i, c_i, c_p, c_ll, c_ll, c_ll, c_i, c_p, c_i, c_p],
+})
+
 
 class LlamaLayer(ctypes.Structure):
     """vsb_llama_layer_t"""

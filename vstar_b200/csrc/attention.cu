@@ -12,6 +12,8 @@
 //  vsb_attn_small_bf16  : tiny-head attention of the SAM two-way transformer (head_dim 16 / 32, 6 tokens
 //                         <-> 2304 image tokens); CUDA-core kernel, fp32 math.
 //                         (/root/reference/VisualSearch/model/segment_anything/modeling/transformer.py:220-242)
+#include <type_traits>
+
 #include "common.cuh"
 #include "vstar_b200.h"
 
@@ -527,8 +529,23 @@ __device__ __forceinline__ int dec_row_splits(int nk, int cap) {
   return s;
 }
 
-template <int D, typename T>
-__global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_slots_kernel(const SlotAttnParams p) {
+// the paged form (vsb_attn_decode_paged): row b's keys / values live in pages of 2^page_shift rows, key j at page
+// page_table[slot[b]*pt_ld + (j >> page_shift)], row j & (page rows - 1); its query is row b of a separate q buffer (stride q_rs)
+struct PagedSlotAttnParams {
+  const void *q, *k, *v;
+  void* o;
+  long long page_stride, row_stride, o_rs, q_rs;
+  const int *slot, *len, *page_table;
+  float scale_log2;
+  int cap;
+  int pt_ld, page_shift;
+};
+
+// one body for both forms: only the addresses of q and of key row j differ, so a row's arithmetic (split rule, key chunks,
+// combine order) is the same in both and they agree bit for bit on the same logical keys
+template <int D, typename T, typename PRM>
+__device__ __forceinline__ void attn_decode_slots_body(const PRM& p) {
+  constexpr bool PAGED = std::is_same<PRM, PagedSlotAttnParams>::value;
   using E = ElemT<T>;
   pdl_prologue();
   constexpr int EPL = D / 32;
@@ -546,10 +563,27 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_slots_kernel(co
   const int chunk = (nk + nsplit - 1) / nsplit;
   const int k_begin = split < nsplit ? split * chunk : nk;
   const int k_end = min(nk, k_begin + chunk);
-  const long long base = (long long)p.slot[b] * p.slot_stride + (long long)h * D + lane * EPL;
-  const T* qb = reinterpret_cast<const T*>(p.q) + base + (long long)len * p.row_stride;
-  const T* kb = reinterpret_cast<const T*>(p.k) + base;
-  const T* vb = reinterpret_cast<const T*>(p.v) + base;
+  const T *qb, *kb, *vb;
+  const int* pages = nullptr;
+  if constexpr (PAGED) {
+    const long long hoff = (long long)h * D + lane * EPL;
+    qb = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_rs + hoff;
+    kb = reinterpret_cast<const T*>(p.k) + hoff;
+    vb = reinterpret_cast<const T*>(p.v) + hoff;
+    pages = p.page_table + (long long)p.slot[b] * p.pt_ld;
+  } else {
+    const long long base = (long long)p.slot[b] * p.slot_stride + (long long)h * D + lane * EPL;
+    qb = reinterpret_cast<const T*>(p.q) + base + (long long)len * p.row_stride;
+    kb = reinterpret_cast<const T*>(p.k) + base;
+    vb = reinterpret_cast<const T*>(p.v) + base;
+  }
+  // element offset of key / value row j from kb / vb
+  auto row_off = [&](int j) -> long long {
+    if constexpr (PAGED)
+      return (long long)__ldg(pages + (j >> p.page_shift)) * p.page_stride + (long long)(j & ((1 << p.page_shift) - 1)) * p.row_stride;
+    else
+      return (long long)j * p.row_stride;
+  };
 
   float q[EPL], acc[EPL], m = -INFINITY, l = 0.f;
 #pragma unroll
@@ -563,14 +597,15 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_slots_kernel(co
     for (int u = 0; u < DEC_U; ++u) {
       const int j = j0 + u * DEC_WARPS;
       if (j < k_end) {
+        const long long ro = row_off(j);
         if (EPL == 4) {
-          const uint2 k2 = *reinterpret_cast<const uint2*>(kb + (long long)j * p.row_stride);
-          const uint2 v2 = *reinterpret_cast<const uint2*>(vb + (long long)j * p.row_stride);
+          const uint2 k2 = *reinterpret_cast<const uint2*>(kb + ro);
+          const uint2 v2 = *reinterpret_cast<const uint2*>(vb + ro);
           kr[u][0] = k2.x; kr[u][(EPL / 2) - 1] = k2.y;
           vr[u][0] = v2.x; vr[u][(EPL / 2) - 1] = v2.y;
         } else {
-          kr[u][0] = *reinterpret_cast<const uint32_t*>(kb + (long long)j * p.row_stride);
-          vr[u][0] = *reinterpret_cast<const uint32_t*>(vb + (long long)j * p.row_stride);
+          kr[u][0] = *reinterpret_cast<const uint32_t*>(kb + ro);
+          vr[u][0] = *reinterpret_cast<const uint32_t*>(vb + ro);
         }
       } else {
 #pragma unroll
@@ -649,6 +684,28 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_slots_kernel(co
   cluster.sync();
 }
 
+template <int D, typename T>
+__global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_slots_kernel(const SlotAttnParams p) {
+  attn_decode_slots_body<D, T>(p);
+}
+
+template <int D, typename T>
+__global__ void __launch_bounds__(DEC_WARPS * 32, 2) attn_decode_paged_kernel(const PagedSlotAttnParams p) {
+  attn_decode_slots_body<D, T>(p);
+}
+
+// launch_decode's rule, split into its batch-size term (the returned cap) and its key-count term (per row in the kernel; here
+// for the longest row, which sizes the cluster: *splits)
+static int slot_split_cap(int B, int H, int max_len, int* splits) {
+  int cap = DEC_SPLITS;
+  if (!vsb_batch_invariant())
+    while (cap > 1 && (long long)cap * H * B > 2LL * vsb_num_sms() + H) cap >>= 1;
+  int s = cap;
+  while (s > 1 && (max_len + 1) / s < 64) s >>= 1;
+  *splits = s;
+  return cap;
+}
+
 template <typename T>
 static int attn_decode_slots(const void* q, const void* k, const void* v, void* o, long long slot_stride, long long row_stride, long long o_rs,
                              int B, int H, int D, float scale, const void* slot, const void* len, int max_len, void* stream) {
@@ -662,18 +719,46 @@ static int attn_decode_slots(const void* q, const void* k, const void* v, void* 
   p.slot_stride = slot_stride; p.row_stride = row_stride; p.o_rs = o_rs;
   p.slot = reinterpret_cast<const int*>(slot); p.len = reinterpret_cast<const int*>(len);
   p.scale_log2 = scale * 1.4426950408889634f;
-  // launch_decode's rule, split into its batch-size term (cap) and its key-count term (per row in the kernel; here for the
-  // longest row, which sizes the cluster)
-  p.cap = DEC_SPLITS;
-  if (!vsb_batch_invariant())
-    while (p.cap > 1 && (long long)p.cap * H * B > 2LL * vsb_num_sms() + H) p.cap >>= 1;
-  int splits = p.cap;
-  while (splits > 1 && (max_len + 1) / splits < 64) splits >>= 1;
+  int splits;
+  p.cap = slot_split_cap(B, H, max_len, &splits);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (D == 64)
     VSB_CUDA(vsb_launch_pdl(attn_decode_slots_kernel<64, T>, dim3(splits, H, B), dim3(DEC_WARPS * 32), 0, st, splits, p));
   else
     VSB_CUDA(vsb_launch_pdl(attn_decode_slots_kernel<128, T>, dim3(splits, H, B), dim3(DEC_WARPS * 32), 0, st, splits, p));
+  return VSB_OK;
+}
+
+template <typename T>
+static int attn_decode_paged(const void* q, long long q_rs, const void* k, const void* v, void* o, long long o_rs, long long page_stride,
+                             long long row_stride, int page_rows, const void* page_table, int pt_ld, int B, int H, int D, float scale,
+                             const void* slot, const void* len, int max_len, void* stream) {
+  VSB_CHECK_ARG(q && k && v && o && page_table && slot && len, "vsb_attn_decode_paged: null pointer");
+  VSB_CHECK_ARG(D == 64 || D == 128, "vsb_attn_decode_paged: head_dim %d unsupported (64/128)", D);
+  VSB_CHECK_ARG(B > 0 && H > 0 && max_len >= 0 && pt_ld > 0, "vsb_attn_decode_paged: bad shape (B=%d, H=%d, max_len=%d, pt_ld=%d)", B, H,
+                max_len, pt_ld);
+  VSB_CHECK_ARG(page_rows >= 16 && (page_rows & (page_rows - 1)) == 0, "vsb_attn_decode_paged: page_rows %d is not a power of two >= 16",
+                page_rows);
+  VSB_CHECK_ARG((long long)max_len < (long long)pt_ld * page_rows, "vsb_attn_decode_paged: max_len %d past the %d x %d rows of a page table row",
+                max_len, pt_ld, page_rows);
+  VSB_CHECK_ARG(q_rs % 4 == 0 && page_stride % 4 == 0 && row_stride % 4 == 0 && ((uintptr_t)q & 7) == 0 && ((uintptr_t)k & 7) == 0 &&
+                    ((uintptr_t)v & 7) == 0,
+                "vsb_attn_decode_paged: q/k/v must be 8-byte aligned with strides that are multiples of 4 elements");
+  PagedSlotAttnParams p;
+  p.q = q; p.k = k; p.v = v; p.o = o;
+  p.page_stride = page_stride; p.row_stride = row_stride; p.o_rs = o_rs; p.q_rs = q_rs;
+  p.slot = reinterpret_cast<const int*>(slot); p.len = reinterpret_cast<const int*>(len);
+  p.page_table = reinterpret_cast<const int*>(page_table);
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.pt_ld = pt_ld;
+  p.page_shift = __builtin_ctz((unsigned)page_rows);
+  int splits;
+  p.cap = slot_split_cap(B, H, max_len, &splits);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (D == 64)
+    VSB_CUDA(vsb_launch_pdl(attn_decode_paged_kernel<64, T>, dim3(splits, H, B), dim3(DEC_WARPS * 32), 0, st, splits, p));
+  else
+    VSB_CUDA(vsb_launch_pdl(attn_decode_paged_kernel<128, T>, dim3(splits, H, B), dim3(DEC_WARPS * 32), 0, st, splits, p));
   return VSB_OK;
 }
 
@@ -821,6 +906,16 @@ extern "C" int vsb_attn_decode_slots(const void* q, const void* k, const void* v
   VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_attn_decode_slots: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)", dtype);
   return dtype == VSB_DTYPE_F16 ? attn_decode_slots<half>(q, k, v, o, slot_stride, row_stride, o_rs, B, H, D, scale, slot_i32, len_i32, max_len, stream)
                                 : attn_decode_slots<bf16>(q, k, v, o, slot_stride, row_stride, o_rs, B, H, D, scale, slot_i32, len_i32, max_len, stream);
+}
+
+extern "C" int vsb_attn_decode_paged(const void* q, long long q_rs, const void* k, const void* v, void* o, long long o_rs, long long page_stride,
+                                     long long row_stride, int page_rows, const void* page_table_i32, int pt_ld, int B, int H, int D, float scale,
+                                     const void* slot_i32, const void* len_i32, int max_len, int dtype, void* stream) {
+  VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_attn_decode_paged: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)", dtype);
+  return dtype == VSB_DTYPE_F16 ? attn_decode_paged<half>(q, q_rs, k, v, o, o_rs, page_stride, row_stride, page_rows, page_table_i32, pt_ld, B, H, D,
+                                                          scale, slot_i32, len_i32, max_len, stream)
+                                : attn_decode_paged<bf16>(q, q_rs, k, v, o, o_rs, page_stride, row_stride, page_rows, page_table_i32, pt_ld, B, H, D,
+                                                          scale, slot_i32, len_i32, max_len, stream);
 }
 
 #define VSB_ATTN_SEG_ENTRY(NAME, T)                                                                                                \

@@ -13,6 +13,9 @@
 // every layer and every pair, in one launch; one row range [lo, hi) for all pairs, or each pair's own (a decode stream, where
 // every beam request forks at its own length).  Pairs travel in the kernel's parameters; a slot that is both a source and a
 // destination (or two pairs with one destination) is refused, so no CTA reads a row another CTA writes.
+//
+// vsb_copy_page_rows_b16: the same ranged copy into a paged KV pool, each row's page found through the page table; the source is
+// the pool itself (a beam fork) or a contiguous cache (a prefilled prompt's k|v rows written into its pages at admission).
 #include <algorithm>
 
 #include "common.cuh"
@@ -273,6 +276,53 @@ void launch_copy_rows(void* cache, int layers, long long layer_stride, long long
                                                                                    row_stride, row_elems, pp);
 }
 
+// where the paged copy finds rows: the destination always in the pool through the page table, the source there too (FROM_POOL) or
+// in a contiguous cache [layers][slots][rows][...]
+struct PageRows {
+  unsigned short* pool;
+  long long layer_stride, page_stride, row_stride;
+  const int* page_table;
+  int pt_ld, page_shift;
+  const unsigned short* src;
+  long long src_layer_stride, src_slot_stride, src_row_stride;
+  __device__ __forceinline__ long long pool_row(int slot, long long row) const {
+    return (long long)__ldg(page_table + (long long)slot * pt_ld + (row >> page_shift)) * page_stride +
+           (row & ((1 << page_shift) - 1)) * row_stride;
+  }
+};
+
+// grid (chunks, layers, pairs): rows [lo, hi) of one page-table row of one layer, as VEC-element vectors
+template <typename VEC, bool FROM_POOL>
+__global__ void __launch_bounds__(256) copy_page_rows_kernel(const PageRows g, int row_elems, const RangedPairs pairs) {
+  constexpr int kVec = sizeof(VEC) / 2;
+  const int p = blockIdx.z;
+  const int lo = pairs.lo[p], hi = pairs.hi[p];
+  const int per_row = row_elems / kVec;
+  const long long total = (long long)(hi - lo) * per_row;
+  unsigned short* dbase = g.pool + (long long)blockIdx.y * g.layer_stride;
+  const unsigned short* sbase = FROM_POOL ? dbase : g.src + (long long)blockIdx.y * g.src_layer_stride + (long long)pairs.src[p] * g.src_slot_stride;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const long long row = lo + e / per_row, c = e % per_row;
+    const long long so = FROM_POOL ? g.pool_row(pairs.src[p], row) : row * g.src_row_stride;
+    reinterpret_cast<VEC*>(dbase + g.pool_row(pairs.dst[p], row))[c] = reinterpret_cast<const VEC*>(sbase + so)[c];
+  }
+}
+
+template <bool FROM_POOL>
+void launch_copy_page_rows(const PageRows& g, int row_elems, const RangedPairs& pp, int layers, int npairs, int rows, void* stream) {
+  const bool vec = ((reinterpret_cast<uintptr_t>(g.pool) | (uintptr_t)g.layer_stride * 2 | (uintptr_t)g.page_stride * 2 |
+                     (uintptr_t)g.row_stride * 2 | (uintptr_t)row_elems * 2 |
+                     (FROM_POOL ? 0 : (reinterpret_cast<uintptr_t>(g.src) | (uintptr_t)g.src_layer_stride * 2 | (uintptr_t)g.src_slot_stride * 2 |
+                                       (uintptr_t)g.src_row_stride * 2))) & 15) == 0;
+  const long long elems = (long long)rows * row_elems / (vec ? 8 : 1);
+  const int chunks = (int)std::min<long long>((elems + 255) / 256, 64);
+  dim3 grid(chunks, layers, npairs);
+  if (vec)
+    copy_page_rows_kernel<uint4, FROM_POOL><<<grid, 256, 0, STREAM(stream)>>>(g, row_elems, pp);
+  else
+    copy_page_rows_kernel<unsigned short, FROM_POOL><<<grid, 256, 0, STREAM(stream)>>>(g, row_elems, pp);
+}
+
 }  // namespace
 
 extern "C" int vsb_beam_candidates_f32(const void* logits, long long ld, int V, int requests, int k_in, int k, const void* rows_i32,
@@ -349,6 +399,56 @@ extern "C" int vsb_copy_slot_rows_b16(void* cache, int layers, long long layer_s
   }
   if (npairs == 0 || rows == 0) return VSB_OK;
   launch_copy_rows(cache, layers, layer_stride, slot_stride, row_stride, row_elems, pp, npairs, rows, stream);
+  VSB_LAUNCH_CHECK();
+  return VSB_OK;
+}
+
+extern "C" int vsb_copy_page_rows_b16(void* pool, int layers, long long layer_stride, long long page_stride, int page_rows, long long row_stride,
+                                      int row_elems, const void* page_table_i32, int pt_ld, int slots, const void* src, long long src_layer_stride,
+                                      long long src_slot_stride, long long src_row_stride, int src_slots, const int* quads_i32, int npairs,
+                                      void* stream) {
+  VSB_CHECK_ARG(pool && page_table_i32 && layers > 0 && slots > 0 && slots <= 65536 && pt_ld > 0 && row_elems > 0 && row_stride >= row_elems &&
+                    page_stride >= (long long)page_rows * row_stride,
+                "vsb_copy_page_rows_b16: bad args");
+  VSB_CHECK_ARG(page_rows >= 16 && (page_rows & (page_rows - 1)) == 0, "vsb_copy_page_rows_b16: page_rows %d is not a power of two >= 16",
+                page_rows);
+  VSB_CHECK_ARG(src == nullptr || (src_slots > 0 && src_slots <= 65536 && src_row_stride >= row_elems),
+                "vsb_copy_page_rows_b16: bad contiguous source");
+  VSB_CHECK_ARG(npairs >= 0 && npairs <= VSB_COPY_ROWS_MAX_PAIRS, "vsb_copy_page_rows_b16: npairs must be in [0, %d], got %d",
+                VSB_COPY_ROWS_MAX_PAIRS, npairs);
+  VSB_CHECK_ARG(npairs == 0 || quads_i32, "vsb_copy_page_rows_b16: null pair list");
+  const long long row_cap = (long long)pt_ld * page_rows;
+  RangedPairs pp;
+  int rows = 0;
+  for (int p = 0; p < npairs; ++p) {
+    const int s = quads_i32[4 * p], d = quads_i32[4 * p + 1], lo = quads_i32[4 * p + 2], hi = quads_i32[4 * p + 3];
+    VSB_CHECK_ARG(s >= 0 && s < (src ? src_slots : slots) && d >= 0 && d < slots, "vsb_copy_page_rows_b16: pair %d (%d -> %d) outside the tables",
+                  p, s, d);
+    VSB_CHECK_ARG(0 <= lo && lo <= hi && hi <= row_cap && (src == nullptr || (long long)hi * src_row_stride <= src_slot_stride),
+                  "vsb_copy_page_rows_b16: pair %d: bad row range [%d, %d)", p, lo, hi);
+    for (int q = 0; q < npairs; ++q) {
+      VSB_CHECK_ARG(src || quads_i32[4 * q + 1] != s, "vsb_copy_page_rows_b16: row %d is both a source and a destination", s);
+      VSB_CHECK_ARG(q == p || quads_i32[4 * q + 1] != d, "vsb_copy_page_rows_b16: row %d is the destination of two pairs", d);
+    }
+    pp.src[p] = (unsigned short)s;
+    pp.dst[p] = (unsigned short)d;
+    pp.lo[p] = lo;
+    pp.hi[p] = hi;
+    rows = std::max(rows, hi - lo);
+  }
+  if (npairs == 0 || rows == 0) return VSB_OK;
+  PageRows g;
+  g.pool = (unsigned short*)pool;
+  g.layer_stride = layer_stride; g.page_stride = page_stride; g.row_stride = row_stride;
+  g.page_table = (const int*)page_table_i32;
+  g.pt_ld = pt_ld;
+  g.page_shift = __builtin_ctz((unsigned)page_rows);
+  g.src = (const unsigned short*)src;
+  g.src_layer_stride = src_layer_stride; g.src_slot_stride = src_slot_stride; g.src_row_stride = src_row_stride;
+  if (src)
+    launch_copy_page_rows<false>(g, row_elems, pp, layers, npairs, rows, stream);
+  else
+    launch_copy_page_rows<true>(g, row_elems, pp, layers, npairs, rows, stream);
   VSB_LAUNCH_CHECK();
   return VSB_OK;
 }

@@ -249,6 +249,50 @@ __global__ void rope_scatter_kernel(const E_T* __restrict__ qkv, long long ldq, 
     *reinterpret_cast<uint4*>(dst + 2 * d + i) = *reinterpret_cast<const uint4*>(src + 2 * d + i);
 }
 
+// Paged form of rope_scatter_kernel: q is rotated in place in qkv (attention reads it there), k rotated and v copied to row
+// len[b] of row b's pages (k|v rows of 2d): page page_table[slot[b]*pt_ld + (len >> page_shift)], row len & (page rows - 1).
+template <typename E_T>
+__global__ void rope_scatter_paged_kernel(E_T* __restrict__ qkv, long long ldq, int H, int D, E_T* __restrict__ pool, long long page_stride,
+                                          long long ldc, int page_shift, const int* __restrict__ page_table, int pt_ld,
+                                          const int* __restrict__ slot, const int* __restrict__ len, const int* __restrict__ positions,
+                                          const E_T* __restrict__ cos_t, const E_T* __restrict__ sin_t) {
+  using E = ElemT<E_T>;
+  pdl_prologue();
+  const int row = blockIdx.x;
+  const int pos = positions[row];
+  const int n = len[row];
+  const int half = D >> 1;
+  const int hv = half >> 3;
+  const int d = H * D;
+  E_T* src = qkv + (long long)row * ldq;
+  E_T* dst = pool + (long long)page_table[(long long)slot[row] * pt_ld + (n >> page_shift)] * page_stride +
+             (long long)(n & ((1 << page_shift) - 1)) * ldc;
+  const E_T* cr = cos_t + (long long)pos * half;
+  const E_T* sr = sin_t + (long long)pos * half;
+  for (int idx = threadIdx.x; idx < 2 * H * hv; idx += blockDim.x) {
+    const int hh = idx / hv;
+    const int v = idx - hh * hv;
+    const long long o = (long long)hh * D + v * 8;
+    const uint4 a = *reinterpret_cast<const uint4*>(src + o);
+    const uint4 b = *reinterpret_cast<const uint4*>(src + o + half);
+    const uint4 c = __ldg(reinterpret_cast<const uint4*>(cr + v * 8));
+    const uint4 s = __ldg(reinterpret_cast<const uint4*>(sr + v * 8));
+    const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w}, cw[4] = {c.x, c.y, c.z, c.w}, sw[4] = {s.x, s.y, s.z, s.w};
+    uint32_t oa[4], ob[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 x1 = E::unpack2(aw[j]), x2 = E::unpack2(bw[j]), cs = E::unpack2(cw[j]), sn = E::unpack2(sw[j]);
+      oa[j] = E::pack2(E::round(x1.x * cs.x) + E::round(-x2.x * sn.x), E::round(x1.y * cs.y) + E::round(-x2.y * sn.y));
+      ob[j] = E::pack2(E::round(x2.x * cs.x) + E::round(x1.x * sn.x), E::round(x2.y * cs.y) + E::round(x1.y * sn.y));
+    }
+    E_T* out = hh < H ? src + o : dst + (o - d);                 // q heads in place, k heads to the page row
+    *reinterpret_cast<uint4*>(out) = make_uint4(oa[0], oa[1], oa[2], oa[3]);
+    *reinterpret_cast<uint4*>(out + half) = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+  }
+  for (int i = threadIdx.x * 8; i < d; i += blockDim.x * 8)
+    *reinterpret_cast<uint4*>(dst + d + i) = *reinterpret_cast<const uint4*>(src + 2 * d + i);
+}
+
 // ------------------------------------------------------------------ embedding splice
 // out[b, t, :] = table[ids[b, t']] for text positions; image rows are left untouched (the
 // mm_projector GEMM writes them directly through its row remap).  ids layout [B, L] with
@@ -543,6 +587,34 @@ extern "C" int vsb_rope_scatter(const void* qkv, long long ldq, int B, int H, in
   VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_rope_scatter: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)", dtype);
   return dtype == VSB_DTYPE_F16 ? rope_scatter<half>(qkv, ldq, B, H, D, cache, ldc, Tmax, slot_i32, len_i32, pos_i32, cos_table, sin_table, stream)
                                 : rope_scatter<bf16>(qkv, ldq, B, H, D, cache, ldc, Tmax, slot_i32, len_i32, pos_i32, cos_table, sin_table, stream);
+}
+
+template <typename E_T>
+static int rope_scatter_paged(void* qkv, long long ldq, int B, int H, int D, void* pool, long long page_stride, long long ldc, int page_rows,
+                              const void* page_table, int pt_ld, const void* slot, const void* len, const void* positions,
+                              const void* cos_table, const void* sin_table, void* stream) {
+  VSB_CHECK_ARG(qkv && pool && page_table && slot && len && positions && cos_table && sin_table, "vsb_rope_scatter_paged: null pointer");
+  VSB_CHECK_ARG(B >= 0 && H > 0 && pt_ld > 0 && D % 16 == 0 && ldq % 8 == 0 && ldc % 8 == 0 && page_stride % 8 == 0 && ldq >= 3LL * H * D &&
+                    ldc >= 2LL * H * D && page_stride >= (long long)page_rows * ldc,
+                "vsb_rope_scatter_paged: bad args (D %% 16, ld %% 8, ldq >= 3*H*D, ldc >= 2*H*D, page_stride >= page_rows*ldc)");
+  VSB_CHECK_ARG(page_rows >= 16 && (page_rows & (page_rows - 1)) == 0, "vsb_rope_scatter_paged: page_rows %d is not a power of two >= 16",
+                page_rows);
+  if (B == 0) return VSB_OK;
+  VSB_CUDA(vsb_launch_pdl(rope_scatter_paged_kernel<E_T>, dim3(B), dim3(256), 0, STREAM(stream), 1, (E_T*)qkv, ldq, H, D, (E_T*)pool, page_stride,
+                          ldc, __builtin_ctz((unsigned)page_rows), (const int*)page_table, pt_ld, (const int*)slot, (const int*)len,
+                          (const int*)positions, (const E_T*)cos_table, (const E_T*)sin_table));
+  return VSB_OK;
+}
+
+extern "C" int vsb_rope_scatter_paged(void* qkv, long long ldq, int B, int H, int D, void* pool, long long page_stride, long long ldc,
+                                      int page_rows, const void* page_table_i32, int pt_ld, const void* slot_i32, const void* len_i32,
+                                      const void* pos_i32, const void* cos_table, const void* sin_table, int dtype, void* stream) {
+  VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_rope_scatter_paged: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)", dtype);
+  return dtype == VSB_DTYPE_F16
+             ? rope_scatter_paged<half>(qkv, ldq, B, H, D, pool, page_stride, ldc, page_rows, page_table_i32, pt_ld, slot_i32, len_i32, pos_i32,
+                                        cos_table, sin_table, stream)
+             : rope_scatter_paged<bf16>(qkv, ldq, B, H, D, pool, page_stride, ldc, page_rows, page_table_i32, pt_ld, slot_i32, len_i32, pos_i32,
+                                        cos_table, sin_table, stream);
 }
 
 extern "C" int vsb_embed_splice_bf16(const void* ids, const void* table, void* out, int B, int L, int img_pos, int n_img, int d,

@@ -67,6 +67,10 @@ struct SlotRows {
   const void* slot;   // int32 [B] cache slot of row b
   const void* len;    // int32 [B] rows already cached in that slot: the new row is written at slot*Tmax + len
   int max_len;        // >= every len[b]
+  // paged cache (vsb_llama_layers_slots_paged), page_table NULL otherwise: `cache` is the pool [n_layers][n_pages][page_rows][2d]
+  // of k|v rows, `slot` indexes the rows of page_table [*, pt_ld]
+  const void* page_table = nullptr;
+  int pt_ld = 0, page_rows = 0, n_pages = 0;
 };
 
 template <typename T>
@@ -165,9 +169,19 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
       T* qkv = gu + rows * inter;                                                      // [B, 3d]
       VSB_TRY(proj(qkv_in, L.wqkv, L.wqkv_scales, qkv, ld, rows, 3 * d, d, false, VSB_EPI_NONE, 0, 0, 0, sq_in, sq_in_chunks, nullptr));
       const int dt = ElemT<T>::is_f16 ? VSB_DTYPE_F16 : VSB_DTYPE_BF16;
-      VSB_TRY(vsb_rope_scatter(qkv, ld, B, H, hd, cl, ld, Tmax, slots->slot, slots->len, positions, rope_cos, rope_sin, dt, stream));
-      VSB_TRY(vsb_attn_decode_slots(cl, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, d, B, H, hd, scale, slots->slot, slots->len,
-                                    slots->max_len, dt, stream));
+      if (slots->page_table) {
+        // q rotated in place in scratch, k|v to the row's page; attention reads q there and k|v through the page table
+        const long long kv = 2LL * d, page = (long long)slots->page_rows * kv;
+        T* pl = reinterpret_cast<T*>(cache) + (long long)li * slots->n_pages * page;  // [n_pages, page_rows, 2d]
+        VSB_TRY(vsb_rope_scatter_paged(qkv, ld, B, H, hd, pl, page, kv, slots->page_rows, slots->page_table, slots->pt_ld, slots->slot, slots->len,
+                                       positions, rope_cos, rope_sin, dt, stream));
+        VSB_TRY(vsb_attn_decode_paged(qkv, ld, pl, pl + d, attn, d, page, kv, slots->page_rows, slots->page_table, slots->pt_ld, B, H, hd, scale,
+                                      slots->slot, slots->len, slots->max_len, dt, stream));
+      } else {
+        VSB_TRY(vsb_rope_scatter(qkv, ld, B, H, hd, cl, ld, Tmax, slots->slot, slots->len, positions, rope_cos, rope_sin, dt, stream));
+        VSB_TRY(vsb_attn_decode_slots(cl, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, d, B, H, hd, scale, slots->slot, slots->len,
+                                      slots->max_len, dt, stream));
+      }
       VSB_TRY(post_attention(L, xb, rows, fused ? sq_a : nullptr));
       continue;
     }
@@ -239,5 +253,31 @@ extern "C" int vsb_llama_layers_slots(const vsb_llama_layer_t* layers, int n_lay
     return llama_layers<half>(layers, n_layers, x, B, 1, 0, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr, 0,
                               nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
   return llama_layers<bf16>(layers, n_layers, x, B, 1, 0, cache, Bc, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr, 0,
+                            nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
+}
+
+// Paged slot decode: vsb_llama_layers_slots on a pool of k|v pages instead of one [Tmax, 3d] slot per sequence.  Row b's new q is
+// rotated in place in scratch, its k|v go to row len[b] of the pages page_table[slot[b]] lists (vsb_rope_scatter_paged), and
+// vsb_attn_decode_paged reads its keys through the same table.  Every other kernel of the layer is the slot runner's.
+extern "C" int vsb_llama_layers_slots_paged(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, void* pool, int n_pages, int page_rows,
+                                            const void* page_table_i32, int pt_ld, int d, int H, int inter, float rms_eps, const void* rope_cos,
+                                            const void* rope_sin, const void* slot_i32, const void* len_i32, const void* pos_i32, int max_len,
+                                            int norm_folded, void* scratch, void* deq_scratch, int dtype, void* stream) {
+  VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_llama_layers_slots_paged: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)",
+                dtype);
+  VSB_CHECK_ARG(page_table_i32 && n_pages > 0 && pt_ld > 0, "vsb_llama_layers_slots_paged: null page table or empty pool");
+  VSB_CHECK_ARG(page_rows >= 16 && (page_rows & (page_rows - 1)) == 0 && (long long)pt_ld * page_rows < (1LL << 30),
+                "vsb_llama_layers_slots_paged: page_rows %d is not a power of two >= 16", page_rows);
+  SlotRows s{slot_i32, len_i32, max_len};
+  s.page_table = page_table_i32;
+  s.pt_ld = pt_ld;
+  s.page_rows = page_rows;
+  s.n_pages = n_pages;
+  // the cache-shape checks of the runner see B sequences of pt_ld * page_rows rows
+  const int Tmax = pt_ld * page_rows;
+  if (dtype == VSB_DTYPE_F16)
+    return llama_layers<half>(layers, n_layers, x, B, 1, 0, pool, B, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr, 0,
+                              nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
+  return llama_layers<bf16>(layers, n_layers, x, B, 1, 0, pool, B, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr, 0,
                             nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
 }

@@ -277,6 +277,95 @@ def llama_layers_slots(table, n_layers, x, cache, eps, rope_cos, rope_sin, scrat
     return x
 
 
+def _pool_shape(pool, page_table):
+    """pool [n_layers, n_pages, P, 2d] or one layer's [n_pages, P, 2d], page_table int32 [rows, pages_per_row] -> (P, pages_per_row)"""
+    assert pool.is_contiguous() and pool.dim() in (3, 4)
+    P = pool.shape[-2]
+    if P < 16 or P & (P - 1):
+        raise _lib.VsbError(f"page rows {P} is not a power of two >= 16")
+    _chk(page_table, torch.int32)
+    assert page_table.dim() == 2 and page_table.is_contiguous()
+    return P, page_table.shape[1]
+
+
+def llama_layers_slots_paged(table, n_layers, x, pool, page_table, eps, rope_cos, rope_sin, scratch, slot, length, pos, max_len, H, inter,
+                             norm_folded=False, deq_scratch=None):
+    """llama_layers_slots on a paged KV pool [n_layers, n_pages, P, 2d] of k|v rows (vsb_llama_layers_slots_paged): row b's
+    keys are rows [0, length[b]] of the pages page_table[slot[b]] lists (page_table int32 [rows, pages_per_row] on the device),
+    its new k|v go to row length[b]; max_len >= max(length) and < pages_per_row * P.  scratch, NF4 tables as llama_layers_slots."""
+    sfx = _sfx(x, pool, scratch, rope_cos, rope_sin)
+    B, d = x.shape
+    L, n_pages, P, W = pool.shape
+    P, ppr = _pool_shape(pool, page_table)
+    assert x.is_contiguous() and W == 2 * d and L >= n_layers
+    assert scratch.numel() >= B * (5 * d + inter)
+    _i32_rows(slot, length, pos, n=B)
+    if table[0].wqkv_scales:
+        if sfx != "f16" or norm_folded:
+            raise _lib.VsbError("NF4 layers run in fp16 with unfolded norms")
+        _chk(deq_scratch, F16)
+        assert deq_scratch.is_contiguous() and deq_scratch.numel() >= 2 * inter * d
+    _lib.launches += 8 * n_layers
+    call("vsb_llama_layers_slots_paged", table, n_layers, x.data_ptr(), B, pool.data_ptr(), n_pages, P, page_table.data_ptr(), ppr, d, H, inter,
+         float(eps), rope_cos.data_ptr(), rope_sin.data_ptr(), slot.data_ptr(), length.data_ptr(), pos.data_ptr(), int(max_len),
+         1 if norm_folded else 0, scratch.data_ptr(), _p(deq_scratch), _DTYPE[sfx], _stream())
+    return x
+
+
+def rope_scatter_paged(qkv, pool, page_table, H, D, cos_t, sin_t, slot, length, pos):
+    """rope_scatter into one layer's pages [n_pages, P, 2*H*D] (vsb_rope_scatter_paged): row b of qkv [B, 3*H*D] has q rotated in
+    place, its rotated k and its v go to row length[b] of the pages page_table[slot[b]] lists"""
+    sfx = _sfx(qkv, pool, cos_t, sin_t)
+    p, B, cols, ld = _rows2d(qkv)
+    P, ppr = _pool_shape(pool, page_table)
+    assert cols == 3 * H * D and pool.dim() == 3 and pool.shape[2] == 2 * H * D
+    _i32_rows(slot, length, pos, n=B)
+    _lib.launches += 1
+    call("vsb_rope_scatter_paged", p, ld, B, H, D, pool.data_ptr(), pool.stride(0), pool.stride(1), P, page_table.data_ptr(), ppr,
+         slot.data_ptr(), length.data_ptr(), pos.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), _DTYPE[sfx], _stream())
+    return pool
+
+
+def attn_decode_paged(q, pool, page_table, out, H, D, scale, slot, length, max_len=None):
+    """attn_decode_slots over one layer's pages [n_pages, P, 2*H*D] (vsb_attn_decode_paged): row b's query is q[b, :H*D] and it
+    attends rows [0, length[b]] of the pages page_table[slot[b]] lists -> out [B, H*D]"""
+    sfx = _sfx(q, pool, out)
+    pq, B, _, ldq = _rows2d(q)
+    P, ppr = _pool_shape(pool, page_table)
+    assert pool.dim() == 3 and pool.shape[2] == 2 * H * D and out.stride(1) == 1 and out.shape[0] == B
+    _i32_rows(slot, length, n=B)
+    if max_len is None:
+        max_len = int(length.max())
+    base = pool.data_ptr()
+    _lib.launches += 1
+    call("vsb_attn_decode_paged", pq, ldq, base, base + 2 * H * D, out.data_ptr(), out.stride(0), pool.stride(0), pool.stride(1), P,
+         page_table.data_ptr(), ppr, B, H, D, float(scale), slot.data_ptr(), length.data_ptr(), int(max_len), _DTYPE[sfx], _stream())
+    return out
+
+
+def copy_page_rows(pool, page_table, quads, src=None):
+    """rows [lo, hi) of every layer into page-table row d's pages of pool [L, n_pages, P, W] for every (s, d, lo, hi) in the host
+    list `quads`, in one vsb_copy_page_rows_b16 launch (at most COPY_ROWS_MAX_PAIRS pairs).  src None: from page-table row s of
+    the pool (the rules of copy_slot_rows); src a [L, S, T, >= W] view with unit inner stride (e.g. the k|v columns of a fused
+    q|k|v cache): from its slot s."""
+    import ctypes
+    _chk(pool)
+    assert pool.dim() == 4 and pool.element_size() == 2
+    P, ppr = _pool_shape(pool, page_table)
+    L, _, _, W = pool.shape
+    if src is None:
+        sp, sls, sss, srs, ns = None, 0, 0, 0, 0
+    else:
+        _chk(src, pool.dtype)
+        assert src.dim() == 4 and src.shape[0] == L and src.shape[3] == W and src.stride(3) == 1
+        sp, sls, sss, srs, ns = src.data_ptr(), src.stride(0), src.stride(1), src.stride(2), src.shape[1]
+    arr = (ctypes.c_int * (4 * max(1, len(quads))))(*[int(v) for q in quads for v in q])
+    _lib.launches += 1
+    call("vsb_copy_page_rows_b16", pool.data_ptr(), L, pool.stride(0), pool.stride(1), P, pool.stride(2), W, page_table.data_ptr(), ppr,
+         page_table.shape[0], sp, sls, sss, srs, ns, arr, len(quads), _stream())
+    return pool
+
+
 def rope_scatter(qkv, cache, H, D, cos_t, sin_t, slot, length, pos):
     """row b of qkv [B, 3*H*D] -> cache row slot[b]*Tmax + length[b] of cache [Bc, Tmax, 3*H*D] (one layer), q and k rotated at
     position pos[b] like rope_, v copied (vsb_rope_scatter)"""

@@ -186,17 +186,19 @@ def open_final_request(vqa_llm, image, question, missing, results):
 
 
 def answer_open_many(vqa_llm, vsm, items, slots=16, searches_in_flight=8, minimum_size_scale=4.0, minimum_size=224, search_batch=16,
-                     search_kwargs=None, temperature=0, top_p=None, num_beams=1):
+                     search_kwargs=None, temperature=0, top_p=None, num_beams=1, kv_pages=None):
     """app.py's inference() for many (image, question) pairs (PIL images), in three phases:
       A. every direct answer on one decode stream (vqa_llm.free_form_inference_stream, `slots` answers decoding at a time);
       B. every missing object's search on one SearchController.stream, `searches_in_flight` searches at a time;
       C. every final answer on one decode stream.
     temperature / top_p (sampling) and num_beams (beam search, num_beams slots per answer) apply to both decode phases, as
-    free_form_inference takes them; the defaults decode greedily, as app.py does.
+    free_form_inference takes them; the defaults decode greedily, as app.py does.  kv_pages = N runs both decode phases on a
+    paged stream whose KV pool holds N pages (VQAEngine.decode_stream), so more answers fit in the same memory.
     -> per item, in input order, app.py's four outputs: (direct answer, None, None, None) when nothing is missing, else
     ("Need to conduct visual search to search for: ...", search-summary string, annotated np.ndarray image, final answer)."""
     # only settings that differ from greedy are passed on, so a VQA LLM with the greedy-only signature still serves the default
-    gen = {k: v for k, v, d in (("temperature", temperature, 0), ("top_p", top_p, None), ("num_beams", num_beams, 1)) if v != d}
+    gen = {k: v for k, v, d in (("temperature", temperature, 0), ("top_p", top_p, None), ("num_beams", num_beams, 1), ("kv_pages", kv_pages, None))
+           if v != d}
     items = [(image.convert("RGB"), question) for image, question in items]
     bg = tuple(int(x * 255) for x in vqa_llm.image_processor.image_mean)
     first = [(expand2square_center(image, bg)[0], q, None, None, None) for image, q in items]
@@ -264,6 +266,9 @@ def build_parser():
     p.add_argument("--temperature", default=0, type=float, help="> 0: sample the answers (app.py's default 0 decodes greedily)")
     p.add_argument("--top_p", default=None, type=float, help="nucleus filter of sampled answers")
     p.add_argument("--num_beams", default=1, type=int, help="> 1: beam-search the answers (num_beams slots per answer)")
+    p.add_argument("--kv-pages", default=None, type=int,
+                   help="hold the answers' KV cache in a pool of this many 64-row pages, each answer reserving only the rows it needs "
+                        "(default: one full-length cache slot per answer)")
     return p
 
 
@@ -317,7 +322,7 @@ def main(argv=None, vqa_llm=None, vsm=None):
     items = [(Image.open(p).convert("RGB"), q) for p, q in questions]
     answers = answer_open_many(vqa_llm, vsm, items, slots=args.slots, searches_in_flight=args.searches_in_flight,
                                minimum_size_scale=args.minimum_size_scale, minimum_size=args.minimum_size, search_batch=args.search_batch,
-                               temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams)
+                               temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams, kv_pages=args.kv_pages)
     return write_answers(args.output_path, questions, answers, args.save_images)
 
 

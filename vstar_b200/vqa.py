@@ -30,6 +30,7 @@ from . import ops
 from .beam import DEFAULT_EARLY_STOPPING, DEFAULT_LENGTH_PENALTY, BeamRequest, check_beams, fork_slots
 from .config import VSMConfig
 from .engine import CoreWeights, LlamaClipCore
+from .kv_pages import PAGE_ROWS, PagePool, pages_for
 from .vsm import CLIP_MEAN, SyntheticTokenizer, _normalize_into
 
 BF = torch.bfloat16
@@ -361,9 +362,11 @@ class VQAEngine(LlamaClipCore):
             res[i] = outs[k]
         return res
 
-    def decode_stream(self, max_slots, max_positions=None, eos_token_id=2, temperature=0, num_beams=1):
+    def decode_stream(self, max_slots, max_positions=None, eos_token_id=2, temperature=0, num_beams=1, kv_pages=None):
         """Decode batch that admits a request whenever a slot is free (DecodeStream).  max_positions: cache rows per slot
-        (default self.max_tokens); a request's prompt plus its max_new_tokens must fit in them.  Generation settings belong to
+        (default self.max_tokens); a request's prompt plus its max_new_tokens must fit in them.  kv_pages = N: the KV cache
+        is a pool of N pages of kv_pages.PAGE_ROWS rows and a request reserves only the pages it needs (DecodeStream); None
+        keeps one cache slot of max_positions rows per decode row.  Generation settings belong to
         each request: DecodeStream.admit(..., temperature=, top_k=, top_p=, seed=, num_beams=, ...) samples or beam-searches
         it; the stream-wide temperature > 0 and num_beams > 1 are refused, since every sampled request needs its own seed."""
         if temperature is not None and temperature > 0:
@@ -372,7 +375,7 @@ class VQAEngine(LlamaClipCore):
         if num_beams != 1:
             raise NotImplementedError("decode_stream takes no stream-wide num_beams: beam-search a request with "
                                       "DecodeStream.admit(..., num_beams=, length_penalty=, early_stopping=)")
-        return DecodeStream(self, max_slots, self.max_tokens if max_positions is None else max_positions, eos_token_id)
+        return DecodeStream(self, max_slots, self.max_tokens if max_positions is None else max_positions, eos_token_id, kv_pages=kv_pages)
 
     def spliced_length(self, input_ids, n_crops=0, images_long=None, objects_long=None):
         """rows the spliced sequence of build_embeds(input_ids, ...) has, computed on the host (the rule of _splice)"""
@@ -604,9 +607,20 @@ class DecodeStream:
     vsb_sample_rows_var_f32 launch for every sampled row, each with its own temperature / top_k / top_p / seed / step) or beam
     search (num_beams = k: the request holds k slots; one vsb_beam_candidates_f32 launch per distinct k, and the forked beams'
     generated rows move by one vsb_copy_slot_rows_b16 launch).  Rows are ordered greedy, sampled, beam, each kind in slot
-    order, so a greedy-only stream issues the launches it always did."""
+    order, so a greedy-only stream issues the launches it always did.
 
-    def __init__(self, engine, max_slots, max_positions, eos_token_id=2):
+    kv_pages = N (paged mode): the cache is a pool [n_layers, N, PAGE_ROWS, 2d] of k|v pages instead of [max_slots,
+    max_positions] rows per slot.  A slot is then a row of the device page table [max_slots, ceil(max_positions / PAGE_ROWS)]:
+    max_slots bounds the rows decoded per step, max_positions one request, and a request reserves ceil((T + max_new_tokens) /
+    PAGE_ROWS) pages at admission (a beam request shares its full prompt pages among its beams; kv_pages.PagePool).  A request
+    is prefilled into a staging cache of its T rows and its k|v rows are written into its pages by one
+    vsb_copy_page_rows_b16 launch; steps run vsb_llama_layers_slots_paged.  Logits and tokens are bit-identical to the
+    contiguous stream's on the same admission schedule.  The page table is uploaded at admission, the only time it changes
+    where a kernel could read it; a step still makes one device-to-host copy."""
+
+    pages = None                                         # PagePool of a paged stream
+
+    def __init__(self, engine, max_slots, max_positions, eos_token_id=2, kv_pages=None):
         max_slots, max_positions = int(max_slots), int(max_positions)
         if max_slots < 1:
             raise ValueError(f"max_slots must be >= 1, got {max_slots}")
@@ -618,7 +632,12 @@ class DecodeStream:
         if engine._layer_table is None:
             engine._layer_table = ops.llama_layer_table(engine.w.layers)
         dev, dt = engine.dev, engine.dtype
-        self._cache = torch.empty((c.n_layers, max_slots, max_positions, 3 * c.hidden), dtype=dt, device=dev)
+        if kv_pages is None:
+            self._cache = torch.empty((c.n_layers, max_slots, max_positions, 3 * c.hidden), dtype=dt, device=dev)
+        else:
+            self.pages = PagePool(int(kv_pages), max_slots, pages_for(max_positions))
+            self._cache = torch.empty((c.n_layers, self.pages.n_pages, PAGE_ROWS, 2 * c.hidden), dtype=dt, device=dev)
+            self._page_table = torch.zeros(self.pages.table.shape, dtype=torch.int32, device=dev)
         self._scratch = torch.empty((max_slots * (5 * c.hidden + c.intermediate),), dtype=dt, device=dev)
         self._deq = torch.empty((2 * c.intermediate * c.hidden,), dtype=dt, device=dev) if getattr(engine.w, "quant", None) else None
         self._slots = [None] * max_slots                 # slot -> active StreamRequest (a beam request in each of its slots)
@@ -654,6 +673,8 @@ class DecodeStream:
         r.done = True
         for s in r.slots:
             self._slots[s] = None
+        if self.pages is not None:
+            self.pages.release(r.slots)
 
     def _beam_advance(self, r, cand):
         """one beam-search step of request r on its 2k candidates [(score, token, beam)] -> the (src, dst, lo, hi) row copies of
@@ -675,7 +696,7 @@ class DecodeStream:
         num_beams = k > 1 runs beam_search's scorer with length_penalty / early_stopping on k slots (stop_ids at most [eos]),
         its first candidates selected here from the prefill logits.  Raises (before any launch) on settings generate() refuses,
         when fewer than num_beams slots are free, num_beams exceeds max_slots or the prompt plus max_new_tokens exceeds
-        max_positions."""
+        max_positions, and in paged mode when the free pages are fewer than the request reserves (RuntimeError)."""
         self._check_open()
         ids, image, crops, il, ol = request
         max_new_tokens = int(max_new_tokens)
@@ -696,18 +717,23 @@ class DecodeStream:
         if self.free_slots < k:
             raise RuntimeError(f"no free slot: all {self.max_slots} slots of the decode stream are in use" if k == 1 else
                                f"no free slot for {k} beams: {self.free_slots} of the decode stream's {self.max_slots} slots are free")
+        slots = [i for i, r in enumerate(self._slots) if r is None][:k]
+        if self.pages is not None:
+            self.pages.check_reserve(slots, T, max_new_tokens)
         if sample and seed is None:
             seed = draw_seeds(1)[0]
-        slots = [i for i, r in enumerate(self._slots) if r is None][:k]
         slot = slots[0]
         x = e.build_embeds(ids, image, crops, il, ol)
         assert x.shape[0] == T
         c = e.cfg
         scratch = torch.empty((T * (2 * c.hidden + c.intermediate),), dtype=e.dtype, device=e.dev)
-        Bc, Tm = self.max_slots, self.max_positions
-        ops.llama_layers(e._layer_table, len(e.w.layers), x, 1, T, 0, self._cache, Bc, Tm, c.hidden, c.n_heads, c.intermediate,
-                         c.rms_eps, e.w.rope_cos, e.w.rope_sin, scratch, cache_row_offset=slot * Tm,
-                         norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
+        if self.pages is None:
+            Bc, Tm = self.max_slots, self.max_positions
+            ops.llama_layers(e._layer_table, len(e.w.layers), x, 1, T, 0, self._cache, Bc, Tm, c.hidden, c.n_heads, c.intermediate,
+                             c.rms_eps, e.w.rope_cos, e.w.rope_sin, scratch, cache_row_offset=slot * Tm,
+                             norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
+        else:
+            self._admit_paged(x, T, max_new_tokens, slots, scratch)
         _, idx, logits = e._logits_rows(x, torch.tensor([T - 1], dtype=torch.int64, device=e.dev))
         r = StreamRequest(self._next_id, slot, T, max_new_tokens, stop_ids, temperature=float(temperature) if sample else 0,
                           top_k=top_k if sample else 0, top_p=top_p if sample else None, seed=seed if sample else None,
@@ -718,7 +744,8 @@ class DecodeStream:
         for s in slots:
             self._slots[s] = r
         if beam:
-            ops.copy_slot_rows(self._cache, [(slot, s, 0, T) for s in slots[1:]])          # the prompt rows of the other beams
+            if self.pages is None:
+                ops.copy_slot_rows(self._cache, [(slot, s, 0, T) for s in slots[1:]])      # the prompt rows of the other beams
             dev = e.dev
             cand = ops.beam_candidates(logits, torch.zeros((1, 1), dtype=torch.int32, device=dev),
                                        torch.zeros((1, 1), dtype=torch.float32, device=dev), k, e.dtype).cpu()
@@ -733,6 +760,20 @@ class DecodeStream:
             self._release(r)
             self._finished.append(r)
         return r
+
+    def _admit_paged(self, x, T, max_new_tokens, slots, scratch):
+        """prefill x [T, d] into a staging cache of T rows with the contiguous runner, reserve the request's pages and write
+        its k|v rows into them: all T rows into the first beam's pages (the shared full pages among them), rows from the
+        last shared page on into every other beam's private pages"""
+        e, c = self.engine, self.engine.cfg
+        staging = torch.empty((c.n_layers, 1, T, 3 * c.hidden), dtype=e.dtype, device=e.dev)
+        ops.llama_layers(e._layer_table, len(e.w.layers), x, 1, T, 0, staging, 1, T, c.hidden, c.n_heads, c.intermediate, c.rms_eps,
+                         e.w.rope_cos, e.w.rope_sin, scratch, norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
+        shared = self.pages.reserve(slots, T, max_new_tokens)
+        self._page_table.copy_(torch.from_numpy(self.pages.table))
+        lo = shared * PAGE_ROWS
+        ops.copy_page_rows(self._cache, self._page_table, [(0, slots[0], 0, T)] + [(0, s, lo, T) for s in slots[1:]],
+                           src=staging[..., c.hidden:])
 
     def step(self):
         """one decode step of every active request -> [(handle, new token ids)] of the requests that ended in it (and of those
@@ -758,9 +799,14 @@ class DecodeStream:
         meta = torch.tensor([[s for _, s, _, _ in rows], lens, lens], dtype=torch.int32).to(e.dev)
         ids = torch.tensor([t for _, _, _, t in rows], dtype=torch.int64).to(e.dev)
         x = ops.gather_rows(ids, e.w.embed)
-        ops.llama_layers_slots(e._layer_table, len(e.w.layers), x, self._cache, c.rms_eps, e.w.rope_cos, e.w.rope_sin, self._scratch,
-                               meta[0], meta[1], meta[2], max(lens), c.n_heads, c.intermediate,
-                               norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
+        if self.pages is None:
+            ops.llama_layers_slots(e._layer_table, len(e.w.layers), x, self._cache, c.rms_eps, e.w.rope_cos, e.w.rope_sin, self._scratch,
+                                   meta[0], meta[1], meta[2], max(lens), c.n_heads, c.intermediate,
+                                   norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
+        else:
+            ops.llama_layers_slots_paged(e._layer_table, len(e.w.layers), x, self._cache, self._page_table, c.rms_eps, e.w.rope_cos,
+                                         e.w.rope_sin, self._scratch, meta[0], meta[1], meta[2], max(lens), c.n_heads, c.intermediate,
+                                         norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
         hn = ops.rmsnorm(x, e.w.final_norm, c.rms_eps)
         logits = ops.gemm(hn, e.w.lm_head, out_dtype=torch.float32)
         G, S = len(greedy), len(sampled)
@@ -795,7 +841,10 @@ class DecodeStream:
                 else:
                     quads += q
         for i in range(0, len(quads), ops.COPY_ROWS_MAX_PAIRS):
-            ops.copy_slot_rows(self._cache, quads[i:i + ops.COPY_ROWS_MAX_PAIRS])
+            if self.pages is None:
+                ops.copy_slot_rows(self._cache, quads[i:i + ops.COPY_ROWS_MAX_PAIRS])
+            else:
+                ops.copy_page_rows(self._cache, self._page_table, quads[i:i + ops.COPY_ROWS_MAX_PAIRS])
         return done
 
     def _select(self, logits, G, sampled, groups, first, sel):
@@ -829,8 +878,11 @@ class DecodeStream:
             off += 3 * R * 2 * k
 
     def close(self):
-        """free the stream's cache and scratch (requests still running are abandoned)"""
-        self._cache = self._scratch = self._deq = None
+        """free the stream's cache and scratch (requests still running are abandoned; in paged mode their pages return to the
+        pool)"""
+        self._cache = self._scratch = self._deq = self._page_table = None
+        if self.pages is not None:
+            self.pages.release_all()
         self._slots = [None] * self.max_slots
         self.last_logits = None
 
@@ -1159,7 +1211,7 @@ class VQA_LLM:
         return text.strip()
 
     @torch.inference_mode()
-    def free_form_inference_stream(self, items, max_new_tokens=200, slots=16, temperature=0, top_p=None, num_beams=1):
+    def free_form_inference_stream(self, items, max_new_tokens=200, slots=16, temperature=0, top_p=None, num_beams=1, kv_pages=None):
         """free_form_inference for many items on one decode stream (VQAEngine.decode_stream): items are (image, question,
         object_crops, images_long, objects_long); yields (index, text) as each answer completes, with the prompt, stop string
         and post-processing of free_form_inference.  The next item is admitted whenever a slot frees, so up to `slots` answers
@@ -1168,13 +1220,16 @@ class VQA_LLM:
         temperature > 0 samples every item with top_k = self.top_k and top_p; the items take one seed each from torch's
         default generator, in item order, before the first admission (so torch.manual_seed(s) reproduces a call, and a call
         equals free_form_inference of each item in order after the same seed).  num_beams = k > 1 beam-searches every item
-        with self.length_penalty / self.early_stopping on k slots; an item is admitted when k slots are free."""
+        with self.length_penalty / self.early_stopping on k slots; an item is admitted when k slots are free.
+        kv_pages = N: a paged stream (VQAEngine.decode_stream) whose pool of N pages holds the KV rows; an item is then
+        admitted when its slots and the pages it reserves are free, and `slots` bounds the answers decoding at a time."""
         reqs = [(self._prompt_ids(question), image, crops, il, ol) for image, question, crops, il, ol in items]
+        paged = {} if kv_pages is None else dict(kv_pages=int(kv_pages))
         if (temperature is None or not temperature > 0) and num_beams == 1:
-            answers = self._decode_stream(reqs, int(max_new_tokens), int(slots))
+            answers = self._decode_stream(reqs, int(max_new_tokens), int(slots), **paged)
         else:
             answers = self._decode_stream(reqs, int(max_new_tokens), int(slots), settings=self._stream_settings(len(reqs), temperature,
-                                                                                                            top_p, num_beams))
+                                                                                                            top_p, num_beams), **paged)
         for i, out in answers:
             yield i, self._answer_text(out)
 
@@ -1188,10 +1243,10 @@ class VQA_LLM:
         top_k, top_p = check_sampling(self.top_k, top_p)
         return [dict(temperature=temperature, top_k=top_k, top_p=top_p, seed=s) for s in draw_seeds(n)]
 
-    def _decode_stream(self, reqs, max_new_tokens, slots, settings=None):
+    def _decode_stream(self, reqs, max_new_tokens, slots, settings=None, kv_pages=None):
         """(prompt ids, image, object_crops, images_long, objects_long) requests -> (index, new token ids) as each ends, on one
         decode stream with min(slots, len(reqs) * num_beams) slots.  settings: per request, DecodeStream.admit's generation
-        keywords (None: greedy)"""
+        keywords (None: greedy); kv_pages: a paged stream of that many pages"""
         if not reqs:
             return
         e = self.engine
@@ -1203,7 +1258,17 @@ class VQA_LLM:
         # generate() reserves min(max_new_tokens, 2048 - T) positions: the same budget here
         budgets = [max(1, min(max_new_tokens, e.MAX_POSITIONS - T)) for T in lens]
         positions = min(e.MAX_POSITIONS, max(T + n for T, n in zip(lens, budgets)))
-        stream = e.decode_stream(min(slots, len(reqs) * need), positions, self.eos)
+        stream = e.decode_stream(min(slots, len(reqs) * need), positions, self.eos, kv_pages=kv_pages)
+        pages = stream.pages
+        if pages is not None and any(pages.need(T, n, need) > pages.n_pages for T, n in zip(lens, budgets)):
+            stream.close()
+            raise ValueError(f"kv_pages = {kv_pages} cannot hold the largest request of this call")
+
+        def fits():                                      # the next request's slots and pages are free
+            if stream.free_slots < need:
+                return False
+            return pages is None or pages.need(lens[nxt], budgets[nxt], need) <= pages.free_pages
+
         try:
             index = {}
             nxt = 0
@@ -1218,14 +1283,14 @@ class VQA_LLM:
                 index[stream.admit((ids, img, crops, il, ol), budgets[nxt], stop_ids=stop, **gen).id] = nxt
                 nxt += 1
 
-            while nxt < len(reqs) and stream.free_slots >= need:
+            while nxt < len(reqs) and fits():
                 admit()
             remaining = len(reqs)
             while remaining:
                 for r, out in stream.step():
                     remaining -= 1
                     yield index[r.id], out
-                while nxt < len(reqs) and stream.free_slots >= need:
+                while nxt < len(reqs) and fits():
                     admit()
         finally:
             stream.close()
