@@ -282,6 +282,17 @@ int vsb_copy_page_rows_b16(void* pool, int layers, long long layer_stride, long 
                            int row_elems, const void* page_table_i32, int pt_ld, int slots, const void* src, long long src_layer_stride,
                            long long src_slot_stride, long long src_row_stride, int src_slots, const int* quads_i32, int npairs,
                            void* stream);
+/* Swap whole pages of a paged pool [layers] (layer_stride) of n_pages pages (page_stride; page_elems contiguous 2-byte elements
+ * per page) to or from a swap area of PINNED HOST memory [host_slots] (host_slot_stride) [layers] (host_layer_stride): for every
+ * pair i of the HOST arrays pages_i32 / slots_i32, to_host != 0 copies page pages_i32[i] of every layer to host slot
+ * slots_i32[i], to_host == 0 the other way.  The kernel reads and writes the host area through its mapped device address in
+ * 16-byte vectors (pointers and strides must be 16-byte aligned), in stream order with the other launches.  A page or slot out
+ * of range, a destination named twice, a null pointer or host memory that is not mapped pinned memory is refused before any
+ * launch.  One launch per VSB_SWAP_PAGES_PER_LAUNCH pairs. */
+#define VSB_SWAP_PAGES_PER_LAUNCH 384
+int vsb_swap_pages_b16(void* pool, int layers, long long layer_stride, int n_pages, long long page_stride, long long page_elems, void* host,
+                       int host_slots, long long host_slot_stride, long long host_layer_stride, const int* pages_i32, const int* slots_i32,
+                       int n, int to_host, void* stream);
 
 /* NF4 weights: the SEAL VQA LLM's 4-bit mode (the reference's load_4bit: bitsandbytes NF4, double-quantised scales, fp16 compute,
  * LLaVA/llava/model/builder.py:26-43).  Format of W [N, K], K % 64 == 0 (csrc/nf4.cu, oracle/nf4_oracle.py): codes u8 [N, K/2], two

@@ -93,6 +93,7 @@ SIGNATURES.update({
     "vsb_rope_scatter_paged": [c_p, c_ll, c_i, c_i, c_i, c_p, c_ll, c_ll, c_i, c_p, c_i, c_p, c_p, c_p, c_p, c_p, c_i, c_p],
     "vsb_attn_decode_paged": [c_p, c_ll, c_p, c_p, c_p, c_ll, c_ll, c_ll, c_i, c_p, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_i, c_i, c_p],
     "vsb_copy_page_rows_b16": [c_p, c_i, c_ll, c_ll, c_i, c_ll, c_i, c_p, c_i, c_i, c_p, c_ll, c_ll, c_ll, c_i, c_p, c_i, c_p],
+    "vsb_swap_pages_b16": [c_p, c_i, c_ll, c_i, c_ll, c_ll, c_p, c_i, c_ll, c_ll, c_p, c_p, c_i, c_i, c_p],
 })
 
 

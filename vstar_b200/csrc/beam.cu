@@ -16,7 +16,12 @@
 //
 // vsb_copy_page_rows_b16: the same ranged copy into a paged KV pool, each row's page found through the page table; the source is
 // the pool itself (a beam fork) or a contiguous cache (a prefilled prompt's k|v rows written into its pages at admission).
+//
+// vsb_swap_pages_b16: whole pages of every layer between the pool and a swap area of pinned host memory, which the kernel reads
+// and writes through its mapped device address in 16-byte vectors (a preempted request of a growing paged stream).  Pairs
+// travel in the kernel's parameters, VSB_SWAP_PAGES_PER_LAUNCH per launch; the whole list is checked before the first launch.
 #include <algorithm>
+#include <vector>
 
 #include "common.cuh"
 #include "radix_select.cuh"
@@ -323,6 +328,39 @@ void launch_copy_page_rows(const PageRows& g, int row_elems, const RangedPairs& 
     copy_page_rows_kernel<unsigned short, FROM_POOL><<<grid, 256, 0, STREAM(stream)>>>(g, row_elems, pp);
 }
 
+// (pool page, host slot) pairs of one launch: 8 bytes each keep the parameters inside the 4 KB kernel-argument limit
+struct SwapPairs {
+  int page[VSB_SWAP_PAGES_PER_LAUNCH];
+  int slot[VSB_SWAP_PAGES_PER_LAUNCH];
+};
+
+struct SwapArea {
+  uint4* pool;
+  uint4* host;
+  long long layer_stride, page_stride, slot_stride, host_layer_stride, vecs;    // in 16-byte vectors
+};
+
+// grid (chunks, layers, pairs): one page of one layer, 4 vectors in flight per thread (the host side is a PCIe round trip)
+template <bool TO_HOST>
+__global__ void __launch_bounds__(256) swap_pages_kernel(const SwapArea a, const SwapPairs pp) {
+  constexpr int kUnroll = 4;
+  const int p = blockIdx.z;
+  const uint4* pool = a.pool + blockIdx.y * a.layer_stride + pp.page[p] * a.page_stride;
+  const uint4* host = a.host + pp.slot[p] * a.slot_stride + blockIdx.y * a.host_layer_stride;
+  const uint4* src = TO_HOST ? pool : host;
+  uint4* dst = const_cast<uint4*>(TO_HOST ? host : pool);
+  const long long step = (long long)gridDim.x * blockDim.x;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < a.vecs; e += kUnroll * step) {
+    uint4 v[kUnroll];
+#pragma unroll
+    for (int u = 0; u < kUnroll; ++u)
+      if (e + u * step < a.vecs) v[u] = src[e + u * step];
+#pragma unroll
+    for (int u = 0; u < kUnroll; ++u)
+      if (e + u * step < a.vecs) dst[e + u * step] = v[u];
+  }
+}
+
 }  // namespace
 
 extern "C" int vsb_beam_candidates_f32(const void* logits, long long ld, int V, int requests, int k_in, int k, const void* rows_i32,
@@ -450,5 +488,55 @@ extern "C" int vsb_copy_page_rows_b16(void* pool, int layers, long long layer_st
   else
     launch_copy_page_rows<true>(g, row_elems, pp, layers, npairs, rows, stream);
   VSB_LAUNCH_CHECK();
+  return VSB_OK;
+}
+
+extern "C" int vsb_swap_pages_b16(void* pool, int layers, long long layer_stride, int n_pages, long long page_stride, long long page_elems,
+                                  void* host, int host_slots, long long host_slot_stride, long long host_layer_stride, const int* pages_i32,
+                                  const int* slots_i32, int n, int to_host, void* stream) {
+  VSB_CHECK_ARG(pool && host, "vsb_swap_pages_b16: null pointer");
+  VSB_CHECK_ARG(n >= 0 && (n == 0 || (pages_i32 && slots_i32)), "vsb_swap_pages_b16: null page list or n < 0");
+  VSB_CHECK_ARG(layers > 0 && n_pages > 0 && host_slots > 0 && page_elems > 0 && page_stride >= page_elems &&
+                    layer_stride >= (long long)n_pages * page_stride && host_layer_stride >= page_elems &&
+                    host_slot_stride >= (long long)layers * host_layer_stride,
+                "vsb_swap_pages_b16: bad shape");
+  VSB_CHECK_ARG(((reinterpret_cast<uintptr_t>(pool) | reinterpret_cast<uintptr_t>(host) | (uintptr_t)(layer_stride * 2) |
+                  (uintptr_t)(page_stride * 2) | (uintptr_t)(page_elems * 2) | (uintptr_t)(host_slot_stride * 2) |
+                  (uintptr_t)(host_layer_stride * 2)) & 15) == 0,
+                "vsb_swap_pages_b16: pointers and strides must be 16-byte aligned");
+  std::vector<int> seen((size_t)(to_host ? host_slots : n_pages), 0);
+  for (int i = 0; i < n; ++i) {
+    const int pg = pages_i32[i], sl = slots_i32[i];
+    VSB_CHECK_ARG(pg >= 0 && pg < n_pages, "vsb_swap_pages_b16: pair %d: page %d outside [0, %d)", i, pg, n_pages);
+    VSB_CHECK_ARG(sl >= 0 && sl < host_slots, "vsb_swap_pages_b16: pair %d: host slot %d outside [0, %d)", i, sl, host_slots);
+    int& d = seen[to_host ? sl : pg];
+    VSB_CHECK_ARG(!d, "vsb_swap_pages_b16: %s %d is the destination of two pairs", to_host ? "host slot" : "page", to_host ? sl : pg);
+    d = 1;
+  }
+  void* mapped = nullptr;
+  if (cudaHostGetDevicePointer(&mapped, host, 0) != cudaSuccess || mapped == nullptr) {
+    cudaGetLastError();
+    VSB_CHECK_ARG(false, "vsb_swap_pages_b16: the swap area is not mapped pinned host memory");
+  }
+  if (n == 0) return VSB_OK;
+  SwapArea a;
+  a.pool = (uint4*)pool;
+  a.host = (uint4*)mapped;
+  a.layer_stride = layer_stride / 8; a.page_stride = page_stride / 8;
+  a.slot_stride = host_slot_stride / 8; a.host_layer_stride = host_layer_stride / 8;
+  a.vecs = page_elems / 8;
+  const int chunks = (int)std::min<long long>((a.vecs + 1023) / 1024, 64);
+  for (int i = 0; i < n; i += VSB_SWAP_PAGES_PER_LAUNCH) {
+    const int m = std::min(n - i, VSB_SWAP_PAGES_PER_LAUNCH);
+    SwapPairs pp;
+    std::copy(pages_i32 + i, pages_i32 + i + m, pp.page);
+    std::copy(slots_i32 + i, slots_i32 + i + m, pp.slot);
+    dim3 grid(chunks, layers, m);
+    if (to_host)
+      swap_pages_kernel<true><<<grid, 256, 0, STREAM(stream)>>>(a, pp);
+    else
+      swap_pages_kernel<false><<<grid, 256, 0, STREAM(stream)>>>(a, pp);
+    VSB_LAUNCH_CHECK();
+  }
   return VSB_OK;
 }

@@ -366,6 +366,25 @@ def copy_page_rows(pool, page_table, quads, src=None):
     return pool
 
 
+def swap_pages(pool, host, pairs, to_host):
+    """whole pages of every layer between pool [L, n_pages, P, W] and the pinned host swap area host [M, L, P, W] of the same
+    2-byte dtype (vsb_swap_pages_b16): for every (page, slot) in the host list `pairs`, page -> host slot when to_host, else
+    host slot -> page.  Runs on the current stream with no host synchronisation; one launch per SWAP_PAGES_PER_LAUNCH pairs."""
+    import ctypes
+    _chk(pool)
+    if host.is_cuda or not host.is_pinned() or host.dtype != pool.dtype:
+        raise _lib.VsbError("the swap area must be pinned host memory of the pool's dtype")
+    assert pool.dim() == 4 and pool.element_size() == 2 and pool.is_contiguous() and host.is_contiguous()
+    assert host.dim() == 4 and tuple(host.shape[1:]) == (pool.shape[0],) + tuple(pool.shape[2:])
+    n = len(pairs)
+    pages = (ctypes.c_int * max(1, n))(*[int(p) for p, _ in pairs])
+    slots = (ctypes.c_int * max(1, n))(*[int(s) for _, s in pairs])
+    _lib.launches += -(-n // SWAP_PAGES_PER_LAUNCH)
+    call("vsb_swap_pages_b16", pool.data_ptr(), pool.shape[0], pool.stride(0), pool.shape[1], pool.stride(1), pool.shape[2] * pool.shape[3],
+         host.data_ptr(), host.shape[0], host.stride(0), host.stride(1), pages, slots, n, 1 if to_host else 0, _stream())
+    return pool
+
+
 def rope_scatter(qkv, cache, H, D, cos_t, sin_t, slot, length, pos):
     """row b of qkv [B, 3*H*D] -> cache row slot[b]*Tmax + length[b] of cache [Bc, Tmax, 3*H*D] (one layer), q and k rotated at
     position pos[b] like rope_, v copied (vsb_rope_scatter)"""
@@ -644,6 +663,7 @@ def sample_rows_var(x, temperature, top_k, top_p, dtype, seeds, steps, out=None)
 
 BEAM_MAX = 16                                   # VSB_BEAM_MAX
 COPY_ROWS_MAX_PAIRS = 256                       # VSB_COPY_ROWS_MAX_PAIRS
+SWAP_PAGES_PER_LAUNCH = 384                     # VSB_SWAP_PAGES_PER_LAUNCH
 
 
 def beam_candidates(x, rows, scores, k, dtype, out=None):

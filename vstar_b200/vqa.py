@@ -30,7 +30,7 @@ from . import ops
 from .beam import DEFAULT_EARLY_STOPPING, DEFAULT_LENGTH_PENALTY, BeamRequest, check_beams, fork_slots
 from .config import VSMConfig
 from .engine import CoreWeights, LlamaClipCore
-from .kv_pages import PAGE_ROWS, PagePool, pages_for
+from .kv_pages import PAGE_ROWS, GrowingPool, PagePool, pages_for
 from .vsm import CLIP_MEAN, SyntheticTokenizer, _normalize_into
 
 BF = torch.bfloat16
@@ -362,11 +362,12 @@ class VQAEngine(LlamaClipCore):
             res[i] = outs[k]
         return res
 
-    def decode_stream(self, max_slots, max_positions=None, eos_token_id=2, temperature=0, num_beams=1, kv_pages=None):
+    def decode_stream(self, max_slots, max_positions=None, eos_token_id=2, temperature=0, num_beams=1, kv_pages=None, kv_swap_pages=None):
         """Decode batch that admits a request whenever a slot is free (DecodeStream).  max_positions: cache rows per slot
         (default self.max_tokens); a request's prompt plus its max_new_tokens must fit in them.  kv_pages = N: the KV cache
         is a pool of N pages of kv_pages.PAGE_ROWS rows and a request reserves only the pages it needs (DecodeStream); None
-        keeps one cache slot of max_positions rows per decode row.  Generation settings belong to
+        keeps one cache slot of max_positions rows per decode row.  kv_swap_pages = M (with kv_pages): requests take pages as
+        they write them and are preempted to a pinned host swap area of M pages when the pool runs dry.  Generation settings belong to
         each request: DecodeStream.admit(..., temperature=, top_k=, top_p=, seed=, num_beams=, ...) samples or beam-searches
         it; the stream-wide temperature > 0 and num_beams > 1 are refused, since every sampled request needs its own seed."""
         if temperature is not None and temperature > 0:
@@ -375,7 +376,8 @@ class VQAEngine(LlamaClipCore):
         if num_beams != 1:
             raise NotImplementedError("decode_stream takes no stream-wide num_beams: beam-search a request with "
                                       "DecodeStream.admit(..., num_beams=, length_penalty=, early_stopping=)")
-        return DecodeStream(self, max_slots, self.max_tokens if max_positions is None else max_positions, eos_token_id, kv_pages=kv_pages)
+        return DecodeStream(self, max_slots, self.max_tokens if max_positions is None else max_positions, eos_token_id, kv_pages=kv_pages,
+                            kv_swap_pages=kv_swap_pages)
 
     def spliced_length(self, input_ids, n_crops=0, images_long=None, objects_long=None):
         """rows the spliced sequence of build_embeds(input_ids, ...) has, computed on the host (the rule of _splice)"""
@@ -572,6 +574,7 @@ class StreamRequest:
         self.slots = [slot] if slots is None else list(slots)
         self.beam_slot = [slot]                          # cache slot of each running beam, in beam order
         self.score = None
+        self.preemptions = 0                             # times a growing paged stream swapped it out
 
     @property
     def kind(self):
@@ -616,16 +619,29 @@ class DecodeStream:
     is prefilled into a staging cache of its T rows and its k|v rows are written into its pages by one
     vsb_copy_page_rows_b16 launch; steps run vsb_llama_layers_slots_paged.  Logits and tokens are bit-identical to the
     contiguous stream's on the same admission schedule.  The page table is uploaded at admission, the only time it changes
-    where a kernel could read it; a step still makes one device-to-host copy."""
+    where a kernel could read it; a step still makes one device-to-host copy.
+
+    kv_swap_pages = M (with kv_pages; growing mode): the stream also holds a swap area [M, n_layers, PAGE_ROWS, 2d] of pinned
+    host memory, and a request takes only the pages its prompt fills at admission and one page per row whenever a step is about
+    to write a page's first row (kv_pages.GrowingPool, which also states the admission rule).  When the free pages cannot
+    cover a step's growth, the newest running request is preempted: vsb_swap_pages_b16 copies its pages to the swap area and
+    they are free.  Preempted requests resume oldest first, before any new admission, on whichever pages and slots are free
+    (their handles' `slot`, `slots` and beam slots change).  Swap copies run on the stream's CUDA stream in order with the
+    steps; a step that changes the page table sends it in the step's one host-to-device upload.  Swapping keeps every bit, so
+    in batch-invariant mode a request's logits do not depend on being preempted.  `preemptions`, `swapped_pages` (copied
+    out) and `restored_pages` (copied back) count the traffic."""
 
     pages = None                                         # PagePool of a paged stream
+    _swap = None                                         # pinned host swap area of a growing stream
 
-    def __init__(self, engine, max_slots, max_positions, eos_token_id=2, kv_pages=None):
+    def __init__(self, engine, max_slots, max_positions, eos_token_id=2, kv_pages=None, kv_swap_pages=None):
         max_slots, max_positions = int(max_slots), int(max_positions)
         if max_slots < 1:
             raise ValueError(f"max_slots must be >= 1, got {max_slots}")
         if not 1 <= max_positions <= engine.MAX_POSITIONS:
             raise ops._lib.VsbError(f"max_positions {max_positions} outside [1, {engine.MAX_POSITIONS}] (the rows of the RoPE tables)")
+        if kv_swap_pages is not None and kv_pages is None:
+            raise ValueError("kv_swap_pages needs kv_pages: only a paged stream can swap its pages")
         c = engine.cfg
         self.engine, self.eos = engine, eos_token_id
         self.max_slots, self.max_positions = max_slots, max_positions
@@ -634,8 +650,12 @@ class DecodeStream:
         dev, dt = engine.dev, engine.dtype
         if kv_pages is None:
             self._cache = torch.empty((c.n_layers, max_slots, max_positions, 3 * c.hidden), dtype=dt, device=dev)
-        else:
+        elif kv_swap_pages is None:
             self.pages = PagePool(int(kv_pages), max_slots, pages_for(max_positions))
+        else:
+            self.pages = GrowingPool(int(kv_pages), max_slots, pages_for(max_positions), int(kv_swap_pages))
+            self._swap = torch.empty((self.pages.swap_pages, c.n_layers, PAGE_ROWS, 2 * c.hidden), dtype=dt, pin_memory=True)
+        if kv_pages is not None:
             self._cache = torch.empty((c.n_layers, self.pages.n_pages, PAGE_ROWS, 2 * c.hidden), dtype=dt, device=dev)
             self._page_table = torch.zeros(self.pages.table.shape, dtype=torch.int32, device=dev)
         self._scratch = torch.empty((max_slots * (5 * c.hidden + c.intermediate),), dtype=dt, device=dev)
@@ -646,10 +666,21 @@ class DecodeStream:
         self.steps = 0
         self.occupied = 0                                # sum over steps of the rows decoded
         self.last_logits = None                          # (requests in row order, fp32 logits [rows, V]) of the latest call
+        self.preemptions = self.swapped_pages = self.restored_pages = 0
+        self._preempted = {}                             # id -> handle of a request swapped out
+
+    @property
+    def growing(self):
+        return isinstance(self.pages, GrowingPool)
 
     @property
     def free_slots(self):
         return sum(r is None for r in self._slots)
+
+    def free_rows(self, k):
+        """the first k free slots, or None when fewer are free"""
+        rows = [i for i, r in enumerate(self._slots) if r is None]
+        return rows[:k] if len(rows) >= k else None
 
     @property
     def active(self):
@@ -673,7 +704,9 @@ class DecodeStream:
         r.done = True
         for s in r.slots:
             self._slots[s] = None
-        if self.pages is not None:
+        if self.growing:
+            self.pages.finish(r.id)
+        elif self.pages is not None:
             self.pages.release(r.slots)
 
     def _beam_advance(self, r, cand):
@@ -696,7 +729,8 @@ class DecodeStream:
         num_beams = k > 1 runs beam_search's scorer with length_penalty / early_stopping on k slots (stop_ids at most [eos]),
         its first candidates selected here from the prefill logits.  Raises (before any launch) on settings generate() refuses,
         when fewer than num_beams slots are free, num_beams exceeds max_slots or the prompt plus max_new_tokens exceeds
-        max_positions, and in paged mode when the free pages are fewer than the request reserves (RuntimeError)."""
+        max_positions, and in paged mode when the free pages are fewer than the request reserves (RuntimeError; in growing
+        mode also while preempted requests wait and when kv_pages.GrowingPool's admission rule refuses)."""
         self._check_open()
         ids, image, crops, il, ol = request
         max_new_tokens = int(max_new_tokens)
@@ -718,7 +752,9 @@ class DecodeStream:
             raise RuntimeError(f"no free slot: all {self.max_slots} slots of the decode stream are in use" if k == 1 else
                                f"no free slot for {k} beams: {self.free_slots} of the decode stream's {self.max_slots} slots are free")
         slots = [i for i, r in enumerate(self._slots) if r is None][:k]
-        if self.pages is not None:
+        if self.growing:
+            self.pages.check_admit(slots, T, max_new_tokens)
+        elif self.pages is not None:
             self.pages.check_reserve(slots, T, max_new_tokens)
         if sample and seed is None:
             seed = draw_seeds(1)[0]
@@ -769,7 +805,10 @@ class DecodeStream:
         staging = torch.empty((c.n_layers, 1, T, 3 * c.hidden), dtype=e.dtype, device=e.dev)
         ops.llama_layers(e._layer_table, len(e.w.layers), x, 1, T, 0, staging, 1, T, c.hidden, c.n_heads, c.intermediate, c.rms_eps,
                          e.w.rope_cos, e.w.rope_sin, scratch, norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
-        shared = self.pages.reserve(slots, T, max_new_tokens)
+        if self.growing:
+            shared = self.pages.admit(self._next_id, slots, T, max_new_tokens)
+        else:
+            shared = self.pages.reserve(slots, T, max_new_tokens)
         self._page_table.copy_(torch.from_numpy(self.pages.table))
         lo = shared * PAGE_ROWS
         ops.copy_page_rows(self._cache, self._page_table, [(0, slots[0], 0, T)] + [(0, s, lo, T) for s in slots[1:]],
@@ -780,6 +819,7 @@ class DecodeStream:
         that ended at admission since the previous step)"""
         self._check_open()
         done, self._finished = [(r, r.tokens) for r in self._finished], []
+        table = self._schedule() if self.growing else False
         act = self.active
         if not act:
             return done
@@ -796,7 +836,12 @@ class DecodeStream:
             rows += [(r, s, n, b[-1]) for s, b in zip(r.beam_slot, r.beam.beams)]
         B = len(rows)
         lens = [n for _, _, n, _ in rows]
-        meta = torch.tensor([[s for _, s, _, _ in rows], lens, lens], dtype=torch.int32).to(e.dev)
+        meta = np.array([[s for _, s, _, _ in rows], lens, lens], dtype=np.int32)
+        if table:                                        # the grown page table travels with the step's metadata
+            up = torch.from_numpy(np.concatenate([meta.ravel(), self.pages.table.ravel()])).to(e.dev)
+            meta, self._page_table = up[:3 * B].view(3, B), up[3 * B:].view(self.pages.table.shape)
+        else:
+            meta = torch.from_numpy(meta).to(e.dev)
         ids = torch.tensor([t for _, _, _, t in rows], dtype=torch.int64).to(e.dev)
         x = ops.gather_rows(ids, e.w.embed)
         if self.pages is None:
@@ -877,10 +922,35 @@ class DecodeStream:
                                 out=sel[off:off + 3 * R * 2 * k].view(3, R, 2 * k))
             off += 3 * R * 2 * k
 
+    def _schedule(self):
+        """a growing stream's page work before a step (GrowingPool.schedule): swap preempted requests back in or the newest
+        running ones out, then grow -> whether the page table changed"""
+        running = {r.id: r for r in self._slots if r is not None}
+        resumed, preempted, changed = self.pages.schedule()
+        for key, pairs in preempted:
+            r = running[key]
+            ops.swap_pages(self._cache, self._swap, pairs, to_host=True)
+            for s in r.slots:
+                self._slots[s] = None
+            r.preemptions += 1
+            self.preemptions += 1
+            self.swapped_pages += len(pairs)
+            self._preempted[key] = r
+        for key, rows, pairs in resumed:
+            r = self._preempted.pop(key)
+            ops.swap_pages(self._cache, self._swap, [(p, s) for s, p in pairs], to_host=False)
+            new = dict(zip(r.slots, rows))
+            r.slots, r.slot, r.beam_slot = list(rows), rows[0], [new[s] for s in r.beam_slot]
+            for s in rows:
+                self._slots[s] = r
+            self.restored_pages += len(pairs)
+        return changed
+
     def close(self):
         """free the stream's cache and scratch (requests still running are abandoned; in paged mode their pages return to the
-        pool)"""
-        self._cache = self._scratch = self._deq = self._page_table = None
+        pool, and a growing stream's swap area is freed)"""
+        self._cache = self._scratch = self._deq = self._page_table = self._swap = None
+        self._preempted = {}
         if self.pages is not None:
             self.pages.release_all()
         self._slots = [None] * self.max_slots
@@ -1211,7 +1281,8 @@ class VQA_LLM:
         return text.strip()
 
     @torch.inference_mode()
-    def free_form_inference_stream(self, items, max_new_tokens=200, slots=16, temperature=0, top_p=None, num_beams=1, kv_pages=None):
+    def free_form_inference_stream(self, items, max_new_tokens=200, slots=16, temperature=0, top_p=None, num_beams=1, kv_pages=None,
+                                   kv_swap_pages=None):
         """free_form_inference for many items on one decode stream (VQAEngine.decode_stream): items are (image, question,
         object_crops, images_long, objects_long); yields (index, text) as each answer completes, with the prompt, stop string
         and post-processing of free_form_inference.  The next item is admitted whenever a slot frees, so up to `slots` answers
@@ -1222,9 +1293,13 @@ class VQA_LLM:
         equals free_form_inference of each item in order after the same seed).  num_beams = k > 1 beam-searches every item
         with self.length_penalty / self.early_stopping on k slots; an item is admitted when k slots are free.
         kv_pages = N: a paged stream (VQAEngine.decode_stream) whose pool of N pages holds the KV rows; an item is then
-        admitted when its slots and the pages it reserves are free, and `slots` bounds the answers decoding at a time."""
+        admitted when its slots and the pages it reserves are free, and `slots` bounds the answers decoding at a time.
+        kv_swap_pages = M (with kv_pages): a growing paged stream with a host swap area of M pages; an item is then admitted
+        by kv_pages.GrowingPool's rule, taking the pages it writes as it writes them."""
         reqs = [(self._prompt_ids(question), image, crops, il, ol) for image, question, crops, il, ol in items]
         paged = {} if kv_pages is None else dict(kv_pages=int(kv_pages))
+        if kv_swap_pages is not None:
+            paged["kv_swap_pages"] = int(kv_swap_pages)
         if (temperature is None or not temperature > 0) and num_beams == 1:
             answers = self._decode_stream(reqs, int(max_new_tokens), int(slots), **paged)
         else:
@@ -1243,10 +1318,10 @@ class VQA_LLM:
         top_k, top_p = check_sampling(self.top_k, top_p)
         return [dict(temperature=temperature, top_k=top_k, top_p=top_p, seed=s) for s in draw_seeds(n)]
 
-    def _decode_stream(self, reqs, max_new_tokens, slots, settings=None, kv_pages=None):
+    def _decode_stream(self, reqs, max_new_tokens, slots, settings=None, kv_pages=None, kv_swap_pages=None):
         """(prompt ids, image, object_crops, images_long, objects_long) requests -> (index, new token ids) as each ends, on one
         decode stream with min(slots, len(reqs) * num_beams) slots.  settings: per request, DecodeStream.admit's generation
-        keywords (None: greedy); kv_pages: a paged stream of that many pages"""
+        keywords (None: greedy); kv_pages: a paged stream of that many pages; kv_swap_pages: growing, with that swap area"""
         if not reqs:
             return
         e = self.engine
@@ -1258,15 +1333,21 @@ class VQA_LLM:
         # generate() reserves min(max_new_tokens, 2048 - T) positions: the same budget here
         budgets = [max(1, min(max_new_tokens, e.MAX_POSITIONS - T)) for T in lens]
         positions = min(e.MAX_POSITIONS, max(T + n for T, n in zip(lens, budgets)))
-        stream = e.decode_stream(min(slots, len(reqs) * need), positions, self.eos, kv_pages=kv_pages)
+        stream = e.decode_stream(min(slots, len(reqs) * need), positions, self.eos, kv_pages=kv_pages, kv_swap_pages=kv_swap_pages)
         pages = stream.pages
         if pages is not None and any(pages.need(T, n, need) > pages.n_pages for T, n in zip(lens, budgets)):
             stream.close()
             raise ValueError(f"kv_pages = {kv_pages} cannot hold the largest request of this call")
+        if stream.growing and any(pages.need(T, n, need) > pages.swap_pages for T, n in zip(lens, budgets)):
+            stream.close()
+            raise ValueError(f"kv_swap_pages = {kv_swap_pages} cannot hold the largest request of this call")
 
         def fits():                                      # the next request's slots and pages are free
-            if stream.free_slots < need:
+            rows = stream.free_rows(need)
+            if rows is None:
                 return False
+            if stream.growing:
+                return pages.can_admit(rows, lens[nxt], budgets[nxt])
             return pages is None or pages.need(lens[nxt], budgets[nxt], need) <= pages.free_pages
 
         try:
