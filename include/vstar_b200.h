@@ -273,6 +273,27 @@ int vsb_rope_scatter_paged(void* qkv, long long ldq, int B, int H, int D, void* 
 int vsb_attn_decode_paged(const void* q, long long q_rs, const void* k, const void* v, void* o, long long o_rs, long long page_stride,
                           long long row_stride, int page_rows, const void* page_table_i32, int pt_ld, int B, int H, int D, float scale,
                           const void* slot_i32, const void* len_i32, int max_len, int dtype, void* stream);
+/* Chunked prefill over pages: causal attention of R prompt rows in S segments, in one launch.  seg_i32 is device int32 [3][S]
+ * (slot, lo, n): segment s holds rows [lo, lo + n) of the request on page-table row slot, its queries are the next n rows of q
+ * (row stride ldq; segments back to back, R = sum of n), and query row lo + i attends keys [0, lo + i] of that request.  pool
+ * is [pool_rows][2*H*D] k|v rows (k then v) and the layer's pages start at pool row row0: key j sits at pool row row0 +
+ * page_table[slot*pt_ld + j/page_rows]*page_rows + j % page_rows.  Output row r at o + r*ldo.  The wgmma flash-attention body
+ * of vsb_flash_attn_* with the K/V tiles loaded through the page table, so every row equals that kernel's row on the same
+ * logical keys bit for bit; the page rows past a segment's last key may hold anything.  head_dim 64 / 128; page_rows a
+ * multiple of 64 (VSB_ERR_ARG otherwise, before any launch). */
+int vsb_attn_chunk_paged(const void* q, long long ldq, const void* pool, long long pool_rows, long long row0, void* o, long long ldo,
+                         int page_rows, const void* page_table_i32, int pt_ld, const void* seg_i32, int S, int R, int H, int D, float scale,
+                         int dtype, void* stream);
+/* vsb_llama_layers_slots_paged with R prompt rows appended after the B decode rows (B >= 0, R >= 1): x is [B + R, d] and
+ * slot / len / pos int32 [B + R] on the device, chunk row i of a segment (slot, lo, n) having slot, len = pos = lo + i.  The
+ * projections and MLP run on all B + R rows, vsb_rope_scatter_paged places every row's k|v, vsb_attn_decode_paged attends the
+ * B decode rows (max_len >= their len) and vsb_attn_chunk_paged the R chunk rows (seg_i32 [3][S] as there).  scratch: (B + R)
+ * * (5d + inter) elements.  In batch-invariant mode the decode rows equal vsb_llama_layers_slots_paged's and the chunk rows'
+ * final hidden states the one-shot vsb_llama_layers prefill's of the whole prompt (Sq >= 64), bit for bit. */
+int vsb_llama_layers_chunked_paged(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int R, void* pool, int n_pages, int page_rows,
+                                   const void* page_table_i32, int pt_ld, int d, int H, int inter, float rms_eps, const void* rope_cos,
+                                   const void* rope_sin, const void* slot_i32, const void* len_i32, const void* pos_i32, int max_len,
+                                   const void* seg_i32, int S, int norm_folded, void* scratch, void* deq_scratch, int dtype, void* stream);
 /* vsb_copy_slot_rows_b16 into a paged pool [layers] (layer_stride) of pages: for every pair (src, dst, lo, hi) of the HOST array
  * quads_i32, rows [lo, hi) of every layer are copied to page-table row dst's pages.  src NULL: the source is page-table row src of
  * the pool (a beam fork; the slot rules of vsb_copy_slot_rows_b16 apply).  src set: a contiguous cache, row r of slot s at

@@ -96,6 +96,13 @@ SIGNATURES.update({
     "vsb_swap_pages_b16": [c_p, c_i, c_ll, c_i, c_ll, c_ll, c_p, c_i, c_ll, c_ll, c_p, c_p, c_i, c_i, c_p],
 })
 
+# chunked prefill on the paged stream (DecodeStream(kv_pages=N, prefill_chunk=C)): prompt rows ride along with the decode rows
+SIGNATURES.update({
+    "vsb_attn_chunk_paged": [c_p, c_ll, c_p, c_ll, c_ll, c_p, c_ll, c_i, c_p, c_i, c_p, c_i, c_i, c_i, c_i, c_f, c_i, c_p],
+    "vsb_llama_layers_chunked_paged": [c_p, c_i, c_p, c_i, c_i, c_p, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_p, c_i,
+                                       c_p, c_i, c_i, c_p, c_p, c_i, c_p],
+})
+
 
 class LlamaLayer(ctypes.Structure):
     """vsb_llama_layer_t"""

@@ -17,6 +17,7 @@
 #include "wgmma.cuh"
 
 #include <mutex>
+#include <type_traits>
 
 namespace {
 
@@ -97,10 +98,24 @@ struct ASmem {
   static constexpr int TOTAL = BAR_OFF + 128;
 };
 
-template <int D, int NWG, typename T>
-__global__ void __launch_bounds__(128 * (NWG + 1), 1)
-attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                  const AttnTcParams p) {
+// the paged chunk form (vsb_attn_chunk_paged): S segments of query rows, segment s = rows [lo, lo + n) of the request on
+// page-table row slot, its queries rows [qoff, qoff + n) of q; key j of that request is row j % page_rows of page
+// page_table[slot*pt_ld + j / page_rows], found in ONE tensor map over the pool's k|v rows from pool row `row0` (the layer) on
+struct ChunkAttnParams {
+  void* o;
+  long long o_rs;
+  const int* seg;          // int32 [3][S]: slot, lo, n
+  const int* page_table;
+  int S, H, pt_ld, page_rows, row0, d;
+  float scale_log2;
+};
+
+// one body for both forms: only where the query tile's rows and the K/V tiles come from differ (and the paged form zeroes the V
+// rows past the tile's last key, which a page may hold unwritten), so a row's scores, online softmax and P V are the same
+// arithmetic in both, and fully masked key blocks add exact zeros: the forms agree bit for bit on the same logical keys
+template <int D, int NWG, typename T, typename PRM>
+__device__ __forceinline__ void attn_wgmma_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const PRM& p) {
+  constexpr bool PAGED = std::is_same<PRM, ChunkAttnParams>::value;
   using L = ASmem<D, NWG>;
   constexpr int NSUB = L::NSUB;
   constexpr int ST = L::KV_ST;
@@ -114,15 +129,39 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   uint64_t* kv_empty = kv_full + ST;            // [ST]
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
-  const int off = p.Sk - p.Sq;
-  int nblk = (p.Sk + BKV - 1) / BKV;
-  if (p.causal) {
-    int last_key = q0 + BQ - 1 + off;
-    if (last_key > p.Sk - 1) last_key = p.Sk - 1;
-    if (last_key < 0) last_key = 0;
-    const int nb = last_key / BKV + 1;
-    if (nb < nblk) nblk = nb;
+  int q0, h, b, off, nblk;
+  int lo = 0, n = 0, kend = 0, qoff = 0;
+  const int* pages = nullptr;
+  if constexpr (PAGED) {
+    // tile blockIdx.x of the segments' tiles of BQ rows (a tile never spans two segments); CTAs past the last tile exit
+    int tile = blockIdx.x, s = 0;
+    for (; s < p.S; ++s) {
+      n = p.seg[2 * p.S + s];
+      const int nt = (n + BQ - 1) / BQ;
+      if (tile < nt) break;
+      tile -= nt;
+      qoff += n;
+    }
+    if (s == p.S) return;
+    lo = p.seg[p.S + s];
+    pages = p.page_table + (long long)p.seg[s] * p.pt_ld;
+    q0 = tile * BQ;                                    // segment-local first row of the tile
+    h = blockIdx.y;
+    b = 0;
+    off = lo;                                          // row i attends keys [0, lo + i]
+    kend = lo + min(q0 + BQ, n);                       // keys [0, kend) are written; the rows past it may hold anything
+    nblk = (kend - 1) / BKV + 1;
+  } else {
+    q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
+    off = p.Sk - p.Sq;
+    nblk = (p.Sk + BKV - 1) / BKV;
+    if (p.causal) {
+      int last_key = q0 + BQ - 1 + off;
+      if (last_key > p.Sk - 1) last_key = p.Sk - 1;
+      if (last_key < 0) last_key = 0;
+      const int nb = last_key / BKV + 1;
+      if (nb < nblk) nblk = nb;
+    }
   }
 
   if (threadIdx.x == 0) {
@@ -139,17 +178,33 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(q_full, L::Q_BYTES);
 #pragma unroll
-      for (int s = 0; s < NSUB; ++s) tma_load_3d(sQ + s * L::Q_SUB, &tmQ, h * D + s * 64, q0, b, q_full);
+      for (int s = 0; s < NSUB; ++s) tma_load_3d(sQ + s * L::Q_SUB, &tmQ, h * D + s * 64, PAGED ? qoff + q0 : q0, b, q_full);
       int stage = 0;
       uint32_t phase = 0;
       for (int j = 0; j < nblk; ++j) {
         mbar_wait(&kv_empty[stage], phase ^ 1);
         uint8_t* dst = sKV + stage * L::KV_STAGE_BYTES;
-        mbar_arrive_expect_tx(&kv_full[stage], L::KV_STAGE_BYTES);
+        if constexpr (PAGED) {
+          // a block of 128 keys is two boxes of 64 rows, each inside one page (page_rows % 64 == 0); a box wholly past the
+          // tile's last key is not loaded (the consumers zero its V rows)
+          const int halves = min(2, (kend - j * BKV + 63) / 64);
+          mbar_arrive_expect_tx(&kv_full[stage], halves * (L::KV_STAGE_BYTES / 2));
+          for (int hf = 0; hf < halves; ++hf) {
+            const int key = j * BKV + hf * 64;
+            const int row = p.row0 + __ldg(pages + key / p.page_rows) * p.page_rows + key % p.page_rows;
 #pragma unroll
-        for (int s = 0; s < NSUB; ++s) {
-          tma_load_3d(dst + s * SUB_BYTES, &tmK, h * D + s * 64, j * BKV, b, &kv_full[stage]);
-          tma_load_3d(dst + (NSUB + s) * SUB_BYTES, &tmV, h * D + s * 64, j * BKV, b, &kv_full[stage]);
+            for (int s = 0; s < NSUB; ++s) {
+              tma_load_3d(dst + s * SUB_BYTES + hf * (SUB_BYTES / 2), &tmK, h * D + s * 64, row, 0, &kv_full[stage]);
+              tma_load_3d(dst + (NSUB + s) * SUB_BYTES + hf * (SUB_BYTES / 2), &tmV, p.d + h * D + s * 64, row, 0, &kv_full[stage]);
+            }
+          }
+        } else {
+          mbar_arrive_expect_tx(&kv_full[stage], L::KV_STAGE_BYTES);
+#pragma unroll
+          for (int s = 0; s < NSUB; ++s) {
+            tma_load_3d(dst + s * SUB_BYTES, &tmK, h * D + s * 64, j * BKV, b, &kv_full[stage]);
+            tma_load_3d(dst + (NSUB + s) * SUB_BYTES, &tmV, h * D + s * 64, j * BKV, b, &kv_full[stage]);
+          }
         }
         if (++stage == ST) { stage = 0; phase ^= 1; }
       }
@@ -165,8 +220,13 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   const int rr = c * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
   const int qrow[2] = {q0 + rr, q0 + rr + 8};
   int kmax[2];
+  if constexpr (PAGED) {
 #pragma unroll
-  for (int hh = 0; hh < 2; ++hh) kmax[hh] = p.causal ? min(qrow[hh] + off, p.Sk - 1) : (p.Sk - 1);   // last visible key of the row
+    for (int hh = 0; hh < 2; ++hh) kmax[hh] = min(qrow[hh] + off, kend - 1);
+  } else {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) kmax[hh] = p.causal ? min(qrow[hh] + off, p.Sk - 1) : (p.Sk - 1);   // last visible key of the row
+  }
   float m_ref[2] = {0.f, 0.f}, l_part[2] = {0.f, 0.f};
   float o[D / 2];
 #pragma unroll
@@ -181,6 +241,22 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     mbar_wait(&kv_full[stage], phase);
     const uint32_t aK = smem_u32(sKV + stage * L::KV_STAGE_BYTES);
     const uint32_t aV = aK + NSUB * SUB_BYTES;
+    if constexpr (PAGED) {
+      // V rows [kend - j*BKV, BKV) of the last block: unwritten page rows (or not loaded) -> zero, so P = 0 there adds exact zeros.
+      // A SW128 row of a sub-tile is its 128 bytes whatever the swizzle; every consumer thread zeroes a share, then all of them
+      // meet before any reads V
+      const int z0 = kend - j * BKV;
+      if (z0 < BKV) {
+        uint8_t* sv = sKV + stage * L::KV_STAGE_BYTES + NSUB * SUB_BYTES;
+        const int per_sub = (BKV - z0) * 8;             // 16-byte chunks per sub-tile
+        for (int i = threadIdx.x - 128; i < NSUB * per_sub; i += 128 * NWG) {
+          const int s = i / per_sub, r = i - s * per_sub;
+          *reinterpret_cast<uint4*>(sv + s * SUB_BYTES + z0 * 128 + r * 16) = make_uint4(0, 0, 0, 0);
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        asm volatile("bar.sync 1, %0;" ::"r"(128 * NWG) : "memory");
+      }
+    }
     // ---- S = Q K_j^T
     fence_regs<BKV / 2>(s);
     wgmma_fence();
@@ -250,13 +326,33 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = l > 0.f ? 1.f / l : 0.f;
-    if (qrow[hh] < p.Sq) {
+    if constexpr (PAGED) {
+      if (qrow[hh] < n) {
+        T* dst = reinterpret_cast<T*>(p.o) + (long long)(qoff + qrow[hh]) * p.o_rs + (long long)h * D + 2 * t;
+#pragma unroll
+        for (int jj = 0; jj < D / 8; ++jj)
+          *reinterpret_cast<uint32_t*>(dst + 8 * jj) = ElemT<T>::pack2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+      }
+    } else if (qrow[hh] < p.Sq) {
       T* dst = reinterpret_cast<T*>(p.o) + (long long)b * p.o_bs + (long long)qrow[hh] * p.o_rs + (long long)h * D + 2 * t;
 #pragma unroll
       for (int jj = 0; jj < D / 8; ++jj)
         *reinterpret_cast<uint32_t*>(dst + 8 * jj) = ElemT<T>::pack2(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
     }
   }
+}
+
+template <int D, int NWG, typename T>
+__global__ void __launch_bounds__(128 * (NWG + 1), 1)
+attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                  const AttnTcParams p) {
+  attn_wgmma_body<D, NWG, T>(tmQ, tmK, tmV, p);
+}
+
+template <int D, int NWG, typename T>
+__global__ void __launch_bounds__(128 * (NWG + 1), 1)
+attn_chunk_paged_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, const ChunkAttnParams p) {
+  attn_wgmma_body<D, NWG, T>(tmQ, tmKV, tmKV, p);
 }
 
 // ---------------------------------------------------------------- host
@@ -337,3 +433,82 @@ template int vsb_flash_attn_tc<bf16>(const void*, const void*, const void*, void
                                      long long, long long, long long, int, int, int, int, int, int, float, cudaStream_t);
 template int vsb_flash_attn_tc<half>(const void*, const void*, const void*, void*, long long, long long, long long, long long, long long,
                                      long long, long long, long long, int, int, int, int, int, int, float, cudaStream_t);
+
+// ---------------------------------------------------------------- paged chunk prefill
+namespace {
+
+template <int D, int NWG, typename T>
+int launch_chunk(const void* q, long long ldq, int R, const CUtensorMap& tkv, const ChunkAttnParams& p, cudaStream_t st) {
+  using L = ASmem<D, NWG>;
+  CUtensorMap tq;
+  int r = make_map3(&tq, q, (long long)p.H * D, R, 1, ldq, (long long)R * ldq, 64 * NWG, ElemT<T>::tma);
+  if (r) return r;
+  static bool set = false;
+  if (!set) { VSB_CUDA(cudaFuncSetAttribute(attn_chunk_paged_kernel<D, NWG, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL)); set = true; }
+  // sum over segments of ceil(n / BQ) <= ceil(R / BQ) + S tiles; the CTAs past the last tile exit at once
+  dim3 grid((R + 64 * NWG - 1) / (64 * NWG) + p.S, p.H);
+  attn_chunk_paged_kernel<D, NWG, T><<<grid, 128 * (NWG + 1), L::TOTAL, st>>>(tq, tkv, p);
+  VSB_LAUNCH_CHECK();
+  return VSB_OK;
+}
+
+}  // namespace
+
+// tensor map over a pool of `rows` k|v rows of `cols` 2-byte elements (boxes of 64 rows): one map serves every layer of a pool
+int vsb_pool_map(CUtensorMap* map, const void* pool, long long rows, long long cols, int f16) {
+  VSB_CHECK_ARG(pool && rows > 0 && rows < (1LL << 31) && cols % 64 == 0, "vsb_attn_chunk_paged: pool of %lld rows x %lld columns", rows, cols);
+  VSB_CHECK_ARG((reinterpret_cast<uintptr_t>(pool) & 15) == 0, "vsb_attn_chunk_paged: pool must be 16-byte aligned");
+  return make_map3(map, pool, cols, rows, 1, cols, rows * cols, 64, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+}
+
+// the refusals of vsb_attn_chunk_paged, before any launch
+int vsb_attn_chunk_check(const void* q, long long ldq, void* o, long long ldo, int page_rows, const void* page_table, int pt_ld,
+                         const void* seg, int S, int R, int H, int D) {
+  VSB_CHECK_ARG(q && o && page_table && seg, "vsb_attn_chunk_paged: null pointer");
+  VSB_CHECK_ARG(D == 64 || D == 128, "vsb_attn_chunk_paged: head_dim %d unsupported (64/128)", D);
+  VSB_CHECK_ARG(S > 0 && R > 0 && H > 0 && pt_ld > 0, "vsb_attn_chunk_paged: bad shape (S=%d, R=%d, H=%d, pt_ld=%d)", S, R, H, pt_ld);
+  VSB_CHECK_ARG(page_rows >= 64 && page_rows % 64 == 0, "vsb_attn_chunk_paged: page_rows %d is not a multiple of 64", page_rows);
+  VSB_CHECK_ARG((long long)pt_ld * page_rows < (1LL << 30), "vsb_attn_chunk_paged: %d pages of %d rows per page-table row", pt_ld, page_rows);
+  VSB_CHECK_ARG(ldq >= (long long)H * D && ldo >= (long long)H * D && ldq % 8 == 0 && ldo % 2 == 0 &&
+                    (reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(o) & 3) == 0,
+                "vsb_attn_chunk_paged: q must be 16-byte aligned with a row stride of 8k elements, o 4-byte aligned");
+  return VSB_OK;
+}
+
+// causal attention of R chunk rows in S segments over paged keys (see vsb_attn_chunk_paged); the pool's map `tkv` from
+// vsb_pool_map, its rows from row0 on the layer's
+template <typename T>
+int vsb_attn_chunk_paged_tc(const void* q, long long ldq, const CUtensorMap& tkv, long long row0, int d, void* o, long long ldo, int page_rows,
+                            const void* page_table, int pt_ld, const void* seg, int S, int R, int H, int D, float scale, cudaStream_t stream) {
+  ChunkAttnParams p;
+  p.o = o; p.o_rs = ldo;
+  p.seg = reinterpret_cast<const int*>(seg);
+  p.page_table = reinterpret_cast<const int*>(page_table);
+  p.S = S; p.H = H; p.pt_ld = pt_ld; p.page_rows = page_rows; p.row0 = (int)row0; p.d = d;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  const bool two = R > 64;
+  if (D == 64) return two ? launch_chunk<64, 2, T>(q, ldq, R, tkv, p, stream) : launch_chunk<64, 1, T>(q, ldq, R, tkv, p, stream);
+  return two ? launch_chunk<128, 2, T>(q, ldq, R, tkv, p, stream) : launch_chunk<128, 1, T>(q, ldq, R, tkv, p, stream);
+}
+template int vsb_attn_chunk_paged_tc<bf16>(const void*, long long, const CUtensorMap&, long long, int, void*, long long, int, const void*, int,
+                                           const void*, int, int, int, int, float, cudaStream_t);
+template int vsb_attn_chunk_paged_tc<half>(const void*, long long, const CUtensorMap&, long long, int, void*, long long, int, const void*, int,
+                                           const void*, int, int, int, int, float, cudaStream_t);
+
+extern "C" int vsb_attn_chunk_paged(const void* q, long long ldq, const void* pool, long long pool_rows, long long row0, void* o, long long ldo,
+                                    int page_rows, const void* page_table_i32, int pt_ld, const void* seg_i32, int S, int R, int H, int D,
+                                    float scale, int dtype, void* stream) {
+  VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_attn_chunk_paged: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)", dtype);
+  int r = vsb_attn_chunk_check(q, ldq, o, ldo, page_rows, page_table_i32, pt_ld, seg_i32, S, R, H, D);
+  if (r) return r;
+  VSB_CHECK_ARG(row0 >= 0 && row0 % page_rows == 0 && row0 < pool_rows, "vsb_attn_chunk_paged: row0 %lld outside the pool's %lld rows", row0,
+                pool_rows);
+  CUtensorMap tkv;
+  r = vsb_pool_map(&tkv, pool, pool_rows, 2LL * H * D, dtype == VSB_DTYPE_F16);
+  if (r) return r;
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return dtype == VSB_DTYPE_F16 ? vsb_attn_chunk_paged_tc<half>(q, ldq, tkv, row0, H * D, o, ldo, page_rows, page_table_i32, pt_ld, seg_i32, S, R, H,
+                                                                D, scale, st)
+                                : vsb_attn_chunk_paged_tc<bf16>(q, ldq, tkv, row0, H * D, o, ldo, page_rows, page_table_i32, pt_ld, seg_i32, S, R, H,
+                                                                D, scale, st);
+}

@@ -60,6 +60,13 @@ struct LayerOps<half> {
   static constexpr auto attn_decode = vsb_attn_decode_f16;
 };
 
+template <typename T>
+int vsb_attn_chunk_paged_tc(const void* q, long long ldq, const CUtensorMap& tkv, long long row0, int d, void* o, long long ldo, int page_rows,
+                            const void* page_table, int pt_ld, const void* seg, int S, int R, int H, int D, float scale, cudaStream_t stream);
+int vsb_pool_map(CUtensorMap* map, const void* pool, long long rows, long long cols, int f16);
+int vsb_attn_chunk_check(const void* q, long long ldq, void* o, long long ldo, int page_rows, const void* page_table, int pt_ld,
+                         const void* seg, int S, int R, int H, int D);
+
 int vsb_nf4_variant(int M);   // nf4.cu: 0 = the NF4 GEMM of M rows dequantises W and runs the tile kernels
 
 // slot decode (vsb_llama_layers_slots): one new row per sequence, each at its own cache slot and length
@@ -71,6 +78,9 @@ struct SlotRows {
   // of k|v rows, `slot` indexes the rows of page_table [*, pt_ld]
   const void* page_table = nullptr;
   int pt_ld = 0, page_rows = 0, n_pages = 0;
+  // chunked prefill (vsb_llama_layers_chunked_paged): the last chunk_rows rows are prompt rows in n_seg segments (seg [3][n_seg])
+  int chunk_rows = 0, n_seg = 0;
+  const void* seg = nullptr;
 };
 
 template <typename T>
@@ -128,6 +138,9 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
     VSB_CHECK_ARG((long long)2 * sqc * rows * 4 <= rows * d * 2, "vsb_llama_layers: scratch too small for the row statistics");
     VSB_TRY(K::rowsq(xb, d, sq_a, (int)rows, d, stream));
   }
+  // one tensor map over the whole pool serves the chunk attention of every layer
+  CUtensorMap pool_map;
+  if (slots && slots->chunk_rows) VSB_TRY(vsb_pool_map(&pool_map, cache, (long long)n_layers * slots->n_pages * slots->page_rows, 2LL * d, ElemT<T>::is_f16));
   // RoPE in the QKV epilogue (head_dim 128): q / k reach the cache already rotated
   const bool rope_fused = g_fuse_rope && hd == 128 && d % 256 == 0 && k_start == nullptr && slots == nullptr && tiles;
 
@@ -173,10 +186,17 @@ static int llama_layers(const vsb_llama_layer_t* layers, int n_layers, void* x, 
         // q rotated in place in scratch, k|v to the row's page; attention reads q there and k|v through the page table
         const long long kv = 2LL * d, page = (long long)slots->page_rows * kv;
         T* pl = reinterpret_cast<T*>(cache) + (long long)li * slots->n_pages * page;  // [n_pages, page_rows, 2d]
+        // chunk rows: row i of a segment is a row with len = pos = lo + i, so the same scatter places it
+        const int nd = B - slots->chunk_rows;                                         // decode rows, first
         VSB_TRY(vsb_rope_scatter_paged(qkv, ld, B, H, hd, pl, page, kv, slots->page_rows, slots->page_table, slots->pt_ld, slots->slot, slots->len,
                                        positions, rope_cos, rope_sin, dt, stream));
-        VSB_TRY(vsb_attn_decode_paged(qkv, ld, pl, pl + d, attn, d, page, kv, slots->page_rows, slots->page_table, slots->pt_ld, B, H, hd, scale,
-                                      slots->slot, slots->len, slots->max_len, dt, stream));
+        if (nd > 0)
+          VSB_TRY(vsb_attn_decode_paged(qkv, ld, pl, pl + d, attn, d, page, kv, slots->page_rows, slots->page_table, slots->pt_ld, nd, H, hd,
+                                        scale, slots->slot, slots->len, slots->max_len, dt, stream));
+        if (slots->chunk_rows)
+          VSB_TRY(vsb_attn_chunk_paged_tc<T>(qkv + nd * ld, ld, pool_map, (long long)li * slots->n_pages * slots->page_rows, d, attn + (long long)nd * d,
+                                             d, slots->page_rows, slots->page_table, slots->pt_ld, slots->seg, slots->n_seg, slots->chunk_rows, H,
+                                             hd, scale, reinterpret_cast<cudaStream_t>(stream)));
       } else {
         VSB_TRY(vsb_rope_scatter(qkv, ld, B, H, hd, cl, ld, Tmax, slots->slot, slots->len, positions, rope_cos, rope_sin, dt, stream));
         VSB_TRY(vsb_attn_decode_slots(cl, cl + d, cl + 2 * d, attn, (long long)Tmax * ld, ld, d, B, H, hd, scale, slots->slot, slots->len,
@@ -280,4 +300,37 @@ extern "C" int vsb_llama_layers_slots_paged(const vsb_llama_layer_t* layers, int
                               nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
   return llama_layers<bf16>(layers, n_layers, x, B, 1, 0, pool, B, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr, 0,
                             nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
+}
+
+// Chunked prefill: vsb_llama_layers_slots_paged on B decode rows followed by R prompt rows in S segments (x [B + R, d]).  Every
+// kernel runs on all B + R rows but attention: vsb_attn_decode_paged for the decode rows, vsb_attn_chunk_paged for the chunk rows.
+extern "C" int vsb_llama_layers_chunked_paged(const vsb_llama_layer_t* layers, int n_layers, void* x, int B, int R, void* pool, int n_pages,
+                                              int page_rows, const void* page_table_i32, int pt_ld, int d, int H, int inter, float rms_eps,
+                                              const void* rope_cos, const void* rope_sin, const void* slot_i32, const void* len_i32,
+                                              const void* pos_i32, int max_len, const void* seg_i32, int S, int norm_folded, void* scratch,
+                                              void* deq_scratch, int dtype, void* stream) {
+  VSB_CHECK_ARG(dtype == VSB_DTYPE_BF16 || dtype == VSB_DTYPE_F16, "vsb_llama_layers_chunked_paged: dtype %d (VSB_DTYPE_BF16 / VSB_DTYPE_F16)",
+                dtype);
+  VSB_CHECK_ARG(page_table_i32 && n_pages > 0 && pt_ld > 0 && B >= 0 && H > 0 && d % H == 0,
+                "vsb_llama_layers_chunked_paged: null page table, empty pool or bad shape");
+  VSB_CHECK_ARG((long long)n_layers * n_pages * page_rows < (1LL << 31), "vsb_llama_layers_chunked_paged: pool of %d x %d x %d rows", n_layers,
+                n_pages, page_rows);
+  // the chunk kernel's refusals before the first launch of the stack (its q / o are the runner's scratch rows)
+  const long long rows = (long long)B + R;
+  const void* q = reinterpret_cast<const char*>(scratch) + rows * (2LL * d + inter) * 2 + (long long)B * 3 * d * 2;
+  VSB_TRY(vsb_attn_chunk_check(q, 3LL * d, scratch, d, page_rows, page_table_i32, pt_ld, seg_i32, S, R, H, d / H));
+  SlotRows s{slot_i32, len_i32, max_len};
+  s.page_table = page_table_i32;
+  s.pt_ld = pt_ld;
+  s.page_rows = page_rows;
+  s.n_pages = n_pages;
+  s.chunk_rows = R;
+  s.n_seg = S;
+  s.seg = seg_i32;
+  const int Tmax = pt_ld * page_rows;
+  if (dtype == VSB_DTYPE_F16)
+    return llama_layers<half>(layers, n_layers, x, (int)rows, 1, 0, pool, (int)rows, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr,
+                              0, nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
+  return llama_layers<bf16>(layers, n_layers, x, (int)rows, 1, 0, pool, (int)rows, Tmax, d, H, inter, rms_eps, rope_cos, rope_sin, pos_i32, nullptr,
+                            0, nullptr, 0, norm_folded, scratch, deq_scratch, stream, &s);
 }

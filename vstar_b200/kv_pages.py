@@ -26,6 +26,25 @@ def pages_for(rows, page_rows=PAGE_ROWS):
     return -(-int(rows) // page_rows)
 
 
+def plan_chunks(pending, budget):
+    """the prompt rows one step of a chunked-prefill stream (DecodeStream(prefill_chunk=C)) carries: pending = [(request,
+    rows written, prompt rows)] of the requests still prefilling, in admission order; budget = C.  -> [(request, first row,
+    rows)], at most `budget` rows in all, taken first come first served: a request's rows continue where its last segment
+    ended, and the next request starts only once the previous one's prompt is complete in this step.  A request's prompt is
+    complete (its first token is due) in the step whose segment ends at its last row."""
+    if budget < 1:
+        raise ValueError(f"prefill_chunk must be >= 1, got {budget}")
+    out = []
+    for r, done, total in pending:
+        if budget == 0:
+            break
+        n = min(total - done, budget)
+        if n > 0:
+            out.append((r, done, n))
+            budget -= n
+    return out
+
+
 class PagePool:
     """pages [0, n_pages) and a page table of `rows` rows x pages_per_row entries (host copy; DecodeStream uploads it).
     Entries past a row's pages are 0, a valid page that the kernels never read (they stop at the row's length)."""

@@ -312,6 +312,54 @@ def llama_layers_slots_paged(table, n_layers, x, pool, page_table, eps, rope_cos
     return x
 
 
+def llama_layers_chunked_paged(table, n_layers, x, pool, page_table, eps, rope_cos, rope_sin, scratch, slot, length, pos, max_len, seg,
+                               chunk_rows, H, inter, norm_folded=False, deq_scratch=None):
+    """llama_layers_slots_paged on B decode rows followed by R = chunk_rows prompt rows (vsb_llama_layers_chunked_paged): x [B + R, d]
+    in place; slot / length / pos int32 [B + R] on the device (chunk row i of segment (slot, lo, n) has length = pos = lo + i); seg
+    int32 [3, S] on the device (slot, lo, n per segment; R = the sum of n); max_len >= the decode rows' lengths.
+    scratch: (B + R) * (5d + inter) elements; NF4 tables as in llama_layers_slots."""
+    sfx = _sfx(x, pool, scratch, rope_cos, rope_sin)
+    rows, d = x.shape
+    L, n_pages, P, W = pool.shape
+    P, ppr = _pool_shape(pool, page_table)
+    assert x.is_contiguous() and W == 2 * d and L >= n_layers
+    assert scratch.numel() >= rows * (5 * d + inter)
+    _i32_rows(slot, length, pos, n=rows)
+    _chk(seg, torch.int32)
+    assert seg.dim() == 2 and seg.shape[0] == 3 and seg.is_contiguous()
+    S, R = seg.shape[1], int(chunk_rows)
+    assert 1 <= R <= rows
+    if table[0].wqkv_scales:
+        if sfx != "f16" or norm_folded:
+            raise _lib.VsbError("NF4 layers run in fp16 with unfolded norms")
+        _chk(deq_scratch, F16)
+        assert deq_scratch.is_contiguous() and deq_scratch.numel() >= 2 * inter * d
+    _lib.launches += 8 * n_layers
+    call("vsb_llama_layers_chunked_paged", table, n_layers, x.data_ptr(), rows - R, R, pool.data_ptr(), n_pages, P, page_table.data_ptr(), ppr,
+         d, H, inter, float(eps), rope_cos.data_ptr(), rope_sin.data_ptr(), slot.data_ptr(), length.data_ptr(), pos.data_ptr(), int(max_len),
+         seg.data_ptr(), S, 1 if norm_folded else 0, scratch.data_ptr(), _p(deq_scratch), _DTYPE[sfx], _stream())
+    return x
+
+
+def attn_chunk_paged(q, pool, page_table, out, H, D, scale, seg, layer=0):
+    """causal attention of prompt-chunk rows over a paged pool [n_layers, n_pages, P, 2*H*D] (or one layer's [n_pages, P, 2*H*D]) of
+    k|v rows, P a multiple of 64 (vsb_attn_chunk_paged): seg int32 [3, S] on the device lists (slot, lo, n) per segment; the
+    segments' query rows are q's rows back to back (q [R, >= H*D], unit inner stride), and row lo + i of segment s attends keys
+    [0, lo + i] of the pages page_table[slot] lists in layer `layer` -> out [R, H*D]"""
+    sfx = _sfx(q, pool, out)
+    pq, R, _, ldq = _rows2d(q)
+    P, ppr = _pool_shape(pool, page_table)
+    assert pool.shape[-1] == 2 * H * D and out.stride(1) == 1 and out.shape[0] == R
+    _chk(seg, torch.int32)
+    assert seg.dim() == 2 and seg.shape[0] == 3 and seg.is_contiguous()
+    pool_rows = pool.numel() // pool.shape[-1]
+    row0 = layer * (pool.shape[-3] * P)
+    _lib.launches += 1
+    call("vsb_attn_chunk_paged", pq, ldq, pool.data_ptr(), pool_rows, row0, out.data_ptr(), out.stride(0), P, page_table.data_ptr(), ppr,
+         seg.data_ptr(), seg.shape[1], R, H, D, float(scale), _DTYPE[sfx], _stream())
+    return out
+
+
 def rope_scatter_paged(qkv, pool, page_table, H, D, cos_t, sin_t, slot, length, pos):
     """rope_scatter into one layer's pages [n_pages, P, 2*H*D] (vsb_rope_scatter_paged): row b of qkv [B, 3*H*D] has q rotated in
     place, its rotated k and its v go to row length[b] of the pages page_table[slot[b]] lists"""

@@ -186,7 +186,8 @@ def open_final_request(vqa_llm, image, question, missing, results):
 
 
 def answer_open_many(vqa_llm, vsm, items, slots=16, searches_in_flight=8, minimum_size_scale=4.0, minimum_size=224, search_batch=16,
-                     search_kwargs=None, temperature=0, top_p=None, num_beams=1, kv_pages=None, kv_swap_pages=None):
+                     search_kwargs=None, temperature=0, top_p=None, num_beams=1, kv_pages=None, kv_swap_pages=None,
+                     prefill_chunk=None):
     """app.py's inference() for many (image, question) pairs (PIL images), in three phases:
       A. every direct answer on one decode stream (vqa_llm.free_form_inference_stream, `slots` answers decoding at a time);
       B. every missing object's search on one SearchController.stream, `searches_in_flight` searches at a time;
@@ -195,12 +196,13 @@ def answer_open_many(vqa_llm, vsm, items, slots=16, searches_in_flight=8, minimu
     free_form_inference takes them; the defaults decode greedily, as app.py does.  kv_pages = N runs both decode phases on a
     paged stream whose KV pool holds N pages (VQAEngine.decode_stream), so more answers fit in the same memory; kv_swap_pages = M
     (with kv_pages) lets an answer take pages as it writes them, preempting answers to a pinned host area of M pages when the
-    pool runs dry.
+    pool runs dry.  prefill_chunk = C (with kv_pages) prefills admitted prompts C rows per step alongside the running answers
+    (DecodeStream), so admissions stop stalling them.
     -> per item, in input order, app.py's four outputs: (direct answer, None, None, None) when nothing is missing, else
     ("Need to conduct visual search to search for: ...", search-summary string, annotated np.ndarray image, final answer)."""
     # only settings that differ from greedy are passed on, so a VQA LLM with the greedy-only signature still serves the default
     gen = {k: v for k, v, d in (("temperature", temperature, 0), ("top_p", top_p, None), ("num_beams", num_beams, 1), ("kv_pages", kv_pages, None),
-                                           ("kv_swap_pages", kv_swap_pages, None))
+                                           ("kv_swap_pages", kv_swap_pages, None), ("prefill_chunk", prefill_chunk, None))
            if v != d}
     items = [(image.convert("RGB"), question) for image, question in items]
     bg = tuple(int(x * 255) for x in vqa_llm.image_processor.image_mean)
@@ -276,6 +278,9 @@ def build_parser():
                    help="with --kv-pages: answers take pages as they write them, and when the pool runs dry the newest answer is "
                         "swapped to a pinned host area of this many pages until pages free (default: reserve every answer's pages "
                         "at admission)")
+    p.add_argument("--prefill-chunk", default=None, type=int,
+                   help="with --kv-pages: prefill admitted prompts this many rows per decode step, alongside the running answers "
+                        "(default: prefill each prompt on its own at admission)")
     return p
 
 
@@ -330,7 +335,7 @@ def main(argv=None, vqa_llm=None, vsm=None):
     answers = answer_open_many(vqa_llm, vsm, items, slots=args.slots, searches_in_flight=args.searches_in_flight,
                                minimum_size_scale=args.minimum_size_scale, minimum_size=args.minimum_size, search_batch=args.search_batch,
                                temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams, kv_pages=args.kv_pages,
-                               kv_swap_pages=args.kv_swap_pages)
+                               kv_swap_pages=args.kv_swap_pages, prefill_chunk=args.prefill_chunk)
     return write_answers(args.output_path, questions, answers, args.save_images)
 
 

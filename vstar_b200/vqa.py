@@ -30,7 +30,7 @@ from . import ops
 from .beam import DEFAULT_EARLY_STOPPING, DEFAULT_LENGTH_PENALTY, BeamRequest, check_beams, fork_slots
 from .config import VSMConfig
 from .engine import CoreWeights, LlamaClipCore
-from .kv_pages import PAGE_ROWS, GrowingPool, PagePool, pages_for
+from .kv_pages import PAGE_ROWS, GrowingPool, PagePool, pages_for, plan_chunks
 from .vsm import CLIP_MEAN, SyntheticTokenizer, _normalize_into
 
 BF = torch.bfloat16
@@ -362,12 +362,15 @@ class VQAEngine(LlamaClipCore):
             res[i] = outs[k]
         return res
 
-    def decode_stream(self, max_slots, max_positions=None, eos_token_id=2, temperature=0, num_beams=1, kv_pages=None, kv_swap_pages=None):
+    def decode_stream(self, max_slots, max_positions=None, eos_token_id=2, temperature=0, num_beams=1, kv_pages=None, kv_swap_pages=None,
+                      prefill_chunk=None):
         """Decode batch that admits a request whenever a slot is free (DecodeStream).  max_positions: cache rows per slot
         (default self.max_tokens); a request's prompt plus its max_new_tokens must fit in them.  kv_pages = N: the KV cache
         is a pool of N pages of kv_pages.PAGE_ROWS rows and a request reserves only the pages it needs (DecodeStream); None
         keeps one cache slot of max_positions rows per decode row.  kv_swap_pages = M (with kv_pages): requests take pages as
-        they write them and are preempted to a pinned host swap area of M pages when the pool runs dry.  Generation settings belong to
+        they write them and are preempted to a pinned host swap area of M pages when the pool runs dry.  prefill_chunk = C (with
+        kv_pages, without kv_swap_pages): admitted prompts are prefilled C rows per step alongside the running requests' decode
+        rows (DecodeStream).  Generation settings belong to
         each request: DecodeStream.admit(..., temperature=, top_k=, top_p=, seed=, num_beams=, ...) samples or beam-searches
         it; the stream-wide temperature > 0 and num_beams > 1 are refused, since every sampled request needs its own seed."""
         if temperature is not None and temperature > 0:
@@ -377,7 +380,7 @@ class VQAEngine(LlamaClipCore):
             raise NotImplementedError("decode_stream takes no stream-wide num_beams: beam-search a request with "
                                       "DecodeStream.admit(..., num_beams=, length_penalty=, early_stopping=)")
         return DecodeStream(self, max_slots, self.max_tokens if max_positions is None else max_positions, eos_token_id, kv_pages=kv_pages,
-                            kv_swap_pages=kv_swap_pages)
+                            kv_swap_pages=kv_swap_pages, prefill_chunk=prefill_chunk)
 
     def spliced_length(self, input_ids, n_crops=0, images_long=None, objects_long=None):
         """rows the spliced sequence of build_embeds(input_ids, ...) has, computed on the host (the rule of _splice)"""
@@ -575,6 +578,11 @@ class StreamRequest:
         self.beam_slot = [slot]                          # cache slot of each running beam, in beam order
         self.score = None
         self.preemptions = 0                             # times a growing paged stream swapped it out
+        self.prefilled = length                          # prompt rows written to the cache (a chunked-prefill stream: 0 at admission)
+
+    @property
+    def prefilling(self):
+        return self.prefilled < self.prompt_len
 
     @property
     def kind(self):
@@ -629,12 +637,23 @@ class DecodeStream:
     (their handles' `slot`, `slots` and beam slots change).  Swap copies run on the stream's CUDA stream in order with the
     steps; a step that changes the page table sends it in the step's one host-to-device upload.  Swapping keeps every bit, so
     in batch-invariant mode a request's logits do not depend on being preempted.  `preemptions`, `swapped_pages` (copied
-    out) and `restored_pages` (copied back) count the traffic."""
+    out) and `restored_pages` (copied back) count the traffic.
+
+    prefill_chunk = C (with kv_pages, not with kv_swap_pages; chunked prefill): admit() reserves the request's pages and builds
+    its embedding but runs no layer: the request is *prefilling* (handle.prefilled counts its prompt rows written, its
+    `tokens` are empty).  Each step takes up to C prompt rows of the prefilling requests, first come first served
+    (kv_pages.plan_chunks), and runs them after the running requests' decode rows in ONE vsb_llama_layers_chunked_paged call,
+    so the running requests gain a token in every step while prompts are admitted.  A request whose last prompt row ran takes
+    its first token from that row's logits in the same step, as admission gives it in the unchunked stream (argmax; (seed,
+    step 0); a beam request copies its prompt rows from the last shared page on into its other beams' pages and selects its
+    first candidates from k_in = 1).  lm_head runs on the decode rows and those last rows only.  In batch-invariant mode
+    every token and logit equals the unchunked paged stream's on the same admission schedule for prompts of 64 rows or more
+    (shorter prompts are prefilled there by the mma.sync attention kernel, which rounds differently)."""
 
     pages = None                                         # PagePool of a paged stream
     _swap = None                                         # pinned host swap area of a growing stream
 
-    def __init__(self, engine, max_slots, max_positions, eos_token_id=2, kv_pages=None, kv_swap_pages=None):
+    def __init__(self, engine, max_slots, max_positions, eos_token_id=2, kv_pages=None, kv_swap_pages=None, prefill_chunk=None):
         max_slots, max_positions = int(max_slots), int(max_positions)
         if max_slots < 1:
             raise ValueError(f"max_slots must be >= 1, got {max_slots}")
@@ -642,6 +661,16 @@ class DecodeStream:
             raise ops._lib.VsbError(f"max_positions {max_positions} outside [1, {engine.MAX_POSITIONS}] (the rows of the RoPE tables)")
         if kv_swap_pages is not None and kv_pages is None:
             raise ValueError("kv_swap_pages needs kv_pages: only a paged stream can swap its pages")
+        if prefill_chunk is not None:
+            if isinstance(prefill_chunk, bool) or int(prefill_chunk) != prefill_chunk or prefill_chunk < 1:
+                raise ValueError(f"prefill_chunk must be an integer >= 1, got {prefill_chunk!r}")
+            if kv_pages is None:
+                raise ValueError("prefill_chunk needs kv_pages: prompt chunks are written through the page table")
+            if kv_swap_pages is not None:
+                raise ValueError("prefill_chunk does not combine with kv_swap_pages (a growing pool)")
+            prefill_chunk = int(prefill_chunk)
+        self.chunk = prefill_chunk
+        self._prefilling = []                            # handles of the requests still prefilling, in admission order
         c = engine.cfg
         self.engine, self.eos = engine, eos_token_id
         self.max_slots, self.max_positions = max_slots, max_positions
@@ -658,7 +687,8 @@ class DecodeStream:
         if kv_pages is not None:
             self._cache = torch.empty((c.n_layers, self.pages.n_pages, PAGE_ROWS, 2 * c.hidden), dtype=dt, device=dev)
             self._page_table = torch.zeros(self.pages.table.shape, dtype=torch.int32, device=dev)
-        self._scratch = torch.empty((max_slots * (5 * c.hidden + c.intermediate),), dtype=dt, device=dev)
+        rows = max_slots + (prefill_chunk or 0)          # a chunked step's decode rows plus at most C prompt rows
+        self._scratch = torch.empty((rows * (5 * c.hidden + c.intermediate),), dtype=dt, device=dev)
         self._deq = torch.empty((2 * c.intermediate * c.hidden,), dtype=dt, device=dev) if getattr(engine.w, "quant", None) else None
         self._slots = [None] * max_slots                 # slot -> active StreamRequest (a beam request in each of its slots)
         self._finished = []                              # ended at admission; reported by the next step()
@@ -761,6 +791,9 @@ class DecodeStream:
         slot = slots[0]
         x = e.build_embeds(ids, image, crops, il, ol)
         assert x.shape[0] == T
+        if self.chunk is not None:
+            return self._admit_chunked(x, T, max_new_tokens, stop_ids, slots, sample, temperature, top_k, top_p, seed, beam, k, len(ids),
+                                       length_penalty, early_stopping)
         c = e.cfg
         scratch = torch.empty((T * (2 * c.hidden + c.intermediate),), dtype=e.dtype, device=e.dev)
         if self.pages is None:
@@ -797,6 +830,23 @@ class DecodeStream:
             self._finished.append(r)
         return r
 
+    def _admit_chunked(self, x, T, max_new_tokens, stop_ids, slots, sample, temperature, top_k, top_p, seed, beam, k, n_ids, length_penalty,
+                       early_stopping):
+        """a chunked-prefill stream's admission: the request's pages and its embedding x [T, d], held until step() has run its
+        last prompt row"""
+        shared = self.pages.reserve(slots, T, max_new_tokens)
+        self._page_table.copy_(torch.from_numpy(self.pages.table))
+        r = StreamRequest(self._next_id, slots[0], T, max_new_tokens, stop_ids, temperature=float(temperature) if sample else 0,
+                          top_k=top_k if sample else 0, top_p=top_p if sample else None, seed=seed if sample else None,
+                          beam=BeamRequest(k, n_ids, max_new_tokens, self.eos, length_penalty, early_stopping) if beam else None,
+                          slots=slots)
+        r.prefilled, r._x, r._shared = 0, x, shared
+        self._next_id += 1
+        for s in slots:
+            self._slots[s] = r
+        self._prefilling.append(r)
+        return r
+
     def _admit_paged(self, x, T, max_new_tokens, slots, scratch):
         """prefill x [T, d] into a staging cache of T rows with the contiguous runner, reserve the request's pages and write
         its k|v rows into them: all T rows into the first beam's pages (the shared full pages among them), rows from the
@@ -824,6 +874,12 @@ class DecodeStream:
         if not act:
             return done
         e, c = self.engine, self.engine.cfg
+        if self.chunk is not None:
+            act = [r for r in act if not r.prefilling]
+            segs = plan_chunks([(r, r.prefilled, r.prompt_len) for r in self._prefilling], self.chunk)
+        else:
+            segs = []
+        comp = [r for r, lo, n in segs if lo + n == r.prompt_len]     # prompts complete in this step: their first token is due
         greedy = [r for r in act if r.kind == "greedy"]
         sampled = [r for r in act if r.kind == "sample"]
         beams = [r for r in act if r.kind == "beam"]
@@ -836,6 +892,8 @@ class DecodeStream:
             rows += [(r, s, n, b[-1]) for s, b in zip(r.beam_slot, r.beam.beams)]
         B = len(rows)
         lens = [n for _, _, n, _ in rows]
+        if segs:
+            return self._step_chunked(done, rows, greedy, sampled, beams, first, segs, comp)
         meta = np.array([[s for _, s, _, _ in rows], lens, lens], dtype=np.int32)
         if table:                                        # the grown page table travels with the step's metadata
             up = torch.from_numpy(np.concatenate([meta.ravel(), self.pages.table.ravel()])).to(e.dev)
@@ -854,17 +912,87 @@ class DecodeStream:
                                          norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
         hn = ops.rmsnorm(x, e.w.final_norm, c.rms_eps)
         logits = ops.gemm(hn, e.w.lm_head, out_dtype=torch.float32)
-        G, S = len(greedy), len(sampled)
-        groups = {}                                      # k -> beam requests of that k, in row order
+        groups = {}                                      # (k, beams in) -> beam requests of that k, in row order
         for r in beams:
-            groups.setdefault(r.beam.k, []).append(r)
-        sel = torch.empty((G + S + sum(3 * len(g) * 2 * k for k, g in groups.items()),), dtype=torch.int32, device=e.dev)
+            groups.setdefault((r.beam.k, r.beam.k), []).append(r)
+        return self._finish_step(done, logits, greedy, sampled, groups, first, [r for r, _, _, _ in rows], B)
+
+    def _step_chunked(self, done, rows, greedy, sampled, beams, first, segs, comp):
+        """step() of a chunked-prefill stream whose step carries prompt rows (segs: kv_pages.plan_chunks' segments; comp: the
+        requests whose prompt completes)"""
+        e, c = self.engine, self.engine.cfg
+        B, R, S = len(rows), sum(n for _, _, n in segs), len(segs)
+        # logits rows: greedy decode rows then the greedy prompts completing, the same for sampled, then the beam decode rows and
+        # each completing beam request's one row (its first candidates are taken from k_in = 1); gather picks them from x
+        end, o = {}, B
+        for r, lo, n in segs:
+            o += n
+            end[r.id] = o - 1
+        cg, cs, cb = ([r for r in comp if r.kind == kd] for kd in ("greedy", "sample", "beam"))
+        G0, S0 = len(greedy), len(sampled)
+        pick = list(range(G0)) + [end[r.id] for r in cg] + list(range(G0, G0 + S0)) + [end[r.id] for r in cs] + \
+            list(range(G0 + S0, B)) + [end[r.id] for r in cb]
+        nb = len(pick) - B                                # logits rows past the decode rows' own
+        shift = {r.id: first[r.id] + len(cg) + len(cs) for r in beams}
+        for i, r in enumerate(cb):
+            shift[r.id] = len(pick) - len(cb) + i
+        lens = [n for _, _, n, _ in rows] + [lo + i for r, lo, n in segs for i in range(n)]
+        slots = [s for _, s, _, _ in rows] + [r.slot for r, lo, n in segs for _ in range(n)]
+        # one upload: the gather rows (int64, first so their view is aligned), slot / len / pos of every row, the segments
+        host = np.empty(2 * len(pick) * (nb > 0) + 3 * (B + R) + 3 * S, dtype=np.int32)
+        q = 2 * len(pick) * (nb > 0)
+        if nb:
+            host[:q].view(np.int64)[:] = pick
+        host[q:q + 3 * (B + R)] = np.array([slots, lens, lens], dtype=np.int32).ravel()
+        host[q + 3 * (B + R):] = np.array([[r.slot for r, _, _ in segs], [lo for _, lo, _ in segs], [n for _, _, n in segs]],
+                                          dtype=np.int32).ravel()
+        up = torch.from_numpy(host).to(e.dev)
+        meta = up[q:q + 3 * (B + R)].view(3, B + R)
+        seg = up[q + 3 * (B + R):].view(3, S)
+        x = torch.empty((B + R, c.hidden), dtype=e.dtype, device=e.dev)
+        if B:
+            ids = torch.tensor([t for _, _, _, t in rows], dtype=torch.int64).to(e.dev)
+            ops.gather_rows(ids, e.w.embed, out=x[:B])
+        o = B
+        for r, lo, n in segs:
+            ops.copy2d(r._x[lo:lo + n], x[o:o + n])
+            o += n
+        ops.llama_layers_chunked_paged(e._layer_table, len(e.w.layers), x, self._cache, self._page_table, c.rms_eps, e.w.rope_cos,
+                                       e.w.rope_sin, self._scratch, meta[0], meta[1], meta[2], max(lens[:B], default=0), seg, R,
+                                       c.n_heads, c.intermediate, norm_folded=getattr(e.w, "fold_norms", False), deq_scratch=self._deq)
+        for r, lo, n in segs:
+            r.prefilled = lo + n
+        for r in comp:
+            self._prefilling.remove(r)
+            r._x = None
+            if r.kind == "beam" and len(r.slots) > 1:   # the prompt rows from the last shared page on, into the other beams' pages
+                ops.copy_page_rows(self._cache, self._page_table, [(r.slots[0], s, r._shared * PAGE_ROWS, r.prompt_len) for s in r.slots[1:]])
+        if not pick:
+            self.steps += 1
+            self.last_logits = None
+            return done
+        hn = ops.rmsnorm(ops.gather_rows(up[:q].view(torch.int64), x) if nb else x[:B], e.w.final_norm, c.rms_eps)
+        logits = ops.gemm(hn, e.w.lm_head, out_dtype=torch.float32)
+        groups = {}
+        for r in beams:
+            groups.setdefault((r.beam.k, r.beam.k), []).append(r)
+        for r in cb:
+            groups.setdefault((r.beam.k, 1), []).append(r)
+        order = [r for r, _, _, _ in rows[:G0]] + cg + [r for r, _, _, _ in rows[G0:G0 + S0]] + cs + [r for r, _, _, _ in rows[G0 + S0:]] + cb
+        return self._finish_step(done, logits, greedy + cg, sampled + cs, groups, shift, order, B)
+
+    def _finish_step(self, done, logits, greedy, sampled, groups, first, order, B):
+        """the selections of a step's logits rows (greedy rows, then sampled ones, then every beam group's rows), its one
+        device-to-host copy, and the requests' advance -> done"""
+        e = self.engine
+        G, S = len(greedy), len(sampled)
+        sel = torch.empty((G + S + sum(3 * len(g) * 2 * k for (k, _), g in groups.items()),), dtype=torch.int32, device=e.dev)
         if G:
             ops.argmax_rows(logits[:G], out=sel[:G])
-        if S or beams:
+        if S or groups:
             self._select(logits, G, sampled, groups, first, sel)
         h = sel.cpu()                                    # the one device-to-host copy of the step
-        self.last_logits = ([r for r, _, _, _ in rows], logits)
+        self.last_logits = (order, logits)
         self.steps += 1
         self.occupied += B
         for r, t in zip(greedy + sampled, h[:G + S].tolist()):
@@ -873,7 +1001,7 @@ class DecodeStream:
                 self._release(r)
                 done.append((r, r.tokens))
         off, quads = G + S, []
-        for k, g in groups.items():
+        for (k, _), g in groups.items():
             R = len(g)
             cand = h[off:off + 3 * R * 2 * k].view(3, R, 2 * k)
             off += 3 * R * 2 * k
@@ -897,7 +1025,7 @@ class DecodeStream:
         rows [G, G + S), then one candidate launch per beam width k (first: each beam request's first logits row); their
         settings travel in one host-to-device copy"""
         e, S = self.engine, len(sampled)
-        nb = sum(len(g) * k for k, g in groups.items())
+        nb = sum(len(g) * kin for (k, kin), g in groups.items())
         host = np.empty(6 * S + 2 * nb, dtype=np.int32)                       # seeds (int64) first, so their view is aligned
         host[:2 * S].view(np.int64)[:] = [_signed64(r.seed) for r in sampled]
         host[2 * S:3 * S].view(np.float32)[:] = [r.temperature for r in sampled]
@@ -905,10 +1033,11 @@ class DecodeStream:
         host[4 * S:5 * S].view(np.float32)[:] = [1.0 if r.top_p is None else r.top_p for r in sampled]
         host[5 * S:6 * S] = [len(r.tokens) for r in sampled]                  # token t is drawn at step t
         o, spans = 6 * S, []
-        for k, g in groups.items():
-            n = len(g) * k
-            host[o:o + n] = [first[r.id] + b for r in g for b in range(k)]   # each request's beams, in beam order
-            host[o + n:o + 2 * n].view(np.float32)[:] = [s for r in g for s in r.beam.scores]
+        for (k, kin), g in groups.items():
+            n = len(g) * kin
+            host[o:o + n] = [first[r.id] + b for r in g for b in range(kin)]   # each request's beams, in beam order
+            # kin = 1: a prompt completed in this step, its first candidates from one row of score 0
+            host[o + n:o + 2 * n].view(np.float32)[:] = [s for r in g for s in (r.beam.scores if kin == k else [0.0])]
             spans.append((k, len(g), o, n))
             o += 2 * n
         dev = torch.from_numpy(host).to(e.dev)
@@ -918,7 +1047,7 @@ class DecodeStream:
                                 out=sel[G:G + S])
         off = G + S
         for k, R, o, n in spans:
-            ops.beam_candidates(logits, dev[o:o + n].view(R, k), dev[o + n:o + 2 * n].view(torch.float32).view(R, k), k, e.dtype,
+            ops.beam_candidates(logits, dev[o:o + n].view(R, n // R), dev[o + n:o + 2 * n].view(torch.float32).view(R, n // R), k, e.dtype,
                                 out=sel[off:off + 3 * R * 2 * k].view(3, R, 2 * k))
             off += 3 * R * 2 * k
 
@@ -951,6 +1080,7 @@ class DecodeStream:
         pool, and a growing stream's swap area is freed)"""
         self._cache = self._scratch = self._deq = self._page_table = self._swap = None
         self._preempted = {}
+        self._prefilling = []
         if self.pages is not None:
             self.pages.release_all()
         self._slots = [None] * self.max_slots
@@ -1282,7 +1412,7 @@ class VQA_LLM:
 
     @torch.inference_mode()
     def free_form_inference_stream(self, items, max_new_tokens=200, slots=16, temperature=0, top_p=None, num_beams=1, kv_pages=None,
-                                   kv_swap_pages=None):
+                                   kv_swap_pages=None, prefill_chunk=None):
         """free_form_inference for many items on one decode stream (VQAEngine.decode_stream): items are (image, question,
         object_crops, images_long, objects_long); yields (index, text) as each answer completes, with the prompt, stop string
         and post-processing of free_form_inference.  The next item is admitted whenever a slot frees, so up to `slots` answers
@@ -1295,11 +1425,14 @@ class VQA_LLM:
         kv_pages = N: a paged stream (VQAEngine.decode_stream) whose pool of N pages holds the KV rows; an item is then
         admitted when its slots and the pages it reserves are free, and `slots` bounds the answers decoding at a time.
         kv_swap_pages = M (with kv_pages): a growing paged stream with a host swap area of M pages; an item is then admitted
-        by kv_pages.GrowingPool's rule, taking the pages it writes as it writes them."""
+        by kv_pages.GrowingPool's rule, taking the pages it writes as it writes them.  prefill_chunk = C (with kv_pages): admitted
+        prompts are prefilled C rows per step alongside the running answers (DecodeStream)."""
         reqs = [(self._prompt_ids(question), image, crops, il, ol) for image, question, crops, il, ol in items]
         paged = {} if kv_pages is None else dict(kv_pages=int(kv_pages))
         if kv_swap_pages is not None:
             paged["kv_swap_pages"] = int(kv_swap_pages)
+        if prefill_chunk is not None:
+            paged["prefill_chunk"] = prefill_chunk
         if (temperature is None or not temperature > 0) and num_beams == 1:
             answers = self._decode_stream(reqs, int(max_new_tokens), int(slots), **paged)
         else:
@@ -1318,10 +1451,11 @@ class VQA_LLM:
         top_k, top_p = check_sampling(self.top_k, top_p)
         return [dict(temperature=temperature, top_k=top_k, top_p=top_p, seed=s) for s in draw_seeds(n)]
 
-    def _decode_stream(self, reqs, max_new_tokens, slots, settings=None, kv_pages=None, kv_swap_pages=None):
+    def _decode_stream(self, reqs, max_new_tokens, slots, settings=None, kv_pages=None, kv_swap_pages=None, prefill_chunk=None):
         """(prompt ids, image, object_crops, images_long, objects_long) requests -> (index, new token ids) as each ends, on one
         decode stream with min(slots, len(reqs) * num_beams) slots.  settings: per request, DecodeStream.admit's generation
-        keywords (None: greedy); kv_pages: a paged stream of that many pages; kv_swap_pages: growing, with that swap area"""
+        keywords (None: greedy); kv_pages: a paged stream of that many pages; kv_swap_pages: growing, with that swap area;
+        prefill_chunk: prompts prefilled that many rows per step"""
         if not reqs:
             return
         e = self.engine
@@ -1333,7 +1467,8 @@ class VQA_LLM:
         # generate() reserves min(max_new_tokens, 2048 - T) positions: the same budget here
         budgets = [max(1, min(max_new_tokens, e.MAX_POSITIONS - T)) for T in lens]
         positions = min(e.MAX_POSITIONS, max(T + n for T, n in zip(lens, budgets)))
-        stream = e.decode_stream(min(slots, len(reqs) * need), positions, self.eos, kv_pages=kv_pages, kv_swap_pages=kv_swap_pages)
+        chunk = {} if prefill_chunk is None else dict(prefill_chunk=prefill_chunk)
+        stream = e.decode_stream(min(slots, len(reqs) * need), positions, self.eos, kv_pages=kv_pages, kv_swap_pages=kv_swap_pages, **chunk)
         pages = stream.pages
         if pages is not None and any(pages.need(T, n, need) > pages.n_pages for T, n in zip(lens, budgets)):
             stream.close()
