@@ -5,10 +5,11 @@ missing objects of an image run in lock-step so their crop frontiers share GPU b
 another, vstar_bench_eval.py:208-211).
 
 Open-ended questions (the reference demo's `inference()`, app.py:130-233, below its Gradio UI): answer_open /
-answer_open_many, and the command line `python -m vstar_b200.seal`.
+answer_open_many (three phases) / answer_open_stream (one pipeline), and the command line `python -m vstar_b200.seal`.
 """
 from __future__ import annotations
 
+from collections import deque
 from copy import deepcopy
 
 import numpy as np
@@ -241,6 +242,91 @@ def answer_open_many(vqa_llm, vsm, items, slots=16, searches_in_flight=8, minimu
     return [tuple(o) for o in out]
 
 
+def answer_open_stream(vqa_llm, vsm, items, slots=16, searches_in_flight=8, minimum_size_scale=4.0, minimum_size=224, search_batch=16,
+                       search_kwargs=None, temperature=0, top_p=None, num_beams=1, kv_pages=None, kv_swap_pages=None,
+                       prefill_chunk=None):
+    """answer_open_many as a pipeline in which each question moves through app.py's stages on its own: its missing objects'
+    searches start when its direct answer ends, and its final answer is admitted when its last search ends.  Yields
+    (index, outputs) as each question completes; outputs are answer_open_many's four for that item, made by the same code.
+
+    One host loop drives one answer session (vqa_llm.answer_session: direct and final answers share one decode stream of
+    min(slots, len(items) * num_beams) slots) and one search session (SearchController.session, `searches_in_flight` searches
+    at a time), on the current CUDA stream.  Each pass admits the final answers that are ready, in the order their last search
+    ended, then (when none waits) direct answers in item order, while the session's admission rule allows; runs one decode
+    step if an answer is running; and runs one search step if a search is active or queued.  The keywords are
+    answer_open_many's.  Since the final prompts are not known when the stream opens, it holds engine.MAX_POSITIONS positions
+    per request: a contiguous stream (kv_pages None) takes about 1.6 GB per slot at 7B, kv_pages bounds the pool instead.  A
+    request the pool (or swap area) cannot hold raises ValueError naming its question before any launch for it; the session
+    is closed then, as it is when the caller stops early.
+
+    Sampling (temperature > 0): two seeds per item are drawn from torch's default generator before the first admission, in
+    item order (direct answer, final answer), so torch.manual_seed(s) reproduces a call.  answer_open_many draws the direct
+    answers' seeds and the final answers' seeds in two separate batches, so sampled answers differ between the two."""
+    items = [(image.convert("RGB"), question) for image, question in items]
+    if not items:
+        return
+    n = len(items)
+    settings = None
+    if (temperature is not None and temperature > 0) or num_beams != 1:
+        settings = vqa_llm._stream_settings(2 * n, temperature, top_p, num_beams)
+    bg = tuple(int(x * 255) for x in vqa_llm.image_processor.image_mean)
+    searches = SearchController(vsm, None, search_batch).session(searches_in_flight)
+    answers = vqa_llm.answer_session(OPEN_MAX_NEW_TOKENS, min(slots, n * num_beams), num_beams=num_beams, kv_pages=kv_pages,
+                                     kv_swap_pages=kv_swap_pages, prefill_chunk=prefill_chunk)
+
+    def prompt(i, item):
+        p = answers.request(item)
+        answers.refuse([p], f"the answer to question {i} ({items[i][1]!r})")
+        return p
+
+    def admit(i, p, stage):                 # stage 0: direct answer, 1: final answer
+        answers.admit((i, stage), p, **({} if settings is None else settings[2 * i + stage]))
+
+    try:
+        ready = deque()                     # (index, final prompt) in the order their last search ended
+        searching = {}                      # index -> (missing objects, their search results so far)
+        finishing = {}                      # index -> its first three outputs while its final answer runs
+        nxt, direct, completed = 0, None, 0
+        while completed < n:
+            while ready and answers.fits(ready[0][1]):
+                admit(*ready.popleft(), 1)
+            while not ready and nxt < n:
+                if direct is None:
+                    image, question = items[nxt]
+                    direct = prompt(nxt, (expand2square_center(image, bg)[0], question, None, None, None))
+                if not answers.fits(direct):
+                    break
+                admit(nxt, direct, 0)
+                nxt, direct = nxt + 1, None
+            if answers.busy:
+                for (i, stage), text in answers.step():
+                    missing = parse_missing_objects(text) if stage == 0 else None
+                    if not missing:
+                        completed += 1
+                        yield i, (finishing.pop(i) + (text,) if stage == 1 else (text, None, None, None))
+                        continue
+                    image = items[i][0]
+                    smallest = smallest_size_for(image, minimum_size_scale, minimum_size)
+                    searching[i] = (missing, [None] * len(missing))
+                    for j, name in enumerate(missing):
+                        st = SearchState(image, name, smallest, confidence_low=OPEN_CONFIDENCE_LOW, **(search_kwargs or {}))
+                        st.owner = (i, j)
+                        searches.add(st)
+            if not searches.idle:
+                for st, res in searches.step():
+                    i, j = st.owner
+                    missing, results = searching[i]
+                    results[j] = res
+                    if all(r is not None for r in results):
+                        del searching[i]
+                        image, question = items[i]
+                        req, summary, annotated = open_final_request(vqa_llm, image, question, missing, results)
+                        finishing[i] = (NEED_SEARCH_MSG.format(", ".join(missing)), summary, annotated)
+                        ready.append((i, prompt(i, req)))
+    finally:
+        answers.close()
+
+
 def answer_open(vqa_llm, vsm, image, question, minimum_size_scale=4.0, minimum_size=224, **kw):
     """app.py:130-233 `inference()` below the UI for one PIL image and question -> its four outputs (see answer_open_many)"""
     return answer_open_many(vqa_llm, vsm, [(image, question)], minimum_size_scale=minimum_size_scale, minimum_size=minimum_size, **kw)[0]
@@ -281,6 +367,10 @@ def build_parser():
     p.add_argument("--prefill-chunk", default=None, type=int,
                    help="with --kv-pages: prefill admitted prompts this many rows per decode step, alongside the running answers "
                         "(default: prefill each prompt on its own at admission)")
+    p.add_argument("--pipeline", action="store_true",
+                   help="answer through answer_open_stream: each question's searches start when its direct answer ends and its final "
+                        "answer when its searches end, direct and final answers sharing one decode stream (default: three phases, "
+                        "answer_open_many)")
     return p
 
 
@@ -332,10 +422,15 @@ def main(argv=None, vqa_llm=None, vsm=None):
         vsm_args.version = args.vsm_model_path
         vsm = VSM(vsm_args)
     items = [(Image.open(p).convert("RGB"), q) for p, q in questions]
-    answers = answer_open_many(vqa_llm, vsm, items, slots=args.slots, searches_in_flight=args.searches_in_flight,
-                               minimum_size_scale=args.minimum_size_scale, minimum_size=args.minimum_size, search_batch=args.search_batch,
-                               temperature=args.temperature, top_p=args.top_p, num_beams=args.num_beams, kv_pages=args.kv_pages,
-                               kv_swap_pages=args.kv_swap_pages, prefill_chunk=args.prefill_chunk)
+    kw = dict(slots=args.slots, searches_in_flight=args.searches_in_flight, minimum_size_scale=args.minimum_size_scale,
+              minimum_size=args.minimum_size, search_batch=args.search_batch, temperature=args.temperature, top_p=args.top_p,
+              num_beams=args.num_beams, kv_pages=args.kv_pages, kv_swap_pages=args.kv_swap_pages, prefill_chunk=args.prefill_chunk)
+    if args.pipeline:
+        answers = [None] * len(items)
+        for i, out in answer_open_stream(vqa_llm, vsm, items, **kw):
+            answers[i] = out
+    else:
+        answers = answer_open_many(vqa_llm, vsm, items, **kw)
     return write_answers(args.output_path, questions, answers, args.save_images)
 
 

@@ -594,52 +594,16 @@ class SearchController:
         active (None = all at once), and yield (state, result) for each search as soon as it ends.  A finished search frees its
         slot for the next one before the next frontier batch is selected, so batches mix searches at different depths.  The
         controller holds no reference to a yielded state; speculative crops of it that are still in flight are dropped with
-        their batch.  Sets `t_admit` / `t_done` (time.perf_counter) on every state."""
-        import time
-        from collections import deque
-        feed = iter(states)
-        more = True
-        active = []
-        inflight = deque()
-        while True:
-            for st in active:
-                self._advance(st)
-            if any(st.done for st in active):
-                finished = [st for st in active if st.done]
-                active = [st for st in active if not st.done]
-                for st in finished:
-                    st.t_done = time.perf_counter()
-                    yield st, self._finish(st)
-                del finished, st
-            while more and (window is None or len(active) < window):
-                st = next(feed, None)
-                if st is None:
-                    more = False
-                    break
-                st.t_admit = time.perf_counter()
-                active.append(st)
-            if self._serve_cues(active):
-                continue               # replies are in: let the parked commits run on before evaluating more crops
-            if not active:
-                break                  # speculative batches still in flight are simply dropped
-            if not self.pipelined:
-                self._evaluate(self._select(active, self.batch_size))
-                continue
-            while len(inflight) < self.depth:
-                reqs = self._select(active, self.batch_size)
-                if not reqs:
-                    break
-                if not inflight and self.depth > 1 and len(reqs) >= 2 * self.split_min:
-                    # nothing queued behind this batch: cut it in two so that the second half runs on the GPU while the host
-                    # commits the first half and launches its successors
-                    half = (len(reqs) + 1) // 2
-                    inflight.append(self._launch(reqs[:half]))
-                    inflight.append(self._launch(reqs[half:]))
-                else:
-                    inflight.append(self._launch(reqs))
-            if not inflight:
-                raise RuntimeError("search controller stalled: active searches but nothing to evaluate")
-            self._collect(inflight.popleft())
+        their batch.  Sets `t_admit` / `t_done` (time.perf_counter) on every state.  Runs session(window, feed=states) until
+        it is idle."""
+        s = self.session(window, feed=states)
+        while not s.idle:
+            yield from s.step()
+
+    def session(self, window=None, feed=None):
+        """-> a SearchSession on this controller: stream()'s admission, one pass per step(), taking searches from add() (and
+        from the iterable `feed`, pulled one state at a time when there is room) while others run"""
+        return SearchSession(self, window, feed)
 
     @staticmethod
     def _finish(st: SearchState):
@@ -659,6 +623,84 @@ class SearchController:
             if max_logit >= st.confidence_low:
                 ok = True
         return final_step, path_length, ok, st.all_valid_boxes
+
+
+class SearchSession:
+    """Continuous admission into one SearchController, driven one pass at a time, so that searches can be added while others
+    run (SearchController.session).  add(state) queues a search; step() advances every active search, retires the ones that
+    ended, admits queued searches up to `window` active (None = all), then either answers the parked weak-cue calls or launches
+    frontier batches (up to the controller's `depth` in flight) and collects the oldest one, and returns the (state, result)
+    pairs of the searches that ended.  `idle`: nothing active, queued, in flight or left in the feed.  The session holds no
+    reference to a state it has returned; when no search is active, the speculative batches still in flight are dropped."""
+
+    def __init__(self, ctl, window=None, feed=None):
+        from collections import deque
+        self.ctl, self.window = ctl, window
+        self._feed = None if feed is None else iter(feed)
+        self._queue = deque()
+        self._active = []
+        self._inflight = deque()
+
+    def add(self, state):
+        self._queue.append(state)
+
+    @property
+    def idle(self):
+        return not (self._active or self._queue or self._inflight or self._feed is not None)
+
+    def _next(self):
+        if self._queue:
+            return self._queue.popleft()
+        if self._feed is not None:
+            st = next(self._feed, None)
+            if st is not None:
+                return st
+            self._feed = None                        # the feed ran dry: it is not pulled again
+        return None
+
+    def step(self):
+        import time
+        ctl, active = self.ctl, self._active
+        for st in active:
+            ctl._advance(st)
+        done = []
+        if any(st.done for st in active):
+            for st in active:
+                if st.done:
+                    st.t_done = time.perf_counter()
+                    done.append((st, ctl._finish(st)))
+            active = self._active = [st for st in active if not st.done]
+        while self.window is None or len(active) < self.window:
+            st = self._next()
+            if st is None:
+                break
+            st.t_admit = time.perf_counter()
+            active.append(st)
+        if ctl._serve_cues(active):
+            return done                # replies are in: let the parked commits run on before evaluating more crops
+        if not active:
+            self._inflight.clear()     # speculative batches of searches that ended are simply dropped
+            return done
+        if not ctl.pipelined:
+            ctl._evaluate(ctl._select(active, ctl.batch_size))
+            return done
+        inflight = self._inflight
+        while len(inflight) < ctl.depth:
+            reqs = ctl._select(active, ctl.batch_size)
+            if not reqs:
+                break
+            if not inflight and ctl.depth > 1 and len(reqs) >= 2 * ctl.split_min:
+                # nothing queued behind this batch: cut it in two so that the second half runs on the GPU while the host
+                # commits the first half and launches its successors
+                half = (len(reqs) + 1) // 2
+                inflight.append(ctl._launch(reqs[:half]))
+                inflight.append(ctl._launch(reqs[half:]))
+            else:
+                inflight.append(ctl._launch(reqs))
+        if not inflight:
+            raise RuntimeError("search controller stalled: active searches but nothing to evaluate")
+        ctl._collect(inflight.popleft())
+        return done
 
 
 def visual_search(vsm, image, target_object_name, target_bbox, smallest_size, confidence_high=0.5, confidence_low=0.3,

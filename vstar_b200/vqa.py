@@ -23,6 +23,8 @@ DecodeStream.admit takes the same settings per request, so one decode stream mix
 """
 from __future__ import annotations
 
+from collections import namedtuple
+
 import numpy as np
 import torch
 
@@ -1453,63 +1455,47 @@ class VQA_LLM:
 
     def _decode_stream(self, reqs, max_new_tokens, slots, settings=None, kv_pages=None, kv_swap_pages=None, prefill_chunk=None):
         """(prompt ids, image, object_crops, images_long, objects_long) requests -> (index, new token ids) as each ends, on one
-        decode stream with min(slots, len(reqs) * num_beams) slots.  settings: per request, DecodeStream.admit's generation
-        keywords (None: greedy); kv_pages: a paged stream of that many pages; kv_swap_pages: growing, with that swap area;
-        prefill_chunk: prompts prefilled that many rows per step"""
+        AnswerSession with min(slots, len(reqs) * num_beams) slots and the positions of the call's largest request, admitting
+        the requests in order.  settings: per request, DecodeStream.admit's generation keywords (None: greedy); kv_pages: a paged
+        stream of that many pages; kv_swap_pages: growing, with that swap area; prefill_chunk: prompts prefilled that many rows
+        per step"""
         if not reqs:
             return
-        e = self.engine
-        kw = self._stop_ids()
         need = settings[0].get("num_beams", 1) if settings else 1
-        if need > slots:
-            raise ValueError(f"num_beams = {need} needs {need} slots, got slots = {slots}")
-        lens = [e.spliced_length(ids, 0 if crops is None else len(crops), il, ol) for ids, _, crops, il, ol in reqs]
-        # generate() reserves min(max_new_tokens, 2048 - T) positions: the same budget here
-        budgets = [max(1, min(max_new_tokens, e.MAX_POSITIONS - T)) for T in lens]
-        positions = min(e.MAX_POSITIONS, max(T + n for T, n in zip(lens, budgets)))
-        chunk = {} if prefill_chunk is None else dict(prefill_chunk=prefill_chunk)
-        stream = e.decode_stream(min(slots, len(reqs) * need), positions, self.eos, kv_pages=kv_pages, kv_swap_pages=kv_swap_pages, **chunk)
-        pages = stream.pages
-        if pages is not None and any(pages.need(T, n, need) > pages.n_pages for T, n in zip(lens, budgets)):
-            stream.close()
-            raise ValueError(f"kv_pages = {kv_pages} cannot hold the largest request of this call")
-        if stream.growing and any(pages.need(T, n, need) > pages.swap_pages for T, n in zip(lens, budgets)):
-            stream.close()
-            raise ValueError(f"kv_swap_pages = {kv_swap_pages} cannot hold the largest request of this call")
+        prompts = [AnswerSession.prompt(self.engine, r, max_new_tokens) for r in reqs]
+        positions = min(self.engine.MAX_POSITIONS, max(p.length + p.budget for p in prompts))
+        session = self.answer_session(max_new_tokens, min(slots, len(reqs) * need), positions, num_beams=need, kv_pages=kv_pages,
+                                      kv_swap_pages=kv_swap_pages, prefill_chunk=prefill_chunk)
+        nxt = 0
 
-        def fits():                                      # the next request's slots and pages are free
-            rows = stream.free_rows(need)
-            if rows is None:
-                return False
-            if stream.growing:
-                return pages.can_admit(rows, lens[nxt], budgets[nxt])
-            return pages is None or pages.need(lens[nxt], budgets[nxt], need) <= pages.free_pages
-
-        try:
-            index = {}
-            nxt = 0
-
-            def admit():
-                nonlocal nxt
-                ids, image, crops, il, ol = reqs[nxt]
-                img, crops = self._pixels(image, crops)
-                gen = {} if settings is None else settings[nxt]
-                # beam hypotheses end at eos alone, as in free_form_inference(num_beams > 1)
-                stop = None if need > 1 else kw
-                index[stream.admit((ids, img, crops, il, ol), budgets[nxt], stop_ids=stop, **gen).id] = nxt
+        def admit():
+            nonlocal nxt
+            while nxt < len(reqs) and session.fits(prompts[nxt]):
+                session.admit(nxt, prompts[nxt], **({} if settings is None else settings[nxt]))
                 nxt += 1
 
-            while nxt < len(reqs) and fits():
-                admit()
+        try:
+            session.refuse(prompts, "the largest request of this call")
+            admit()
             remaining = len(reqs)
             while remaining:
-                for r, out in stream.step():
+                for i, out in session.step_tokens():
                     remaining -= 1
-                    yield index[r.id], out
-                while nxt < len(reqs) and fits():
-                    admit()
+                    yield i, out
+                admit()
         finally:
-            stream.close()
+            session.close()
+
+    def answer_session(self, max_new_tokens, slots, max_positions=None, num_beams=1, kv_pages=None, kv_swap_pages=None,
+                       prefill_chunk=None):
+        """-> an AnswerSession: free_form_inference's answers on one decode stream of `slots` slots and `max_positions` positions
+        per request (None: engine.MAX_POSITIONS), which takes requests while it runs.  A contiguous stream (kv_pages None) holds
+        slots * max_positions KV rows whatever its requests need: at max_positions = engine.MAX_POSITIONS (2048) that is about
+        1.6 GB per slot at 7B in bf16 or fp16 (32 layers * 2048 rows * 3 * 4096 values), so a long-lived session wants kv_pages,
+        whose pool is what it says.  kv_swap_pages / prefill_chunk as in free_form_inference_stream; num_beams: the beams of
+        every request"""
+        return AnswerSession(self, max_new_tokens, slots, self.engine.MAX_POSITIONS if max_positions is None else max_positions,
+                             num_beams, kv_pages, kv_swap_pages, prefill_chunk)
 
     def _choice_item(self, image, question, options, object_crops, images_long, objects_long):
         qs = DEFAULT_IMAGE_TOKEN + "\n" + question
@@ -1532,3 +1518,78 @@ class VQA_LLM:
         Not in the reference (one sample at a time, vstar_bench_eval.py:257): same per-sample result, batched execution."""
         items = [self._choice_item(*r) for r in requests]
         return [c for _, c in self.engine.option_losses_batch(items)]
+
+
+class AnswerSession:
+    """free_form_inference's answers on one decode stream that takes requests while it runs (VQA_LLM.answer_session): the
+    admission rule, per-request budget, stop ids and text post-processing that free_form_inference_stream and
+    seal.answer_open_stream share.  A request is a `prompt` (its ids, pixels, spliced length and budget); fits(p) says whether
+    its slots and pages are free now, admit(key, p, **settings) starts it (DecodeStream.admit's generation keywords), and
+    step() runs one decode step -> [(key, answer text)] of the requests that ended (step_tokens: their new token ids).
+    `busy` while an admitted request has not been returned; close() frees the stream."""
+
+    Prompt = namedtuple("Prompt", "ids image object_crops images_long objects_long length budget")
+
+    @staticmethod
+    def prompt(engine, request, max_new_tokens):
+        """(prompt ids, image, object_crops, images_long, objects_long) -> Prompt with the spliced length T and generate()'s
+        budget min(max_new_tokens, 2048 - T) new tokens"""
+        ids, image, crops, il, ol = request
+        T = engine.spliced_length(ids, 0 if crops is None else len(crops), il, ol)
+        return AnswerSession.Prompt(ids, image, crops, il, ol, T, max(1, min(max_new_tokens, engine.MAX_POSITIONS - T)))
+
+    def __init__(self, llm, max_new_tokens, slots, max_positions, num_beams=1, kv_pages=None, kv_swap_pages=None, prefill_chunk=None):
+        if num_beams > slots:
+            raise ValueError(f"num_beams = {num_beams} needs {num_beams} slots, got slots = {slots}")
+        self.llm, self.max_new_tokens, self.need = llm, int(max_new_tokens), num_beams
+        self.kv_pages, self.kv_swap_pages = kv_pages, kv_swap_pages
+        chunk = {} if prefill_chunk is None else dict(prefill_chunk=prefill_chunk)
+        self.stream = llm.engine.decode_stream(slots, max_positions, llm.eos, kv_pages=kv_pages, kv_swap_pages=kv_swap_pages, **chunk)
+        # beam hypotheses end at eos alone, as in free_form_inference(num_beams > 1)
+        self.stop_ids = None if num_beams > 1 else llm._stop_ids()
+        self._keys = {}                                  # stream request id -> key, until returned
+
+    def request(self, item):
+        """item (image, question, object_crops, images_long, objects_long) -> its Prompt"""
+        image, question, crops, il, ol = item
+        return self.prompt(self.llm.engine, (self.llm._prompt_ids(question), image, crops, il, ol), self.max_new_tokens)
+
+    def refuse(self, prompts, what):
+        """ValueError naming `what` when the pool, or a growing stream's swap area, cannot hold one of the prompts however
+        empty it is (checked before any launch for them)"""
+        pages = self.stream.pages
+        if pages is None:
+            return
+        if any(pages.need(p.length, p.budget, self.need) > pages.n_pages for p in prompts):
+            raise ValueError(f"kv_pages = {self.kv_pages} cannot hold {what}")
+        if self.stream.growing and any(pages.need(p.length, p.budget, self.need) > pages.swap_pages for p in prompts):
+            raise ValueError(f"kv_swap_pages = {self.kv_swap_pages} cannot hold {what}")
+
+    def fits(self, p):
+        """whether p's slots and pages are free now (a growing stream: kv_pages.GrowingPool's admission rule)"""
+        stream, pages = self.stream, self.stream.pages
+        rows = stream.free_rows(self.need)
+        if rows is None:
+            return False
+        if stream.growing:
+            return pages.can_admit(rows, p.length, p.budget)
+        return pages is None or pages.need(p.length, p.budget, self.need) <= pages.free_pages
+
+    def admit(self, key, p, **settings):
+        img, crops = self.llm._pixels(p.image, p.object_crops)
+        r = self.stream.admit((p.ids, img, crops, p.images_long, p.objects_long), p.budget, stop_ids=self.stop_ids, **settings)
+        self._keys[r.id] = key
+
+    @property
+    def busy(self):
+        return bool(self._keys)
+
+    def step_tokens(self):
+        return [(self._keys.pop(r.id), out) for r, out in self.stream.step()]
+
+    def step(self):
+        return [(key, self.llm._answer_text(out)) for key, out in self.step_tokens()]
+
+    def close(self):
+        self.stream.close()
+        self._keys = {}
